@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- pair-solves/sec of the focal-pair Laplacian solve loop on B200.
+"""bench.py -- pair-solves/sec of the focal-pair Laplacian solve loop on H100.
 
 Contract (one JSON line on stdout from rank 0):
   python bench.py --gpus N --steps K --warmup W            (N>1 under torchrun)
@@ -27,6 +27,10 @@ cholesky factor" / "construct preconditioner" is likewise once per component, sr
                an instrumented repeat of one step; `spmv_1e7` = the SpMV / SpMM micro-benchmark
   cpu_baseline the oracle's CG+AMG port on the host cores, one pair per core, bounded sample
   parity       max relative deviation of R from the oracle's CG+AMG run to rtol 1e-10
+
+`--dump-outputs DIR` writes what the timed path returned in its last step (resistances, iteration
+counts, relative residuals, cumulative / max node-current maps) as DIR/<name>.npy, so that two builds
+can be compared output for output on the same seeded inputs.
 """
 import argparse
 import json
@@ -74,7 +78,13 @@ def parse():
     ap.add_argument("--cpu-sample", type=int, default=16, help="pairs per CPU step (one per core)")
     ap.add_argument("--ref-budget-s", type=float, default=330.0,
                     help="--impl reference: wall budget of the timed steps")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="write the outputs of the last timed step to DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1:
+        ap.error("--steps must be >= 1")
+    if a.dump_outputs and a.impl == "reference":
+        ap.error("--dump-outputs writes the outputs of the CUDA path; --impl reference has none")
     c = CONFIGS[a.config]
     a.rows = a.rows or c["rows"]
     a.cols = a.cols or c["cols"]
@@ -87,7 +97,7 @@ def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.isfile(p):
         return json.load(open(p))["hbm_gbs"], "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def b_spmm(n, nnz, k, sv):
@@ -234,7 +244,7 @@ def config_dict(args, L, npairs, world):
            else f"{args.pairs} focal pairs per GPU")
     ws_gb = (L.nnz * 12 + L.nnz * 6 + 10 * n * 8 * 8) / 1e9      # CSR + fp32 operator copy + ~10 fp64 k = 8 panels
     l2 = (f"working set per iteration (operator {L.nnz * 12 / 1e9:.2f} GB + its fp32 copy + panels, ~{ws_gb:.1f} GB) "
-          + ("exceeds the 126 MB L2" if ws_gb > 0.126 else "FITS the 126 MB L2: not an HBM measurement"))
+          + ("exceeds the 50 MB L2" if ws_gb > 0.05 else "FITS the 50 MB L2: not an HBM measurement"))
     return {"workload": f"{name}: {args.rows}x{args.cols} synthetic raster (R~U[1,10] seed 42), 8-neighbour "
                         f"avg-conductance, {per}, {args.precision}",
             "n": int(L.shape[0]), "nnz": int(L.nnz), "pairs_total": int(npairs), "rtol": args.rtol,
@@ -309,6 +319,29 @@ def cpu_direct_leg(rows=1000, cols=1000, npairs=10):
             "factor_s": tf, "solve_s": tsv, "pairs": len(src),
             "pair_solves_per_s_incl_factor": len(src) / (tf + tsv),
             "pair_solves_per_s_excl_factor": len(src) / tsv, "R": [float(x) for x in Rd]}, (L, src, dst)
+
+
+DUMP_ROWS = 1 << 20
+
+
+def dump_outputs(path, R, iters, relres, factor):
+    """The last timed step as a caller receives it: R, the iteration counts and the relative
+    residuals of every pair of the job (in pair order, whatever the number of GPUs), and the
+    cumulative / max node-current maps.  Maps longer than DUMP_ROWS are cut to a fixed seeded
+    sample of rows (listed in current_rows.npy), which keeps the files of the 10^7-node workload
+    at 24 MB."""
+    os.makedirs(path, exist_ok=True)
+    cum, mx = factor.read_currents()
+    arrays = {"R": np.asarray(R, dtype=np.float64), "iters": np.asarray(iters, dtype=np.float64),
+              "relres": np.asarray(relres, dtype=np.float64)}
+    rows = np.arange(len(cum))
+    if len(cum) > DUMP_ROWS:
+        rows = np.sort(np.random.default_rng(0).choice(len(cum), DUMP_ROWS, replace=False))
+        arrays["current_rows"] = rows.astype(np.float64)
+    arrays["cum_current"] = cum[rows].astype(np.float64)
+    arrays["max_current"] = mx[rows].astype(np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(path, name + ".npy"), a)
 
 
 # ---------------------------------------------------------------------------
@@ -430,6 +463,13 @@ def main():
     clocks = sampler.stop() if sampler else None
     R, out, st = res[-1]
     launches = sum(r[2]["kernel_launches"] for r in res)
+    if args.dump_outputs:                                # before any later leg resets the current maps
+        d_iters, d_relres = out["iters"], out["relres"]
+        if distributed:                                  # collectives: every rank takes part
+            d_iters = comm.gather_pairs(mine, out["iters"], npairs)
+            d_relres = comm.gather_pairs(mine, out["relres"], npairs)
+        if rank == 0:
+            dump_outputs(args.dump_outputs, R, d_iters, d_relres, factor)
     iters = out["iters"]
     value = npairs * args.steps / (ms / 1e3)
     it_all = None
@@ -497,14 +537,6 @@ def main():
         pms, pl = factor.profile_spmm(False)
         avg_bytes = pbytes / max(pl, 1)
         achieved = pbytes / (pms * 1e-3) / 1e9
-        traffic = None
-        tnote = "no ncu --set full capture for this size"
-        tpath = os.path.join(ROOT, "profiles", "r2_traffic.json")
-        if os.path.exists(tpath):
-            tj = json.load(open(tpath)).get(f"finest_level_{args.rows}x{args.cols}")
-            if tj:
-                traffic = tj.get("traffic_bytes_per_launch")
-                tnote = tj.get("note", "")
         t_full = time.time()
         factor.reset_currents()
         o2 = factor.solve_pairs(msrc[:kk], mdst[:kk], accumulate=True)
@@ -515,7 +547,7 @@ def main():
                           + " on the finest-level operator, k = 8 panels, every epilogue of the AMG-PCG "
                           "iteration (fp64 CG SpMM / residual gate, fp32 residual + Jacobi sweep of the V-cycle)",
                 "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic, "traffic_note": tnote, "peak_source": peak_src, "launches": int(pl),
+                "peak_source": peak_src, "launches": int(pl),
                 "avg_launch_ms": pms / max(pl, 1), "algorithmic_bytes_per_launch": avg_bytes,
                 "spmm_share_of_step": pms / max(t_full, 1e-9),
                 "by_kernel": {k: {"launches": c, "avg_ms": m / c, "GB/s": b / (m * 1e-3) / 1e9, "frac": b / (m * 1e-3) / 1e9 / peak}

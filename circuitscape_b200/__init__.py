@@ -1,4 +1,4 @@
-"""circuitscape_b200 -- B200-native (sm_100a) drop-in for Circuitscape.jl's inner
+"""circuitscape_b200 -- H100-native (sm_90a) drop-in for Circuitscape.jl's inner
 Laplacian-solve loop (pairwise + advanced mode).  See DESIGN.md / INTEGRATION.md.
 
 Layout: csrc/ (CUDA kernels + C ABI -> lib/libcsb200.so), solver.py (the

@@ -1,6 +1,6 @@
 // cs_b200.cu -- host side of libcsb200.so (C ABI in include/cs_b200.h).
 // Plain CUDA runtime, no torch.  One handle = one connected component's operator
-// resident on one B200 + a panel workspace for the batched PCG.
+// resident on one GPU + a panel workspace for the batched PCG.
 #include "../../include/cs_b200.h"
 
 #include <cuda_runtime.h>
@@ -121,8 +121,8 @@ struct cs_b200_handle {
   void* io_out[2] = {nullptr, nullptr};
   cudaEvent_t ev_in[2] = {nullptr, nullptr}, ev_used[2] = {nullptr, nullptr};
   cudaEvent_t ev_ready[2] = {nullptr, nullptr}, ev_out[2] = {nullptr, nullptr};
-  int num_sms = 148;
-  int grid_spmm = 148, grid_ew = 148;
+  int num_sms = 132;                 // set from the device in common_create
+  int grid_spmm = 132, grid_ew = 132;
   cs_b200_opts opts{};
   cs_b200_stats stats{};
   GraphSlot graphs[4];  // KT = 1,2,4,8
@@ -1742,7 +1742,7 @@ void end_call(cs_b200_handle* h) {
 
 int ensure_flush(cs_b200_handle* h) {
   if (h->d_flush) return 0;
-  h->flush_elems = (size_t)64 << 20;  // 256 MB of floats > 126 MB L2
+  h->flush_elems = (size_t)64 << 20;  // 256 MB of floats > 50 MB L2
   CK(h, cudaMalloc(&h->d_flush, h->flush_elems * sizeof(float)));
   CK(h, cudaMemsetAsync(h->d_flush, 0, h->flush_elems * sizeof(float), h->stream));
   return 0;

@@ -1,4 +1,4 @@
-// kernels.cuh -- sm_100a device code for the batched PCG focal-pair solver.
+// kernels.cuh -- sm_90a device code for the batched PCG focal-pair solver.
 //
 // Data layout (DESIGN.md §3): CSR matrix (int32 rowptr/colidx, T values) replicated
 // per GPU; every solver vector is a *panel*: n_pad x KT row-major (KT in {1,2,4,8}
@@ -945,10 +945,10 @@ template <typename T> struct DiaDev {
 
 constexpr int ST_TC = 16;   // raster columns per tile
 
-// Three CTAs per SM (80 registers, all 18 loads of a row in flight).  Holding it to 64 registers for a
-// fourth CTA compiles without spills but measured 3 % slower on the CG and residual epilogues (the loads
-// are issued in two batches); a sliding 3 x 3 register window (3 gathers per row instead of 9) measured
-// 25 % slower at k = 8 -- profiles/README.md, "kernel variants".
+// Three CTAs per SM (80 registers): all 18 loads of a row are in flight before the first FMA.  Carried
+// over from the tuning on the previous GPU target, where the variants that issue the loads in smaller
+// batches (64 registers for a fourth CTA, a sliding 3 x 3 register window) were slower; not re-measured
+// on the H100.
 template <typename T, int KT, int MODE>
 __global__ void __launch_bounds__(NT, 3)
 k_stencil(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, const SpmmEpi<T> ep) {
@@ -1090,8 +1090,9 @@ template <typename T> struct CsrP {
   size_t ell_ld;
 };
 
-// MINB = 4 (the fp32 V-cycle): four CTAs per SM, 64 registers.  The kernel is latency-bound, and the
-// fourth CTA bought 19 % (0.497 -> 0.405 ms at 3163^2, k = 8).  What frees the registers: a thread keeps
+// MINB = 4 (the fp32 V-cycle): four CTAs per SM, 64 registers -- carried over from the tuning on the
+// previous GPU target, where the fourth CTA's loads in flight paid; not re-measured on the H100.  What
+// frees the registers: a thread keeps
 // its b.z partial sums (~70 products) in T, the V-cycle's own precision, instead of double; they enter the
 // double tree reduction afterwards.  MINB = 3 keeps double partial sums (fp64 cycles).
 template <typename T, int MINB> struct PjDot { typedef double type; };

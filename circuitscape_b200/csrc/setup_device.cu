@@ -28,6 +28,9 @@ namespace csb_dev {
 namespace {
 
 constexpr int TPB = 256;
+// Grid caps are multiples of the H100's 132 SMs.  Fixed rather than queried: the power iteration
+// combines one partial per CTA, so a fixed grid keeps the setup bit-reproducible on any device.
+constexpr int SMS = 132;
 
 #define CKD(call)                                                                                   \
   do {                                                                                              \
@@ -39,7 +42,7 @@ constexpr int TPB = 256;
     }                                                                                               \
   } while (0)
 
-inline int grid_for(int64_t n, int cap = 148 * 32) {
+inline int grid_for(int64_t n, int cap = SMS * 32) {
   return (int)std::max<int64_t>(1, std::min<int64_t>((n + TPB - 1) / TPB, cap));
 }
 
@@ -486,7 +489,7 @@ int transpose(cudaStream_t s, const DCsr& P, DCsr& R, std::string& err) {
 // [0.7, 1] x ||D^-1 A||_inf  (amg_host.hpp diag_and_rho)
 int diag_and_rho(cudaStream_t s, const DCsr& A, double* dinv, double* rho, std::string& err) {
   const int n = (int)A.nrows;
-  const int g = grid_for(n, 148 * 8);
+  const int g = grid_for(n, SMS * 8);
   Scratch<double> u, y, part, scal;
   Scratch<unsigned long long> rbits;
   CKD(u.alloc((size_t)n, s));
@@ -1052,7 +1055,7 @@ int build_windowed(cudaStream_t s, const int* d_rowptr, const int* d_colidx, con
   cudaError_t e = cudaMalloc(&blob, blob_bytes);
   if (e != cudaSuccess) { cudaFree(meta); err = std::string("CUDA error ") + cudaGetErrorString(e) + " allocating the window records"; return -2; }
   cudaMemsetAsync(blob, 0, blob_bytes, s);
-  k_win_build<T><<<std::max(1, std::min(nb, 148 * 16)), WB_T, 0, s>>>(nb, d_bstart, d_rowptr, d_colidx, d_vals, d_dinv,
+  k_win_build<T><<<std::max(1, std::min(nb, SMS * 16)), WB_T, 0, s>>>(nb, d_bstart, d_rowptr, d_colidx, d_vals, d_dinv,
                                                                       (long long)ncols_pad, wcap, off.p, meta, blob, nwin.p);
   int hw = 0;
   e = cudaGetLastError();

@@ -74,7 +74,7 @@ class SolverResidualError(RuntimeError):
 
 
 class B200Factor:
-    """Opaque factor: CSR + preconditioner resident on one B200 (cs_b200_create)."""
+    """Opaque factor: CSR + preconditioner resident on one GPU (cs_b200_create)."""
 
     def __init__(self, matrix, solver: CUDASolver, log_transform=False):
         lib = _lib.load()

@@ -1,5 +1,5 @@
 /*
- * cs_b200.h -- C ABI of libcsb200.so: a B200-native (sm_100a) replacement for the
+ * cs_b200.h -- C ABI of libcsb200.so: an H100-native (sm_90a) replacement for the
  * inner Laplacian-solve loop of Circuitscape.jl (pairwise + advanced mode).
  *
  * This is the drop-in boundary.  The reference (Julia) reaches a solver through

@@ -1,13 +1,14 @@
 #!/usr/bin/env python
 """Windowed vs plain SpMM on the (square-padded) SA prolongator of a raster (debug aid)."""
-import os, sys, ctypes as C, subprocess
+import os, sys, ctypes as C, subprocess, tempfile
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, "tests"))
 import numpy as np, scipy.sparse as sp
 import circuitscape_b200 as cb
 from circuitscape_b200 import graph
-subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-o", "/tmp/libamgh.so", os.path.join(ROOT, "tests", "amg_host_harness.cpp")])
-lib = C.CDLL("/tmp/libamgh.so")
+SO = os.path.join(tempfile.mkdtemp(), "libamgh.so")
+subprocess.check_call(["g++", "-O2", "-std=c++17", "-shared", "-fPIC", "-o", SO, os.path.join(ROOT, "tests", "amg_host_harness.cpp")])
+lib = C.CDLL(SO)
 import test_amg_host as t
 lib.amgh_build.restype = C.c_void_p; lib.amgh_build.argtypes = [C.c_long, C.c_long, C.c_void_p, C.c_void_p, C.c_void_p]
 lib.amgh_nlevels.argtypes = [C.c_void_p]; lib.amgh_dims.argtypes = [C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 4

@@ -1,5 +1,5 @@
-// alloc_probe.cu -- what do the allocation calls of the device-side setup cost on this box?
-// nvcc -O2 -arch=sm_100a -o alloc_probe alloc_probe.cu ; ./alloc_probe
+// alloc_probe.cu -- what do the allocation calls of the device-side setup cost on this GPU?
+// nvcc -O2 -arch=sm_90a -o alloc_probe alloc_probe.cu ; ./alloc_probe
 #include <cuda_runtime.h>
 #include <chrono>
 #include <cstdio>

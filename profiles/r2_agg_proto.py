@@ -1,5 +1,7 @@
 import sys, time, numpy as np, scipy.sparse as sp, scipy.sparse.linalg as spla
-sys.path.insert(0,'/root/repo'); sys.path.insert(0,'/root/repo/tests')
+import os
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT); sys.path.insert(0, os.path.join(ROOT, 'tests'))
 from circuitscape_b200 import graph
 
 def hash32(x):

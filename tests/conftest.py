@@ -10,7 +10,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs an H100 (run with -m gpu)")
 
 
 def _cuda_device_present():
@@ -29,7 +29,7 @@ def pytest_collection_modifyitems(config, items):
     B200Unavailable (the product path itself still fails loudly: tests/test_abi.py)."""
     if _cuda_device_present():
         return
-    skip = pytest.mark.skip(reason="no CUDA device: gpu-marked parity tests need a B200 (pytest -m gpu on the GPU box)")
+    skip = pytest.mark.skip(reason="no CUDA device: gpu-marked parity tests need an H100 (pytest -m gpu)")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

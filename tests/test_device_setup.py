@@ -1,7 +1,7 @@
 """Device-side setup (circuitscape_b200/csrc/setup_device.cu) against the round-1 host setup
 (amg_host.hpp / win_host.hpp) and against SciPy: hierarchy operators, Galerkin identities, window
 records on every operator shape, the 1-based Int64 boundary Julia uses, and a non-Python caller.
-Needs a B200: `pytest -m gpu`."""
+Needs an H100: `pytest -m gpu`."""
 import ctypes as C
 import os
 import subprocess

@@ -1,5 +1,5 @@
 """Parity of the CUDA path (through the C ABI) against the CPU oracle and the
-reference's golden vectors.  Needs a B200: `pytest -m gpu`.
+reference's golden vectors.  Needs an H100: `pytest -m gpu`.
 
 Tolerances (fp64): effective resistances 1e-6 relative (BASELINE.json north_star),
 voltages max|dv|/R <= 1e-5, maps sum(d^2) < 1e-6 (test/test_utils.jl:196).

@@ -1,6 +1,6 @@
 """Parity at the sizes BASELINE.json names (round-1 verdict, "parity at scale"): the 10^7-node
 raster against the oracle's CG+AMG run to rtol 1e-10, C3 as written (precision = single, 100 pairs,
-4000 x 4000), C5 (power-law network, all-to-one) against a grounded SciPy solve.  Needs a B200 and
+4000 x 4000), C5 (power-law network, all-to-one) against a grounded SciPy solve.  Needs an H100 and
 a few minutes of host time for the CPU references: `pytest -m gpu`.
 
 Tolerances (SURVEY.md section 8d parity gate): effective resistances 1e-6 relative, voltages
