@@ -69,6 +69,7 @@ _PROTOS = {
     "cs_b200_destroy": (None, [_H]),
     "cs_b200_spmv": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_double)]),
     "cs_b200_spmm": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p]),
+    "cs_b200_apply_precond": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_b200_bench_spmm": (C.c_int, [_H, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_double)]),
     "cs_b200_bench_cg_iter": (C.c_int, [_H, C.c_int, C.c_int, C.POINTER(C.c_double)]),
     "cs_b200_solve_rhs": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_double, C.c_int64,

@@ -731,9 +731,10 @@ int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::
   const bool want_win = h->opts.window >= 0 && (h->opts.window > 0 || h->n >= 20000) && (win_mask() & 1);
   const bool want_amg = h->opts.precond == CS_B200_PRECOND_AMG;
   Tick tick;
-  if (want_win) {
+  // stencil = 1 asks for the stencil form at any size, also where no windows are wanted
+  if (want_win || h->opts.stencil > 0) {
     rc = device_stencil<T>(h, h->A0);
-    if (!rc && !h->A0.dia) rc = device_windows<T>(h, h->A0, h->n_pad, (const T*)h->d_dinv);
+    if (!rc && !h->A0.dia && want_win) rc = device_windows<T>(h, h->A0, h->n_pad, (const T*)h->d_dinv);
     if (rc) { csb_dev::seed_discard(job); return rc; }
     tick(h->A0.dia ? "finest operator: stencil form" : "finest operator: windows");
   }
@@ -1863,10 +1864,41 @@ static void teardown_operators(cs_b200_handle* h) {
   h->mixed = false;
 }
 
+// Z = M^-1 R with the cycle solve_panel launches for its first z (k_set_ctl first, so the last kernel
+// runs cg_after_precond's init branch and leaves |r.z| in ctl->rho0).  r, z: host column-major n x KT.
+template <typename T, int KT>
+int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
+  const size_t bytes = (size_t)h->n * KT * sizeof(T);
+  const size_t nelem = (size_t)h->n_pad * KT;
+  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int g = ew_grid<T, KT>(h);
+  CK(h, cudaMemcpyAsync(h->stage, r, bytes, cudaMemcpyHostToDevice, h->stream));
+  CK(h, cudaMemsetAsync(h->R, 0, nelem * sizeof(T), h->stream));
+  k_cm_to_panel<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->stage, (T*)h->R, KT);
+  k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, 0.0, 0.0, 1, 40);
+  const T* zp = (const T*)h->Z;
+  if (h->mixed) {
+    k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
+    launch_vcycle<T, KT>(h, false);
+    k_convert<float, T><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X);
+    zp = (const T*)h->X;
+  } else {
+    launch_vcycle<T, KT>(h, false);   // uses h->stage as its finest x: staging is done by now
+  }
+  k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, zp, (T*)h->stage, h->d_ctl, 0);
+  CK(h, cudaGetLastError());
+  CK(h, cudaMemcpyAsync(z, h->stage, bytes, cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  if (rz)
+    for (int c = 0; c < KT; ++c) rz[c] = h->h_ctl->rho0[c];
+  return CS_B200_OK;
+}
+
 
 extern "C" {
 
-int cs_b200_version(void) { return 1001; }
+int cs_b200_version(void) { return 1002; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2439,6 +2471,18 @@ int cs_b200_spmm(cs_b200_handle* h, int k, const void* x, void* y) {
   CK(h, cudaStreamSynchronize(h->stream));
   end_call(h);
   return CS_B200_OK;
+}
+
+int cs_b200_apply_precond(cs_b200_handle* h, int k, const void* r, void* z, double* rz) {
+  if (!h || !r || !z || (k != 1 && k != 2 && k != 4 && k != 8) || k > h->ktmax)
+    return set_err(h, CS_B200_ERR_ARG, "bad apply_precond arguments");
+  if (!h->amg) return set_err(h, CS_B200_ERR_UNSUPPORTED, "apply_precond: the handle has no multigrid preconditioner");
+  begin_call(h);
+  int rc = CS_B200_OK;
+  if (h->dtype == CS_B200_F64) { DISPATCH_KT(k, (rc = apply_precond_t<double, KT>(h, r, z, rz))); }
+  else { DISPATCH_KT(k, (rc = apply_precond_t<float, KT>(h, r, z, rz))); }
+  end_call(h);
+  return rc;
 }
 
 int cs_b200_bench_spmm(cs_b200_handle* h, int k, int reps, int flush_l2, double* ms_per_rep) {

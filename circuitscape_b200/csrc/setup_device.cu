@@ -1098,6 +1098,10 @@ __global__ void k_dia_fill(int n, int nr, size_t ld, const int* __restrict__ ptr
       else if (off >= nr - 1 && off <= nr + 1) s = 7 + (off - nr);
       else if (-off >= nr - 1 && -off <= nr + 1) s = 1 + (off + nr);
       if (s < 0) { miss = 1; continue; }
+      // the neighbour must lie in the same or an adjacent raster column: a row offset that leaves
+      // [0, nr) is a wrapped neighbour (NODATA before it shifted the numbering), not a stencil entry
+      const int r = i % nr + s % 3 - 1;
+      if (r < 0 || r >= nr) { miss = 1; continue; }
       const T v = val[j];
 #pragma unroll
       for (int q = 0; q < 9; ++q) if (q == s) d[q] += v;
@@ -1117,6 +1121,10 @@ int build_dia(cudaStream_t s, const int* d_rowptr, const int* d_colidx, const T*
   *nr = 0;
   *ld = 0;
   if (n < 16) return 0;
+  // Invariant of the form: every entry (i, i + dc nr + dr) has (i % nr) + dr in [0, nr), i.e. row i is
+  // raster cell (i % nr, i / nr) and its neighbours are cells of the 3 x 3 block around it.  The
+  // tile-based kernels (k_stencil_prolong_jacobi reads the 9 neighbours from a shared-memory tile by
+  // raster position) rely on it; an operator with a wrapped entry keeps the CSR / windowed path.
   // stride candidate from row 0: its first column beyond 1 (row 0 of a raster has neighbours 1, nr, nr + 1)
   int rp[2] = {0, 0};
   CKD(cudaMemcpyAsync(rp, d_rowptr, 2 * sizeof(int), cudaMemcpyDeviceToHost, s));

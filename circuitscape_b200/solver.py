@@ -288,6 +288,19 @@ class B200Factor:
         _lib.check(self._lib, self._h, rc)
         return Y
 
+    def apply_precond(self, R):
+        """One application of the multigrid preconditioner, Z = M^-1 R, for R (n,) or (n, k),
+        k in {1,2,4,8} (cs_b200_apply_precond).  Returns (Z, rz) with rz[c] = |r_c . z_c| as the
+        cycle's last kernel reduces it."""
+        R = np.asarray(R, dtype=self.dtype)
+        vec = R.ndim == 1
+        X = np.asfortranarray(R.reshape(self.n, -1))
+        Z = np.empty_like(X, order="F")
+        rz = np.zeros(X.shape[1])
+        rc = self._lib.cs_b200_apply_precond(self._h, X.shape[1], _lib._ptr(X), _lib._ptr(Z), _lib._ptr(rz))
+        _lib.check(self._lib, self._h, rc)
+        return (Z[:, 0] if vec else Z), rz
+
     def bench_spmm(self, k, reps=20, flush_l2=False):
         ms = C.c_double()
         rc = self._lib.cs_b200_bench_spmm(self._h, k, reps, 1 if flush_l2 else 0, C.byref(ms))

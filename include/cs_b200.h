@@ -183,6 +183,12 @@ int cs_b200_spmv(cs_b200_handle* h, const void* x, void* y, int reps, double* ms
  * column-major n x k.  Parity hook for the batched kernel at any size.             */
 int cs_b200_spmm(cs_b200_handle* h, int k, const void* x, void* y);
 
+/* Z = M^-1 R for k in {1,2,4,8} columns through ONE application of the multigrid preconditioner --
+ * the V-cycle the solver launches for its first z (in fp32 when the cycle is mixed).  r, z: host,
+ * column-major n x k of the handle's dtype.  rz (k values, may be NULL): |r.z| per column as the
+ * cycle's last kernel reduces it.  CS_B200_ERR_UNSUPPORTED without a hierarchy.  Parity hook.   */
+int cs_b200_apply_precond(cs_b200_handle* h, int k, const void* r, void* z, double* rz);
+
 /* Y = A X for a row-major n x k panel resident on the device (k in 1,2,4,8),
  * timing only -- no host traffic.  flush_l2 != 0 writes a >L2 buffer between reps. */
 int cs_b200_bench_spmm(cs_b200_handle* h, int k, int reps, int flush_l2, double* ms_per_rep);

@@ -11,6 +11,8 @@ import scipy.sparse as sp
 
 from circuitscape_b200 import graph
 
+from .reference_ops import vcycle
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
 
@@ -61,26 +63,6 @@ def build(lib, A):
     return levels, pinv
 
 
-def vcycle(levels, pinv, b, l=0):
-    if l == len(levels) - 1:
-        A = levels[l]["A"]
-        if A.shape[0] <= 320:
-            return pinv @ b
-        # coarsening stopped above the dense limit: 4 damped-Jacobi sweeps (as on the device)
-        dinv = 1.0 / A.diagonal()
-        x = levels[l]["omega"] * dinv * b
-        for _ in range(3):
-            x = x + levels[l]["omega"] * dinv * (b - A @ x)
-        return x
-    L = levels[l]
-    A = L["A"]
-    dinv = 1.0 / A.diagonal()
-    x = L["omega"] * dinv * b
-    r = b - A @ x
-    x = x + L["P"] @ vcycle(levels, pinv, L["R"] @ r, l + 1)
-    return x + L["omega"] * dinv * (b - A @ x)
-
-
 def pcg(A, b, M, rtol=1e-6, itmax=500):
     x = np.zeros_like(b); r = b.copy(); z = M(r); p = z.copy(); g = r @ z
     eps = 1.5e-8 + rtol * np.sqrt(g); it = 0
@@ -117,7 +99,7 @@ def test_hierarchy_and_convergence(harness, kind):
     assert np.abs(Ac @ pinv @ Ac - Ac).max() < 1e-9 * np.abs(Ac).max()
     n = A.shape[0]
     b = np.zeros(n); b[3] = -1.0; b[n - 5] = 1.0
-    x, it = pcg(A, b, lambda r: vcycle(levels, pinv, r))
+    x, it = pcg(A, b, lambda r: vcycle(levels, r, pinv))
     assert it <= 30, it
     assert np.linalg.norm(A @ x - b) / np.sqrt(2) < 1e-4
     import scipy.sparse.linalg as spla
@@ -146,7 +128,7 @@ def test_spd_with_grounds_and_hub(harness):
     for l in range(len(levels) - 1):
         assert levels[l + 1]["A"].nnz <= levels[l]["A"].nnz
     b = rng.standard_normal(n)
-    M_apply = (lambda r: vcycle(levels, pinv, r)) if len(levels) > 1 else (lambda r: r / M.diagonal())
+    M_apply = (lambda r: vcycle(levels, r, pinv)) if len(levels) > 1 else (lambda r: r / M.diagonal())
     x, it = pcg(M, b, M_apply, rtol=1e-8, itmax=2000)
     assert it <= 600, it
     assert np.linalg.norm(M @ x - b) / np.linalg.norm(b) < 1e-6
@@ -226,7 +208,7 @@ def test_random_rasters_give_a_sound_hierarchy(harness, nr, nc, seed, sigma, hol
             Dm = sp.diags(1.0 / np.sqrt(d))
             lam = spla.eigsh((Dm @ L["A"] @ Dm).asfptype(), k=1, which="LA", return_eigenvectors=False, tol=1e-4)[0]
             assert 0 < L["omega"] * lam < 2.0, (L["omega"], lam)
-    M = (lambda r: vcycle(levels, pinv, r)) if len(levels) > 1 else None
+    M = (lambda r: vcycle(levels, r, pinv)) if len(levels) > 1 else None
     if M is not None:
         u, w = rng.standard_normal(n), rng.standard_normal(n)
         if not grounded:

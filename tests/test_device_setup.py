@@ -219,16 +219,12 @@ def test_c_program_links_and_solves(tmp_path):
 
 
 # ---- stencil (DIA) form: SURVEY.md 8f rank 2 ------------------------------------------------------
-@pytest.mark.parametrize("four", [False, True])
-@pytest.mark.parametrize("dtype", [np.float64, np.float32])
-def test_stencil_form_spmm(dtype, four):
-    """Full raster (every cell a node): the operator is stored as 9 diagonals and multiplied by
-    k_stencil; every panel width against SciPy, first / last raster columns and rows included."""
-    A = graph.synthetic_raster_laplacian(233, 171, seed=5, four_neighbors=four)[0].tocsr()
+def _check_stencil_spmm(A, dtype):
     n = A.shape[0]
     prec = "single" if dtype == np.float32 else "double"
     rng = np.random.default_rng(4)
     with cb.B200Factor(A, cb.CUDASolver(precision=prec, f32_compute=True, precond="jacobi", stencil="on")) as f:
+        assert f.operator_form() == "stencil"
         for k in (1, 2, 4, 8):
             X = rng.standard_normal((n, k))
             Y = f.spmm(X)
@@ -237,6 +233,31 @@ def test_stencil_form_spmm(dtype, four):
             assert np.abs(Y - ref).max() <= tol, k
         y, _ = f.spmv(X[:, 0])
         assert np.abs(y - A.astype(dtype) @ X[:, 0].astype(dtype)).max() <= tol
+
+
+@pytest.mark.parametrize("four", [False, True])
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+def test_stencil_form_spmm(dtype, four):
+    """Full raster (every cell a node): the operator is stored as 9 diagonals and multiplied by
+    k_stencil; every panel width against SciPy, first / last raster columns and rows included."""
+    A = graph.synthetic_raster_laplacian(233, 171, seed=5, four_neighbors=four)[0].tocsr()
+    _check_stencil_spmm(A, dtype)
+
+
+@pytest.mark.parametrize("four", [False, True])
+@pytest.mark.parametrize("dtype", [np.float64, np.float32])
+@pytest.mark.parametrize("shape", [(3, 50), (20, 37), (65, 43), (257, 29), "ragged"])
+def test_stencil_form_spmm_tile_edges(shape, dtype, four):
+    """The same below 20 000 rows (stencil = on): rasters shorter than one tile (3, 20 rows), not a
+    multiple of it (65, 257), and a last raster column that ends early (NODATA below row 120: still a
+    stencil form)."""
+    if shape == "ragged":
+        g = 1.0 / np.random.default_rng(5).uniform(1.0, 10.0, size=(301, 97))
+        g[120:, 96] = 0.0
+        A = graph.laplacian(graph.construct_graph(g, graph.construct_node_map(g), False, four))
+    else:
+        A = graph.synthetic_raster_laplacian(*shape, seed=5, four_neighbors=four)[0].tocsr()
+    _check_stencil_spmm(A, dtype)
 
 
 @pytest.mark.parametrize("mixed", [True, False])
