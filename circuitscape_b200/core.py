@@ -19,6 +19,7 @@ from dataclasses import dataclass, field
 import numpy as np
 import scipy.sparse as sp
 
+from . import _lib
 from . import solver as S
 
 NODATA = -9999.0
@@ -594,6 +595,84 @@ def compute_omniscape_current(conductance, source, ground, cs_cfg, solver=None):
                                             np.asarray(ground, dtype=np.float64), nodemap, G.shape[0], "rmvsrc")
     prob = AdvancedProblem(G, cc, s, g, f, nodemap, None, cellmap, solver if solver is not None else get_solver(cs_cfg))
     return advanced_kernel(prob, Flags(is_raster=True, is_advanced=True), cs_cfg).curmap
+
+
+@dataclass
+class OmniscapeBatch:
+    """Result of compute_omniscape_currents, one entry per input window in input order."""
+    currents: list                 # float64 rasters of each window's own shape
+    voltages: list | None          # the same for the voltages (want_voltages=True)
+    iterations: np.ndarray         # CG iterations, summed over the window's solved components
+    relres: np.ndarray             # largest true relative residual of the window's solved components
+
+
+def _windows(a, name):
+    ws = list(a) if isinstance(a, (list, tuple)) or (isinstance(a, np.ndarray) and a.ndim == 3) else None
+    if ws is None:
+        raise ValueError(f"{name}: expected a 3-D stack or a list of 2-D windows")
+    out = []
+    for k, w in enumerate(ws):
+        w = np.asarray(w)
+        if w.ndim != 2 or w.size == 0 or not (np.issubdtype(w.dtype, np.number) or w.dtype == bool):
+            raise ValueError(f"{name}[{k}]: expected a non-empty numeric 2-D window, got shape {w.shape} "
+                             f"dtype {w.dtype}")
+        out.append(w)
+    return out
+
+
+def compute_omniscape_currents(conductances, sources, grounds, cs_cfg, want_voltages=False, solver=None,
+                               max_batch_bytes=1 << 30) -> OmniscapeBatch:
+    """`compute_omniscape_current` for many windows at once: window w of the result is what
+    compute_omniscape_current(conductances[w], sources[w], grounds[w], cs_cfg) returns, computed by
+    cs_b200_solve_advanced_batch (one CTA per window, Jacobi-preconditioned CG per connected
+    component; same rtol / itmax / device and 1e-4 residual gate as the per-window path).
+
+    conductances / sources / grounds: 3-D stacks (nwin, nrows, ncols) or lists of 2-D windows; the
+    three must agree window by window, but windows may differ in shape -- they are padded to a common
+    shape with g = 0 cells (not nodes) and cropped back.  float32 inputs stay float32 on the way in
+    when all three are float32; the device arithmetic and the outputs are float64.
+    Windows go to the device in batches of at most `max_batch_bytes` of device memory (at least one
+    window per batch).  A window whose component fails the gate raises SolverResidualError naming it."""
+    gs, ss, ns = (_windows(a, n) for a, n in ((conductances, "conductances"), (sources, "sources"),
+                                               (grounds, "grounds")))
+    if not len(gs) == len(ss) == len(ns):
+        raise ValueError(f"{len(gs)} conductance, {len(ss)} source and {len(ns)} ground windows")
+    for k, (g, s, n) in enumerate(zip(gs, ss, ns)):
+        if not g.shape == s.shape == n.shape:
+            raise ValueError(f"window {k}: conductance {g.shape}, source {s.shape}, ground {n.shape} differ")
+    if max_batch_bytes <= 0:
+        raise ValueError("max_batch_bytes must be positive")
+    solver = solver if solver is not None else get_solver(cs_cfg)
+    four = _flag(cs_cfg, "connect_four_neighbors_only")
+    nwin = len(gs)
+    dtype = np.float32 if all(a.dtype == np.float32 for a in gs + ss + ns) else np.float64
+    nr = max((g.shape[0] for g in gs), default=1)
+    nc = max((g.shape[1] for g in gs), default=1)
+    # one padded shape for every batch, so a window's result does not depend on the split
+    per = S.advanced_batch_bytes(nr * nc, np.dtype(dtype).itemsize, want_voltages)
+    bw = max(1, int(max_batch_bytes // per))
+    out = OmniscapeBatch([], [] if want_voltages else None, np.zeros(nwin, dtype=np.int64), np.zeros(nwin))
+    for b0 in range(0, nwin, bw):
+        idx = range(b0, min(nwin, b0 + bw))
+        stacks = [np.zeros((len(idx), nr, nc), dtype=dtype) for _ in range(3)]
+        for j, w in enumerate(idx):
+            r, c = gs[w].shape
+            for st, src in zip(stacks, (gs[w], ss[w], ns[w])):
+                st[j, :r, :c] = src
+        res = S.solve_advanced_batch(*stacks, four, solver.device, solver.rtol, solver.itmax, want_voltages)
+        if res["rc"] == _lib.ERR_RESIDUAL:
+            w = b0 + res["first_failed"]
+            err = S.SolverResidualError(res["msg"].replace(f"for window {res['first_failed']} ", f"for window {w} "))
+            err.window = w
+            raise err
+        out.iterations[b0:b0 + len(idx)] = res["iters"]
+        out.relres[b0:b0 + len(idx)] = res["relres"]
+        for j, w in enumerate(idx):
+            r, c = gs[w].shape
+            out.currents.append(np.array(res["cur"][j, :r, :c]))
+            if want_voltages:
+                out.voltages.append(np.array(res["volt"][j, :r, :c]))
+    return out
 
 
 def resolve_conflicts(sources, grounds, policy):

@@ -1,0 +1,475 @@
+// advanced_batch.cu -- many small advanced-mode problems in one launch: the moving-window solve of
+// compute_omniscape_current (src/utils.jl:145-257) for a stack of conductance windows.
+//
+// The handle-based solver keeps one large operator resident and amortises an AMG setup over many
+// right-hand sides; a window is the opposite shape (thousands of independent operators of ~10^4
+// cells, one right-hand side each).  So each window is one CTA that runs the whole advanced-mode
+// kernel (src/raster/advanced.jl:151-305 with the raster branch of src/out.jl:178-207) on its own:
+//   1. valid cells (g > 0; NODATA, 0 and NaN are not nodes), outputs zeroed
+//   2. conflict resolution, policy rmvsrc (src/raster/advanced.jl:119-149)
+//   3. connected-component labels: hooking with atomicMin + pointer jumping; label = smallest cell
+//   4. skip rule (sum(sources) == 0 or sum(grounds) == 0), candidates flagged with integer ops first
+//   5. Jacobi-preconditioned CG per solved component, in order of its smallest cell, with the
+//      Krylov stop rule sqrt(r'z) <= atol + rtol sqrt(r0'z0)
+//   6. true-residual gate ||b - A x|| / ||b|| on the reduced system (Inf grounds deleted)
+//   7. node currents max(inflow, outflow) with the 1e-8 cut relative to the component's maxima
+// The operator is never stored: edge weights come from the conductances through ras::weight and the
+// Dirichlet (Inf-ground) cells are held at 0.  Window data is window-major, column-major inside a
+// window (cell r + c * nrows), so a CTA's passes are coalesced down raster columns.  Every
+// reduction is a fixed-order CTA tree and there are no floating-point atomics, so a window's
+// result depends on its own data and shape only: repeat runs and any split into batches give
+// bit-identical outputs.
+#include "../../include/cs_b200.h"
+
+#include <cuda_runtime.h>
+
+#include <cub/block/block_scan.cuh>
+
+#include <climits>
+#include <cmath>
+#include <cstdarg>
+#include <cstdio>
+#include <vector>
+
+#include "raster_assembly.cuh"
+
+int set_handleless_error(int code, const char* msg);   // cs_b200.cu: the text of cs_b200_last_error(NULL)
+
+namespace {
+
+int set_err(int code, const char* fmt, ...) {
+  char buf[1024];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof buf, fmt, ap);
+  va_end(ap);
+  return set_handleless_error(code, buf);
+}
+
+constexpr int BT = 256;               // threads per window
+constexpr int NWARP = BT / 32;
+constexpr int NVEC = 5;               // x, r, p, q, diag
+constexpr double kNodata = -9999.0;
+constexpr double kCut = 1e-8;         // src/out.jl:281-287
+constexpr double kGate = 1e-4;        // src/core.jl:641
+
+enum WinStatus { WIN_OK = 0, WIN_MAXITER = 1, WIN_RESIDUAL = 2 };
+
+struct WinOut {
+  double relres;         // max over the window's solved components
+  double fail_relres;    // first component that failed the gate (or ran into itmax)
+  long long iters;       // summed over the window's solved components
+  int fail_iters;
+  int status;            // WinStatus
+};
+
+struct Shape {
+  int nrows, ncols, ncell, four;
+};
+
+// visit the valid stencil neighbours of cell i: f(j, diagonal).  Slot k -> (dr, dc) = (k % 3 - 1,
+// k / 3 - 1) as in raster_assembly.cuh, so FORWARD (k > 4) visits exactly the neighbours j > i.
+template <bool FORWARD, typename T, class F>
+__device__ __forceinline__ void for_nbrs(const Shape& s, const T* __restrict__ g, int i, F&& f) {
+  const int r = i % s.nrows, c = i / s.nrows;
+#pragma unroll
+  for (int k = FORWARD ? 5 : 0; k < 9; ++k) {
+    if (k == 4) continue;
+    const int dr = k % 3 - 1, dc = k / 3 - 1;
+    const bool diagonal = dr != 0 && dc != 0;
+    if (s.four && diagonal) continue;
+    const int rr = r + dr, cc = c + dc;
+    if (rr < 0 || rr >= s.nrows || cc < 0 || cc >= s.ncols) continue;
+    const int j = cc * s.nrows + rr;
+    const double gj = (double)g[j];
+    if (gj > 0.0) f(j, gj, diagonal);
+  }
+}
+
+// fixed-order CTA reductions (shuffle tree per warp, then the warps in order); every thread gets the result
+__device__ __forceinline__ double block_sum(double v, double* sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = sh[0];
+    for (int w = 1; w < NWARP; ++w) t += sh[w];
+    sh[NWARP] = t;
+  }
+  __syncthreads();
+  return sh[NWARP];
+}
+
+__device__ __forceinline__ double dmax(double a, double b) { return a > b ? a : b; }
+
+__device__ __forceinline__ double block_max(double v, double* sh) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v = dmax(v, __shfl_down_sync(0xffffffffu, v, o));
+  __syncthreads();
+  if ((threadIdx.x & 31) == 0) sh[threadIdx.x >> 5] = v;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = sh[0];
+    for (int w = 1; w < NWARP; ++w) t = dmax(t, sh[w]);
+    sh[NWARP] = t;
+  }
+  __syncthreads();
+  return sh[NWARP];
+}
+
+__device__ __forceinline__ int find_root(const volatile int* lab, int x) {
+  int p = lab[x];
+  while (p != x) { x = p; p = lab[x]; }
+  return x;
+}
+
+// source of a node after resolve_conflicts(..., "rmvsrc"): dropped where the cell is also grounded
+__device__ __forceinline__ double node_source(double s, double gnd) { return (s != 0.0 && gnd != 0.0) ? 0.0 : s; }
+
+// ground after resolve_conflicts: Inf grounds under a positive source are dropped (a no-op once
+// rmvsrc has zeroed those sources, kept so the rule reads as the reference's)
+__device__ __forceinline__ double node_ground(double s, double gnd) {
+  return (isinf(gnd) && node_source(s, gnd) > 0.0) ? 0.0 : gnd;
+}
+
+// the finite-ground conductance of a node (Inf grounds are Dirichlet nodes, not conductances)
+__device__ __forceinline__ double node_finite(double gnd) { return isfinite(gnd) ? gnd : 0.0; }
+
+__device__ __forceinline__ double cut(double b, double mx) { return fabs(b / mx) < kCut ? 0.0 : b; }
+
+template <typename T>
+__global__ void __launch_bounds__(BT)
+k_advanced_batch(Shape s, const T* __restrict__ g_all, const T* __restrict__ src_all,
+                 const T* __restrict__ gnd_all, double rtol, double atol, long long itmax,
+                 double* __restrict__ cur_all, double* __restrict__ volt_all, double* __restrict__ vec_all,
+                 int* __restrict__ lab_all, int* __restrict__ flag_all, int* __restrict__ list_all,
+                 WinOut* __restrict__ out) {
+  using Scan = cub::BlockScan<int, BT>;
+  __shared__ typename Scan::TempStorage scan_tmp;
+  __shared__ double red[NWARP + 1];
+
+  const int n = s.ncell;
+  const int64_t base = (int64_t)blockIdx.x * n;
+  const T* __restrict__ g = g_all + base;
+  const T* __restrict__ src = src_all + base;
+  const T* __restrict__ gnd = gnd_all + base;
+  double* __restrict__ cur = cur_all + base;
+  double* __restrict__ volt = volt_all ? volt_all + base : nullptr;
+  double* __restrict__ X = vec_all + (int64_t)blockIdx.x * NVEC * n;
+  double* __restrict__ R = X + n;
+  double* __restrict__ P = R + n;
+  double* __restrict__ Q = P + n;
+  double* __restrict__ D = Q + n;      // diagonal of the reduced operator; 0 = not an unknown
+  int* lab = lab_all + base;            // read and hooked concurrently: no __restrict__
+  int* __restrict__ flag = flag_all + base;
+  int* __restrict__ list = list_all + base;
+  volatile int* vlab = lab;
+
+  // 1. valid cells, outputs zeroed
+  for (int i = threadIdx.x; i < n; i += BT) {
+    lab[i] = (double)g[i] > 0.0 ? i : -1;
+    flag[i] = 0;
+    cur[i] = 0.0;
+    if (volt) volt[i] = 0.0;
+  }
+  __syncthreads();
+
+  // 3. component labels.  Hook the larger of two roots under the smaller (labels only decrease and
+  // always point to a smaller cell, so there are no cycles and the final root is the component's
+  // smallest cell), then compress every path; repeat until a pass sees no edge between two trees.
+  for (;;) {
+    int changed = 0;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      if (lab[i] < 0) continue;
+      for_nbrs<true>(s, g, i, [&](int j, double, bool) {
+        const int ri = find_root(vlab, i), rj = find_root(vlab, j);
+        if (ri != rj) {
+          atomicMin(&lab[max(ri, rj)], min(ri, rj));
+          changed = 1;
+        }
+      });
+    }
+    changed = __syncthreads_or(changed);
+    for (int i = threadIdx.x; i < n; i += BT)
+      if (lab[i] >= 0) vlab[i] = find_root(vlab, i);
+    __syncthreads();
+    if (!changed) break;
+  }
+
+  // 2 + 4. after rmvsrc: flag every root whose component has a nonzero source (1) / ground (2)
+  for (int i = threadIdx.x; i < n; i += BT) {
+    const int root = lab[i];
+    if (root < 0) continue;
+    const double si = (double)src[i], gi = (double)gnd[i];
+    int f = 0;
+    if (node_source(si, gi) != 0.0) f |= 1;
+    if (node_ground(si, gi) != 0.0) f |= 2;
+    if (f) atomicOr(&flag[root], f);
+  }
+  __syncthreads();
+
+  // candidate roots in ascending cell order
+  int ncand = 0;
+  for (int b0 = 0; b0 < n; b0 += BT) {
+    const int i = b0 + threadIdx.x;
+    const int is = (i < n && lab[i] == i && flag[i] == 3) ? 1 : 0;
+    int pos, total;
+    Scan(scan_tmp).ExclusiveSum(is, pos, total);
+    if (is) list[ncand + pos] = i;
+    ncand += total;
+    __syncthreads();
+  }
+
+  WinOut wo{0.0, 0.0, 0, 0, WIN_OK};
+  for (int ci = 0; ci < ncand; ++ci) {
+    const int root = list[ci];
+    // 4. the exact rule of src/raster/advanced.jl:194-196 on the component's own sums
+    double ss = 0.0, gs = 0.0;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      if (lab[i] != root) continue;
+      const double si = (double)src[i], gi = (double)gnd[i];
+      ss += node_source(si, gi);
+      gs += node_ground(si, gi);
+    }
+    ss = block_sum(ss, red);
+    gs = block_sum(gs, red);
+    if (ss == 0.0 || gs == 0.0) continue;
+    // multiple_solver adds the finite grounds unless the component's first entry is the NODATA
+    // sentinel (src/raster/advanced.jl:284-285); the first node is the root cell
+    const bool use_fin = node_finite((double)gnd[root]) != kNodata;
+
+    // 5. reduced system: unknowns = the component's cells that are not Inf grounds
+    double rz = 0.0, bb = 0.0;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      double d = 0.0, b = 0.0;
+      const double gi = (double)g[i], grd = (double)gnd[i];
+      if (lab[i] == root && !(grd == INFINITY)) {
+        for_nbrs<false>(s, g, i, [&](int, double gj, bool dg) { d += ras::weight(gi, gj, dg, false); });
+        if (use_fin) d += node_finite(grd);
+        b = node_source((double)src[i], grd);
+      }
+      const double z = d != 0.0 ? b / d : 0.0;
+      D[i] = d;
+      X[i] = 0.0;
+      R[i] = b;
+      P[i] = z;
+      rz += b * z;
+      bb += b * b;
+    }
+    rz = block_sum(rz, red);
+    bb = block_sum(bb, red);
+    const double tol = atol + rtol * sqrt(rz);
+    long long it = 0;
+    bool active = rz > 0.0 && sqrt(rz) > tol && itmax > 0;
+    while (active) {
+      double pq = 0.0;
+      for (int i = threadIdx.x; i < n; i += BT) {
+        const double d = D[i];
+        if (d == 0.0) continue;
+        const double gi = (double)g[i];
+        double q = d * P[i];
+        for_nbrs<false>(s, g, i, [&](int j, double gj, bool dg) { q -= ras::weight(gi, gj, dg, false) * P[j]; });
+        Q[i] = q;
+        pq += P[i] * q;
+      }
+      const double alpha = rz / block_sum(pq, red);
+      double rn = 0.0;
+      for (int i = threadIdx.x; i < n; i += BT) {
+        const double d = D[i];
+        if (d == 0.0) continue;
+        X[i] += alpha * P[i];
+        const double r = R[i] - alpha * Q[i];
+        R[i] = r;
+        rn += r * (r / d);
+      }
+      rn = block_sum(rn, red);
+      ++it;
+      if (!(sqrt(rn) > tol) || it >= itmax) {
+        active = false;
+        rz = rn;
+        break;
+      }
+      const double beta = rn / rz;
+      rz = rn;
+      for (int i = threadIdx.x; i < n; i += BT) {
+        const double d = D[i];
+        if (d != 0.0) P[i] = R[i] / d + beta * P[i];
+      }
+      __syncthreads();
+    }
+
+    // 6. true residual of the reduced system
+    double rr = 0.0;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      const double d = D[i];
+      if (d == 0.0) continue;
+      const double gi = (double)g[i];
+      double ax = d * X[i];
+      for_nbrs<false>(s, g, i, [&](int j, double gj, bool dg) { ax -= ras::weight(gi, gj, dg, false) * X[j]; });
+      const double res = node_source((double)src[i], (double)gnd[i]) - ax;
+      rr += res * res;
+    }
+    rr = block_sum(rr, red);
+    const double relres = bb > 0.0 ? sqrt(rr / bb) : 0.0;
+    wo.iters += it;
+    wo.relres = dmax(wo.relres, relres);
+    int st = WIN_OK;
+    if (!(relres < kGate)) st = WIN_RESIDUAL;
+    else if (it >= itmax && sqrt(rz) > tol) st = WIN_MAXITER;
+    if (st > wo.status) {
+      wo.status = st;
+      wo.fail_relres = relres;
+      wo.fail_iters = (int)min(it, (long long)INT_MAX);
+    }
+
+    // 7. node currents (src/out.jl:178-207): branch currents e = w (v_lo - v_hi) over the edges
+    // lo < hi, cut at 1e-8 of the component's max of e (inflow) and of -e (outflow) separately
+    double mp = -INFINITY, mq = -INFINITY;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      if (lab[i] != root) continue;
+      const double gi = (double)g[i], vi = X[i];
+      for_nbrs<true>(s, g, i, [&](int j, double gj, bool dg) {
+        const double e = ras::weight(gi, gj, dg, false) * (vi - X[j]);
+        mp = dmax(mp, e);
+        mq = dmax(mq, -e);
+      });
+    }
+    mp = block_max(mp, red);
+    mq = block_max(mq, red);
+    for (int i = threadIdx.x; i < n; i += BT) {
+      if (lab[i] != root) continue;
+      const double gi = (double)g[i], vi = X[i];
+      double in = 0.0, outf = 0.0;
+      for_nbrs<false>(s, g, i, [&](int j, double gj, bool dg) {
+        const double w = ras::weight(gi, gj, dg, false);
+        const double e = j > i ? w * (vi - X[j]) : w * (X[j] - vi);
+        const double ep = cut(e, mp), eq = cut(-e, mq);
+        if (j < i) { in += ep > 0.0 ? ep : 0.0; outf += eq > 0.0 ? eq : 0.0; }
+        else       { in += -ep > 0.0 ? -ep : 0.0; outf += -eq > 0.0 ? -eq : 0.0; }
+      });
+      if (use_fin) {
+        const double fg = node_finite((double)gnd[i]) * vi;
+        in += fg < 0.0 ? -fg : 0.0;
+        outf += fg > 0.0 ? fg : 0.0;
+      }
+      cur[i] = in > outf ? in : outf;
+      if (volt) volt[i] = vi;
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) out[blockIdx.x] = wo;
+}
+
+template <typename T>
+cudaError_t launch(int nwin, Shape s, const void* g, const void* src, const void* gnd, double rtol, double atol,
+                   long long itmax, double* cur, double* volt, double* vec, int* lab, int* flag, int* list,
+                   WinOut* out, cudaStream_t st) {
+  k_advanced_batch<T><<<nwin, BT, 0, st>>>(s, (const T*)g, (const T*)src, (const T*)gnd, rtol, atol, itmax, cur,
+                                           volt, vec, lab, flag, list, out);
+  return cudaGetLastError();
+}
+
+size_t align256(size_t b) { return (b + 255) / 256 * 256; }
+
+}  // namespace
+
+#define CKB(call)                                                                              \
+  do {                                                                                         \
+    cudaError_t _e = (call);                                                                   \
+    if (_e != cudaSuccess) {                                                                   \
+      rc = set_err(CS_B200_ERR_CUDA, "CUDA error %s at %s:%d (%s)", cudaGetErrorString(_e), \
+                   __FILE__, __LINE__, #call);                                                 \
+      goto done;                                                                               \
+    }                                                                                          \
+  } while (0)
+
+extern "C" int cs_b200_solve_advanced_batch(int64_t nwin, int64_t nrows, int64_t ncols, const void* g,
+                                            const void* src, const void* gnd, int dtype, int four_neighbors,
+                                            int device, double rtol, int64_t itmax, void* cur, void* volt,
+                                            int64_t* iters, double* relres, int64_t* first_failed) {
+  if (first_failed) *first_failed = -1;
+  if (nwin < 0 || nrows < 1 || ncols < 1)
+    return set_err(CS_B200_ERR_ARG, "bad batch shape (nwin=%lld nrows=%lld ncols=%lld)",
+                   (long long)nwin, (long long)nrows, (long long)ncols);
+  if (nrows > INT_MAX / ncols || nwin > INT_MAX)
+    return set_err(CS_B200_ERR_ARG, "batch too large (nwin=%lld, %lld x %lld cells per window)",
+                   (long long)nwin, (long long)nrows, (long long)ncols);
+  if (dtype != CS_B200_F32 && dtype != CS_B200_F64) return set_err(CS_B200_ERR_ARG, "bad dtype %d", dtype);
+  if (!(rtol >= 0.0) || itmax < 0)
+    return set_err(CS_B200_ERR_ARG, "bad rtol %g / itmax %lld", rtol, (long long)itmax);
+  if (nwin > 0 && (!g || !src || !gnd || !cur))
+    return set_err(CS_B200_ERR_ARG, "g, src, gnd and cur must not be NULL");
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return set_err(CS_B200_ERR_CUDA, "no CUDA device available (%s): libcsb200 has no CPU fallback",
+                   cudaGetErrorString(e));
+  if (device < 0 || device >= ndev)
+    return set_err(CS_B200_ERR_ARG, "device %d out of range (0..%d)", device, ndev - 1);
+  if (nwin == 0) return CS_B200_OK;
+
+  int rc = CS_B200_OK;
+  const Shape s{(int)nrows, (int)ncols, (int)(nrows * ncols), four_neighbors ? 1 : 0};
+  const size_t cells = (size_t)nwin * s.ncell;
+  const size_t isz = dtype == CS_B200_F64 ? 8 : 4;
+  const size_t b_in = align256(cells * isz), b_out = align256(cells * 8), b_vec = align256(cells * 8 * NVEC),
+               b_int = align256(cells * 4), b_win = align256((size_t)nwin * sizeof(WinOut));
+  unsigned char* dbuf = nullptr;
+  cudaStream_t st = nullptr;
+  std::vector<WinOut> wo((size_t)nwin);
+  const long long itm = (long long)itmax;
+  const double atol = std::sqrt(2.220446049250313e-16);   // sqrt(eps(Float64)), Krylov.jl's default
+  double *d_cur, *d_volt, *d_vec;
+  int *d_lab, *d_flag, *d_list;
+  WinOut* d_out;
+  unsigned char* p;
+  int64_t bad = -1;
+  int worst = WIN_OK;
+
+  CKB(cudaSetDevice(device));
+  CKB(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  CKB(cudaMalloc(&dbuf, 3 * b_in + 2 * b_out + b_vec + 3 * b_int + b_win));
+  p = dbuf + 3 * b_in;
+  d_cur = (double*)p;   p += b_out;
+  d_volt = volt ? (double*)p : nullptr; p += b_out;
+  d_vec = (double*)p;   p += b_vec;
+  d_lab = (int*)p;      p += b_int;
+  d_flag = (int*)p;     p += b_int;
+  d_list = (int*)p;     p += b_int;
+  d_out = (WinOut*)p;
+  CKB(cudaMemcpyAsync(dbuf, g, cells * isz, cudaMemcpyHostToDevice, st));
+  CKB(cudaMemcpyAsync(dbuf + b_in, src, cells * isz, cudaMemcpyHostToDevice, st));
+  CKB(cudaMemcpyAsync(dbuf + 2 * b_in, gnd, cells * isz, cudaMemcpyHostToDevice, st));
+  if (dtype == CS_B200_F64)
+    CKB((launch<double>((int)nwin, s, dbuf, dbuf + b_in, dbuf + 2 * b_in, rtol, atol, itm, d_cur, d_volt, d_vec,
+                        d_lab, d_flag, d_list, d_out, st)));
+  else
+    CKB((launch<float>((int)nwin, s, dbuf, dbuf + b_in, dbuf + 2 * b_in, rtol, atol, itm, d_cur, d_volt, d_vec,
+                       d_lab, d_flag, d_list, d_out, st)));
+  CKB(cudaMemcpyAsync(cur, d_cur, cells * 8, cudaMemcpyDeviceToHost, st));
+  if (volt) CKB(cudaMemcpyAsync(volt, d_volt, cells * 8, cudaMemcpyDeviceToHost, st));
+  CKB(cudaMemcpyAsync(wo.data(), d_out, (size_t)nwin * sizeof(WinOut), cudaMemcpyDeviceToHost, st));
+  CKB(cudaStreamSynchronize(st));
+
+  for (int64_t w = 0; w < nwin; ++w) {
+    if (iters) iters[w] = wo[w].iters;
+    if (relres) relres[w] = wo[w].relres;
+    if (wo[w].status > worst) { worst = wo[w].status; bad = w; }
+  }
+  if (worst == WIN_RESIDUAL) {
+    rc = set_err(CS_B200_ERR_RESIDUAL,
+                 "CUDA PCG solver residual %g exceeds tolerance %g for window %lld (%d iterations)",
+                 wo[bad].fail_relres, kGate, (long long)bad, wo[bad].fail_iters);
+  } else if (worst == WIN_MAXITER) {
+    rc = set_err(CS_B200_ERR_MAXITER,
+                 "CUDA PCG solver reached itmax = %lld before rtol for window %lld (residual %g)",
+                 (long long)itmax, (long long)bad, wo[bad].fail_relres);
+  }
+  if (first_failed) *first_failed = bad;
+done:
+  if (dbuf) cudaFree(dbuf);
+  if (st) cudaStreamDestroy(st);
+  return rc;
+}

@@ -1751,6 +1751,12 @@ int ensure_flush(cs_b200_handle* h) {
 
 }  // namespace
 
+// the text cs_b200_last_error(NULL) returns, for handle-less entry points in other translation units
+int set_handleless_error(int code, const char* msg) {
+  g_create_error = msg;
+  return code;
+}
+
 // ---------------------------------------------------------------------------
 // C ABI
 // ---------------------------------------------------------------------------
@@ -1898,7 +1904,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1002; }
+int cs_b200_version(void) { return 1003; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();

@@ -34,8 +34,9 @@ __global__ void k_valid(int64_t ncell, const T* __restrict__ g, int* __restrict_
     valid[i] = g[i] > T(0) ? 1 : 0;   // NODATA (-9999), 0 and NaN are not nodes
 }
 
-// rowcnt[node] = 1 (diagonal) + number of valid stencil neighbours
-__global__ void k_count(int nrows, int ncols, int four, const int* __restrict__ valid,
+// rowcnt[node] = 1 (diagonal) + number of valid stencil neighbours.  Internal linkage: the header
+// is included by more than one translation unit.
+static __global__ void k_count(int nrows, int ncols, int four, const int* __restrict__ valid,
                         const int* __restrict__ nodeid, int* __restrict__ rowcnt) {
   const int64_t ncell = (int64_t)nrows * ncols;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < ncell; i += (int64_t)gridDim.x * blockDim.x) {

@@ -451,6 +451,40 @@ class B200Factor:
         _lib.check(self._lib, self._h, rc)
 
 
+def advanced_batch_bytes(ncell, itemsize, want_volt):
+    """Device bytes cs_b200_solve_advanced_batch allocates per window of `ncell` cells: the three
+    inputs, the current (and voltage) raster, five fp64 CG vectors and three int32 label arrays."""
+    return ncell * (3 * itemsize + 8 * (2 if want_volt else 1) + 5 * 8 + 3 * 4) + 32
+
+
+def solve_advanced_batch(g, src, gnd, four_neighbors, device, rtol, itmax, want_volt=False):
+    """One cs_b200_solve_advanced_batch call on stacks of equal-shape windows (nwin, nrows, ncols)
+    of one float dtype (float32 or float64).  Returns dict with cur, volt (nwin, nrows, ncols)
+    float64 | None, iters, relres (nwin,), rc (OK, ERR_RESIDUAL or ERR_MAXITER), first_failed
+    (window index or -1) and msg; other failures raise."""
+    lib = _lib.load()
+    nwin, nr, nc = g.shape
+    dt = _lib.dtype_code(g.dtype)
+    # window-major, column-major inside a window: (nwin, ncols, nrows) in C order
+    g_, s_, gnd_ = (np.ascontiguousarray(np.asarray(a, dtype=g.dtype).transpose(0, 2, 1)) for a in (g, src, gnd))
+    cur = np.empty((nwin, nc, nr), dtype=np.float64)
+    volt = np.empty((nwin, nc, nr), dtype=np.float64) if want_volt else None
+    iters = np.zeros(nwin, dtype=np.int64)
+    relres = np.zeros(nwin, dtype=np.float64)
+    bad = C.c_int64(-1)
+    rc = lib.cs_b200_solve_advanced_batch(nwin, nr, nc, _lib._ptr(g_), _lib._ptr(s_), _lib._ptr(gnd_), dt,
+                                          1 if four_neighbors else 0, device, float(rtol), int(itmax),
+                                          _lib._ptr(cur), _lib._ptr(volt), _lib._ptr(iters), _lib._ptr(relres),
+                                          C.byref(bad))
+    msg = ""
+    if rc not in (_lib.OK, _lib.ERR_RESIDUAL, _lib.ERR_MAXITER):
+        _lib.check(lib, None, rc)
+    if rc != _lib.OK:
+        msg = lib.cs_b200_last_error(None).decode()
+    return dict(cur=cur.transpose(0, 2, 1), volt=None if volt is None else volt.transpose(0, 2, 1),
+                iters=iters, relres=relres, rc=rc, first_failed=int(bad.value), msg=msg)
+
+
 # ---------------------------------------------------------------------------
 # the three plug-in hooks
 # ---------------------------------------------------------------------------

@@ -249,6 +249,30 @@ int cs_b200_solve_sources(cs_b200_handle* h, int64_t k, const int64_t* colptr, c
                           void* probe_volt, void* volt, void* curr, int accumulate,
                           int64_t* iters, double* relres);
 
+/* Omniscape's moving-window solve (compute_omniscape_current, src/utils.jl:145-257) for a batch of
+ * nwin windows of nrows x ncols cells, without a handle: one upload, one kernel launch (one CTA per
+ * window), one download, whatever nwin is.
+ *   g, src, gnd: host, the nwin windows stacked, each column-major (cell r + c * nrows), element type
+ *                `dtype`.  Cells with g <= 0 (0, NODATA -9999, NaN) are not nodes; pad windows of
+ *                other shapes with g = 0.  Ground values are conductances: Inf = direct ground (0 V),
+ *                finite = added to the diagonal.  Conflicts: rmvsrc.  Neighbours: 4 or 8 with the
+ *                average-conductance rule.
+ *   Every connected component of a window is its own advanced-mode solve (skipped when its sources
+ *   or its grounds sum to 0): Jacobi-preconditioned CG in fp64 with the stop rule
+ *   sqrt(r'z) <= sqrt(eps) + rtol sqrt(r0'z0), at most itmax iterations, then the true-residual
+ *   gate 1e-4 on the reduced system and the node currents of src/out.jl:178-207.
+ *   cur:  host, nwin x nrows x ncols fp64 (same layout), node current per cell, 0 off solved components.
+ *   volt: NULL or the same for the voltages.
+ *   iters[nwin] (CG iterations summed over the window's components), relres[nwin] (largest true
+ *   relative residual of its components), first_failed: may be NULL.
+ * CS_B200_ERR_RESIDUAL / CS_B200_ERR_MAXITER name the first window that failed the gate / ran into
+ * itmax in *first_failed (-1 otherwise) and in cs_b200_last_error(NULL); every output is still
+ * written.  Bad shapes, a NULL required pointer or a bad dtype give CS_B200_ERR_ARG.               */
+int cs_b200_solve_advanced_batch(int64_t nwin, int64_t nrows, int64_t ncols, const void* g, const void* src,
+                                 const void* gnd, int dtype, int four_neighbors, int device, double rtol,
+                                 int64_t itmax, void* cur, void* volt, int64_t* iters, double* relres,
+                                 int64_t* first_failed);
+
 /* Cumulative / max node-current vectors (n values of dtype each; either may be
  * NULL).  max is initialised to -9999 like src/utils.jl:124.                        */
 int cs_b200_read_currents(cs_b200_handle* h, void* cum, void* max);
