@@ -953,14 +953,19 @@ void launch_prolong_jacobi(cs_b200_handle* h, DevLevel& L, const T* Yc, const T*
   const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
   const CsrP<T> p{L.P.rowptr, L.P.colidx, (const T*)L.P.vals, L.P.ell_col, (const T*)L.P.ell_val, L.P.ell_ld};
   const SpmmEpi<T> ep{B, (const T*)L.dinv, (T)L.omega, h->d_ctl, h->d_partials};
-  constexpr int V16 = 16 / (int)sizeof(T);
-  constexpr int CGn = KT / (KT < V16 ? KT : V16);
-  constexpr int RPP = NT / CGn;
-  constexpr int SMEM = (RPP + 2) * (PJ_TC + 2) * KT * (int)sizeof(T);
-  static_assert(SMEM <= 48 * 1024, "tile fits the default dynamic shared memory");
-  const long long ntiles = (long long)((m.dia_nr + RPP - 1) / RPP) *
-                           ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + PJ_TC - 1) / PJ_TC);
-  const int grid = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));
+  using S = PjShape<T, KT>;
+  constexpr int SMEM = S::SMEM;
+  constexpr int MINB = sizeof(T) == 4 ? PJ_MINB_F32 : PJ_MINB_F64;
+  static_assert(SMEM <= 48 * 1024, "the strip buffers fit the default dynamic shared memory");
+  // one resident wave: every CTA's run of (strip, column) steps is as long as possible, which keeps the
+  // halo columns a CTA rebuilds at the start of each run rare
+  // asked per launch, on the handle's device (host-side query; the launches are captured into graphs)
+  int occ = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_stencil_prolong_jacobi<T, KT, MODE, MINB>, NT, SMEM);
+  occ = std::max(1, occ);
+  const long long nsteps = (long long)((m.dia_nr + S::RPS - 1) / S::RPS) *
+                           (((long long)m.nrows + m.dia_nr - 1) / m.dia_nr);
+  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min(h->grid_spmm, h->num_sms * occ), nsteps));
   cudaEvent_t e0 = nullptr, e1 = nullptr;
   const bool prof = h->profile && timed;
   if (prof) {
@@ -978,7 +983,6 @@ void launch_prolong_jacobi(cs_b200_handle* h, DevLevel& L, const T* Yc, const T*
     h->prof_pair_bytes.push_back(fb);
     cudaEventRecord(e0, h->stream);
   }
-  constexpr int MINB = sizeof(T) == 4 ? 4 : 3;
   k_stencil_prolong_jacobi<T, KT, MODE, MINB><<<grid, NT, SMEM, h->stream>>>(a, p, Yc, X0, Yout, ep);
   if (prof) cudaEventRecord(e1, h->stream);
   h->stats.kernel_launches++;

@@ -876,6 +876,9 @@ k_spmm_win(const WinCsr<T> A, const T* __restrict__ X, T* __restrict__ Y, const 
           for (int i = 0; i < CPT; ++i) {
             const int col = gt * CPT + i;
             double t = 0.0;
+            // not unrolled: a full unroll of the GRP-term chain (GRP = 64 .. 512) times the CPT columns
+            // held the shared-memory operands of all of them in registers and spilled to local memory
+#pragma unroll 1
             for (int q = 0; q < GRP; ++q) t += s_long[g * GT + q * KT + col];
             spmm_epilogue<T, MODE>(row0, (size_t)row0 * KT + col, (T)t, X, Y, ep, dot0[i], dot1[i]);
           }
@@ -1069,15 +1072,23 @@ k_stencil(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, const S
 
 // ---------------------------------------------------------------------------
 // Upward leg of the V-cycle on a stencil-form level, fused:  prolongate + correct + post-smooth
-//     x1 = x0 + P y          (y: the coarser level's correction, P: plain CSR, ~3 entries per row)
+//     x1 = x0 + P y          (y: the coarser level's correction, P: ~3 entries per row)
 //     z  = x1 + omega D^-1 (b - A x1)        [+ dot(b, z) -> CG beta / stop test on the finest level]
-// One CTA owns a tile of RPP rows x PJ_TC raster columns; it first builds x1 for the tile AND its one-cell
-// halo in shared memory (the halo's P rows are recomputed: 27 % more P / x0 traffic at 128 x 8), then applies
-// the 9 diagonals out of shared memory.  x1 never goes to global memory: against the two-kernel form
-// (k_spmm_win SP_ADD then k_stencil SP_JACOBI_DOT) that saves the write and both re-reads of the x panel
-// and the per-block overhead of the windowed kernel on the 3-entry rows of P.
+// Streaming form.  The rows of every raster column are cut into strips of PJ_RH - 2 rows; the (strip, raster
+// column) steps, strip-major, are dealt to the CTAs in contiguous runs, and a CTA sweeps its run column by
+// column.  Thread (rr, g) owns row rr - 1 of the strip (rr = 0 and RH - 1 are the one-row halo) and column
+// group g of the panel.  Per column step a thread builds x1 of its row of column c into a four-column ring in
+// shared memory, the CTA synchronises once, and the strip's threads apply the 9 diagonals to column c - 1 out
+// of the ring.  So each x1 is built once (the halo rows add 2 / (RH - 2) of P / x0 traffic, against 27 % for
+// the 128 x 8 tiles with a recomputed halo this replaces), a row's b and 1/diag are read once for both x0 and
+// the Jacobi step, and the prolongator row of column c + 1 is in flight while column c is built.  x1 never
+// goes to global memory: against the two-kernel form (k_spmm_win SP_ADD then k_stencil SP_JACOBI_DOT) that
+// saves the write and both re-reads of the x panel.  Per element the arithmetic is that of the two-kernel
+// form: the P terms summed in slot order onto x0, the 9 diagonal terms in slot order.
 // ---------------------------------------------------------------------------
-constexpr int PJ_TC = 8;
+constexpr int PJ_RING = 4;   // x1 columns in shared memory: c - 2 (still being read by slow threads), c - 1, c, c + 1
+constexpr int PJ_MINB_F32 = 3;   // CTAs per SM of k_stencil_prolong_jacobi (see below)
+constexpr int PJ_MINB_F64 = 2;
 
 template <typename T> struct CsrP {
   const int* rowptr;
@@ -1090,207 +1101,197 @@ template <typename T> struct CsrP {
   size_t ell_ld;
 };
 
-// MINB = 4 (the fp32 V-cycle): four CTAs per SM, 64 registers -- carried over from the tuning on the
-// previous GPU target, where the fourth CTA's loads in flight paid; not re-measured on the H100.  What
-// frees the registers: a thread keeps
-// its b.z partial sums (~70 products) in T, the V-cycle's own precision, instead of double; they enter the
-// double tree reduction afterwards.  MINB = 3 keeps double partial sums (fp64 cycles).
-template <typename T, int MINB> struct PjDot { typedef double type; };
-template <typename T> struct PjDot<T, 4> { typedef T type; };
+template <typename T, int KT> struct PjShape {
+  static constexpr int V16 = 16 / (int)sizeof(T);
+  static constexpr int CPT = KT < V16 ? KT : V16;     // panel columns per thread (one 16-byte vector)
+  static constexpr int CG = KT / CPT;                 // column groups per row
+  static constexpr int RH = NT / CG;                  // strip rows + the two halo rows
+  static constexpr int RPS = RH - 2;                  // rows per strip
+  // fp32: the 9 diagonal values of a row wait for the Jacobi step in shared memory (fp64: in registers)
+  static constexpr bool VSMEM = sizeof(T) == 4;
+  // the x1 ring, per thread the b vector and omega / diag of its row, and (VSMEM) per strip row its 9
+  // diagonal values, the last two double-buffered by column parity
+  static constexpr int SMEM = (PJ_RING * RH * KT + 2 * NT * CPT + 2 * NT + (VSMEM ? 2 * 9 * RH : 0)) * (int)sizeof(T);
+};
 
+// MINB: CTAs per SM the register budget is cut for (launch_prolong_jacobi).  The b.z partial sums are
+// double in every instantiation.  What waits for the Jacobi step of the next column step -- the row's b and
+// omega / diag, and in fp32 its 9 diagonal values (cp.async) -- waits in shared memory, not in registers:
+// that keeps the fp32 variants within the 80 registers of three CTAs per SM without spills.  Measured on an
+// H100 80GB HBM3 (700 W), fp32 k = 8 on the 3163^2 raster, with those values still in registers: one PCG
+// iteration took 4.30 ms at MINB = 2 (no spills), 4.14 ms at 3 and 4.04 ms at 4, where ptxas spilled 16-48 B
+// of the SP_JACOBI_DOT variant.  With the shared-memory slots MINB = 3 is spill-free; MINB = 4 (64 registers)
+// still spills.  fp64 needs up to 128 registers (k = 1) and keeps its diagonals in registers: MINB = 2.
 template <typename T, int KT, int MODE, int MINB>
 __global__ void __launch_bounds__(NT, MINB)
 k_stencil_prolong_jacobi(const DiaDev<T> A, const CsrP<T> P, const T* __restrict__ Yc, const T* __restrict__ X0,
                          T* __restrict__ Z, const SpmmEpi<T> ep) {
   static_assert(MODE == SP_JACOBI || MODE == SP_JACOBI_DOT, "post-smoothing modes only");
-  constexpr int V16 = 16 / (int)sizeof(T);
-  constexpr int CPT = KT < V16 ? KT : V16;
-  constexpr int CG = KT / CPT;
-  constexpr int RPP = NT / CG;
-  constexpr int RH = RPP + 2, CH = PJ_TC + 2;
+  using S = PjShape<T, KT>;
+  constexpr int CPT = S::CPT, CG = S::CG, RH = S::RH, RPS = S::RPS;
   extern __shared__ __align__(16) unsigned char pj_smem[];
-  T* xs = reinterpret_cast<T*>(pj_smem);                 // [CH][RH][KT]
+  T* xs = reinterpret_cast<T*>(pj_smem);                 // [PJ_RING][RH][KT]
+  T* bsm = xs + PJ_RING * RH * KT;                       // [2][NT][CPT]
+  T* wsm = bsm + 2 * NT * CPT;                           // [2][NT]
+  T* vsm = wsm + 2 * NT;                                 // [2][9][RH] (VSMEM)
   const int tid = threadIdx.x;
-  const int cg = tid % CG, rl = tid / CG, c0 = cg * CPT;
+  const int g = tid % CG, rr = tid / CG, c0 = g * CPT;
+  const bool inner = rr >= 1 && rr <= RPS;
   const int n = A.n, nr = A.nr;
   const int ncol = (n + nr - 1) / nr;
-  const int nrc = (nr + RPP - 1) / RPP;
-  const int ntc = (ncol + PJ_TC - 1) / PJ_TC;
-  const long long ntiles = (long long)nrc * ntc;
-  typedef typename PjDot<T, MINB>::type DotT;
-  DotT dot0[CPT];
+  const int nstrip = (nr + RPS - 1) / RPS;
+  // nstep <= nr * ncol < n + nr: int for every operator launch_prolong_jacobi accepts (n + nr < 2^31)
+  const int nstep = nstrip * ncol;
+  const int per = (nstep + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int s_beg = (int)min((long long)nstep, (long long)blockIdx.x * per);
+  const int s_end = (int)min((long long)nstep, ((long long)blockIdx.x + 1) * per);
+  const bool ell = P.ell_col != nullptr;
+  double dot0[CPT];
 #pragma unroll
-  for (int i = 0; i < CPT; ++i) dot0[i] = DotT(0);
+  for (int i = 0; i < CPT; ++i) dot0[i] = 0.0;
 
-  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
-    const int tc = (int)(t / nrc), rc = (int)(t % nrc);
-    __syncthreads();                                     // the previous tile's readers are done
-    // ---- phase 1: x1 = x0 + P y on the tile and its halo
-    if (P.ell_col) {
-      // ELL-4 prolongator: no row-offset indirection; two tile rows per thread and trip, so that
-      // 2 x (x0 + 4 columns + 4 values) independent loads, then 2 x 4 gathers of y, are in flight
-      constexpr int ITEMS = RH * CH * CG;
-      for (int it0 = tid; it0 < ITEMS; it0 += 2 * NT) {
-        int rowu[2], slot[2];
-        bool ok[2];
+  for (int s0 = s_beg; s0 < s_end;) {
+    // one segment: raster columns [cb, ce) of one strip
+    const int strip = s0 / ncol, cb = s0 % ncol;
+    const int ce = min(ncol, cb + (s_end - s0));
+    s0 += ce - cb;
+    const int r = strip * RPS + rr - 1;                  // this thread's row within a raster column
+    const bool rok = r >= 0 && r < nr;
+    auto row_of = [&](int c, int& row) {
+      const long long rl = (long long)c * nr + r;
+      const bool ok = rok && c >= 0 && c < ncol && rl < n;
+      row = ok ? (int)rl : 0;                            // out of the raster: x1 = 0, any row will do for the loads
+      return ok;
+    };
+    auto ell_row = [&](int row, int (&cj)[4], T (&pv)[4]) {
 #pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int it = it0 + u * NT;
-          const int g = it % CG;
-          const int rr = (it / CG) % RH;
-          const int cc = it / (CG * RH);
-          const int c = tc * PJ_TC + cc - 1, r = rc * RPP + rr - 1;
-          const long long row_l = (long long)c * nr + r;
-          ok[u] = it < ITEMS && c >= 0 && c < ncol && r >= 0 && r < nr && row_l < n;
-          rowu[u] = ok[u] ? (int)row_l : 0;
-          slot[u] = it < ITEMS ? (cc * RH + rr) * KT + g * CPT : -1;
-        }
-        T x1[2][CPT], pv[2][4];
-        int cj[2][4];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int g = (it0 + u * NT) % CG;
-          if (X0) {
-            ldvec<T, CPT>(X0 + (size_t)rowu[u] * KT + g * CPT, x1[u]);
-          } else {                       // x0 = omega D^-1 b, never stored
-            ldvec<T, CPT>(ep.B + (size_t)rowu[u] * KT + g * CPT, x1[u]);
-            const T w0 = ep.omega * ep.dinv[rowu[u]];
-#pragma unroll
-            for (int i = 0; i < CPT; ++i) x1[u][i] *= w0;
-          }
-#pragma unroll
-          for (int q = 0; q < 4; ++q) {
-            cj[u][q] = __ldg(P.ell_col + (size_t)q * P.ell_ld + rowu[u]);
-            pv[u][q] = __ldg(P.ell_val + (size_t)q * P.ell_ld + rowu[u]);
-          }
-        }
-        T yv[2][4][CPT];
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          const int g = (it0 + u * NT) % CG;
-#pragma unroll
-          for (int q = 0; q < 4; ++q) ldvec<T, CPT>(Yc + (size_t)cj[u][q] * KT + g * CPT, yv[u][q]);
-        }
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-          if (slot[u] < 0) continue;
-#pragma unroll
-          for (int i = 0; i < CPT; ++i) {
-            T a = x1[u][i];
-#pragma unroll
-            for (int q = 0; q < 4; ++q) a += pv[u][q] * yv[u][q][i];
-            x1[u][i] = ok[u] ? a : T(0);
-          }
-          stvec<T, CPT>(xs + slot[u], x1[u]);
-        }
+      for (int q = 0; q < 4; ++q) {
+        cj[q] = __ldg(P.ell_col + (size_t)q * P.ell_ld + row);
+        pv[q] = __ldg(P.ell_val + (size_t)q * P.ell_ld + row);
       }
-    } else
-    for (int it = tid; it < RH * CH * CG; it += NT) {
-      const int g = it % CG;
-      const int rr = (it / CG) % RH;
-      const int cc = it / (CG * RH);
-      const int c = tc * PJ_TC + cc - 1, r = rc * RPP + rr - 1;
-      T x1[CPT];
+    };
+    int rowc, rowp = 0;
+    bool okc = row_of(cb - 1, rowc), okp = false;
+    int cj[4] = {0, 0, 0, 0};
+    T pv[4] = {T(0), T(0), T(0), T(0)};
+    if (ell) ell_row(rowc, cj, pv);
+    __syncthreads();                                     // the ring's readers of the previous segment are done
+    for (int c = cb - 1; c <= ce; ++c) {
+      const int rel = c - (cb - 1);                      // ring slot of column c: rel % PJ_RING
+      const bool zdo = inner && c > cb && okp;           // z of column c - 1 (row rowp) after the barrier
+      // ---- loads: diagonals of column c - 1, the prolongator row of column c + 1, then b, 1/diag, x0 and the
+      //      y gathers of column c
+      T v[9];
+      if constexpr (S::VSMEM) {
+        // straight to shared memory (cp.async), one copy per row by its column group 0
+        if (zdo && g == 0) {
 #pragma unroll
-      for (int i = 0; i < CPT; ++i) x1[i] = T(0);
-      const long long row_l = (long long)c * nr + r;
-      if (c >= 0 && c < ncol && r >= 0 && r < nr && row_l < n) {
-        const int row = (int)row_l;
-        const int a = P.rowptr[row], b = P.rowptr[row + 1];
-        if (X0) {
-          ldvec<T, CPT>(X0 + (size_t)row * KT + g * CPT, x1);
-        } else {
-          ldvec<T, CPT>(ep.B + (size_t)row * KT + g * CPT, x1);
-          const T w0 = ep.omega * ep.dinv[row];
-#pragma unroll
-          for (int i = 0; i < CPT; ++i) x1[i] *= w0;
+          for (int s = 0; s < 9; ++s)
+            asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(smem_u32(vsm + ((rel & 1) * 9 + s) * RH + rr)),
+                         "l"(A.vals + (size_t)s * A.ld + rowp), "n"((int)sizeof(T)) : "memory");
         }
-        int cj[4];
-        T pv[4];
+      } else {
+#pragma unroll
+        for (int s = 0; s < 9; ++s) v[s] = zdo ? __ldcs(A.vals + (size_t)s * A.ld + rowp) : T(0);   // streamed once
+      }
+      int rown;
+      const bool okn = row_of(c + 1, rown);
+      int cjn[4] = {0, 0, 0, 0};
+      T pvn[4] = {T(0), T(0), T(0), T(0)};
+      if (ell && c < ce) ell_row(rown, cjn, pvn);
+      T bc[CPT], x1[CPT];
+      ldvec<T, CPT>(ep.B + (size_t)rowc * KT + c0, bc);
+      const T wc = ep.omega * ep.dinv[rowc];
+      if (X0) {
+        ldvec<T, CPT>(X0 + (size_t)rowc * KT + c0, x1);
+      } else {                                           // x0 = omega D^-1 b, never stored
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) x1[i] = bc[i] * wc;
+      }
+      if (ell) {
+        T yv[4][CPT];
+#pragma unroll
+        for (int q = 0; q < 4; ++q) ldvec<T, CPT>(Yc + (size_t)cj[q] * KT + c0, yv[q]);
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) {
+          T a = x1[i];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) a += pv[q] * yv[q][i];
+          x1[i] = okc ? a : T(0);
+        }
+      } else if (okc) {                                  // plain CSR (rows with more than 4 entries)
+        const int a = P.rowptr[rowc], b = P.rowptr[rowc + 1];
+        int cq[4];
+        T pq[4];
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
           const bool ok = a + q < b;
-          cj[q] = ok ? __ldg(P.colidx + a + q) : 0;
-          pv[q] = ok ? __ldg(P.vals + a + q) : T(0);
+          cq[q] = ok ? __ldg(P.colidx + a + q) : 0;
+          pq[q] = ok ? __ldg(P.vals + a + q) : T(0);
         }
         T yv[4][CPT];
 #pragma unroll
-        for (int q = 0; q < 4; ++q) ldvec<T, CPT>(Yc + (size_t)cj[q] * KT + g * CPT, yv[q]);
+        for (int q = 0; q < 4; ++q) ldvec<T, CPT>(Yc + (size_t)cq[q] * KT + c0, yv[q]);
 #pragma unroll
         for (int q = 0; q < 4; ++q)
 #pragma unroll
-          for (int i = 0; i < CPT; ++i) x1[i] += pv[q] * yv[q][i];
+          for (int i = 0; i < CPT; ++i) x1[i] += pq[q] * yv[q][i];
         for (int j = a + 4; j < b; ++j) {
           const T pw = P.vals[j];
           T yw[CPT];
-          ldvec<T, CPT>(Yc + (size_t)P.colidx[j] * KT + g * CPT, yw);
+          ldvec<T, CPT>(Yc + (size_t)P.colidx[j] * KT + c0, yw);
 #pragma unroll
           for (int i = 0; i < CPT; ++i) x1[i] += pw * yw[i];
         }
+      } else {
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) x1[i] = T(0);
       }
-      stvec<T, CPT>(xs + ((size_t)cc * RH + rr) * KT + g * CPT, x1);
-    }
-    __syncthreads();
-    // ---- phase 2: z = x1 + omega D^-1 (b - A x1)
-    const int r = rc * RPP + rl;
-    if (r < nr) {
-      const int cbeg = tc * PJ_TC;
-      int cend = min(ncol, (tc + 1) * PJ_TC);
-      if ((long long)(cend - 1) * nr + r >= n) cend = (int)((n - 1 - r) / nr) + 1;      // ragged last column
-      // the global operands of column c + 1 (9 diagonals, b, 1/diag) are requested before column c is
-      // combined out of shared memory
-      T v[9], bb[CPT], dv = T(0);
-      auto fetch = [&](int c, T (&vv)[9], T (&bv)[CPT], T& d) {
-        const int row = c * nr + r;
-#pragma unroll
-        for (int s = 0; s < 9; ++s) vv[s] = __ldcs(A.vals + (size_t)s * A.ld + row);
-        ldvec<T, CPT>(ep.B + (size_t)row * KT + c0, bv);
-        d = ep.omega * ep.dinv[row];
-      };
-      if (cbeg < cend) fetch(cbeg, v, bb, dv);
-      for (int c = cbeg; c < cend; ++c) {
-        const int row = c * nr + r;
-        const int cc = c - cbeg + 1, rr = rl + 1;
-        T vn[9], bn[CPT], dn = T(0);
-#pragma unroll
-        for (int s = 0; s < 9; ++s) vn[s] = T(0);
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) bn[i] = T(0);
-        if (c + 1 < cend) fetch(c + 1, vn, bn, dn);
+      stvec<T, CPT>(xs + ((size_t)(rel % PJ_RING) * RH + rr) * KT + c0, x1);
+      stvec<T, CPT>(bsm + ((rel & 1) * NT + tid) * CPT, bc);     // for the Jacobi step of column c (next step)
+      wsm[(rel & 1) * NT + tid] = wc;
+      if constexpr (S::VSMEM) asm volatile("cp.async.wait_all;" ::: "memory");
+      __syncthreads();
+      // ---- z = x1 + omega D^-1 (b - A x1) on column c - 1
+      if (zdo) {
         T acc[CPT], xo[CPT];
 #pragma unroll
         for (int i = 0; i < CPT; ++i) acc[i] = T(0);
 #pragma unroll
         for (int s = 0; s < 9; ++s) {
+          const T vs = S::VSMEM ? vsm[((rel & 1) * 9 + s) * RH + rr] : v[s];
           T xv[CPT];
-          ldvec<T, CPT>(xs + ((size_t)(cc + s / 3 - 1) * RH + (rr + s % 3 - 1)) * KT + c0, xv);
+          ldvec<T, CPT>(xs + ((size_t)((rel + s / 3 - 2) % PJ_RING) * RH + (rr + s % 3 - 1)) * KT + c0, xv);
 #pragma unroll
           for (int i = 0; i < CPT; ++i) {
-            acc[i] += v[s] * xv[i];
+            acc[i] += vs * xv[i];
             if (s == 4) xo[i] = xv[i];
           }
         }
-        T out[CPT];
+        T bp[CPT], out[CPT];                             // b and omega / diag of row rowp, stored one step back
+        ldvec<T, CPT>(bsm + ((~rel & 1) * NT + tid) * CPT, bp);
+        const T wp = wsm[(~rel & 1) * NT + tid];
 #pragma unroll
         for (int i = 0; i < CPT; ++i) {
-          const T zn = xo[i] + dv * (bb[i] - acc[i]);
+          const T zn = xo[i] + wp * (bp[i] - acc[i]);
           out[i] = zn;
-          if (MODE == SP_JACOBI_DOT) dot0[i] += (DotT)bb[i] * (DotT)zn;
+          if (MODE == SP_JACOBI_DOT) dot0[i] += (double)bp[i] * (double)zn;
         }
-        stvec<T, CPT>(Z + (size_t)row * KT + c0, out);
-#pragma unroll
-        for (int s = 0; s < 9; ++s) v[s] = vn[s];
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) bb[i] = bn[i];
-        dv = dn;
+        stvec<T, CPT>(Z + (size_t)rowp * KT + c0, out);
       }
+      rowp = rowc;
+      okp = okc;
+      rowc = rown;
+      okc = okn;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) { cj[q] = cjn[q]; pv[q] = pvn[q]; }
     }
   }
   if (MODE == SP_JACOBI_DOT) {
     CSB_REDUCE_SMEM(1, KT)
     double v[1][CPT];
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) v[0][i] = (double)dot0[i];
+    for (int i = 0; i < CPT; ++i) v[0][i] = dot0[i];
     if (grid_reduce<KT, CPT, 1, false>(v, ep.partials, &ep.ctl->ticket, s_warp, s_tree, s_out))
       cg_after_precond<KT>(ep.ctl, s_out);
   }
