@@ -722,6 +722,230 @@ class OneToAllOutput:
     num_solves: int = 0
 
 
+# ---------------------------------------------------------------------------
+# raster pairwise front end  (src/raster/pairwise.jl:14-135)
+# ---------------------------------------------------------------------------
+def raster_pairwise(data: RasterData, flags: Flags, cfg, solver=None, four_neighbors=False, avg_res=False,
+                    sink=None) -> PairwiseOutput:
+    """src/raster/pairwise.jl:14-30.  Focal points with distinct ids: one graph, single_ground_all_pairs.
+    An id on several cells makes focal regions (_pt_file_polygons_path): every region pair is a Dirichlet
+    problem on the raster's own Laplacian (region a at 0 V, region b at 1 V), so the pairs are columns of
+    cs_b200_solve_region_pairs on ONE whole-raster handle; pairs that operator cannot express exactly take
+    the reference's per-pair path (polygon map, graph and solve per pair).  `sink` as in `solve`."""
+    from . import graph
+    solver = solver or get_solver(cfg)
+    cellmap, polymap = data.cellmap, data.polymap
+    points_rc = tuple(np.asarray(a) for a in data.points_rc)
+    inc = data.included_pairs
+    exclude = set()
+    regions = len(points_rc[0]) != len(np.unique(points_rc[2]))
+    if inc is not None:
+        points_rc, exclude = graph.generate_exclude_pairs(points_rc, inc)
+    if not regions:
+        nodemap = graph.construct_node_map(cellmap, polymap)
+        G = graph.laplacian(graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors))
+        points = nodemap[points_rc[0] - 1, points_rc[1] - 1]
+        prob = GraphProblem(G, graph.connected_components(G), points, points_rc[2], exclude, nodemap, polymap,
+                            cellmap, solver)
+        return single_ground_all_pairs(prob, flags, cfg, sink=sink)
+    return _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink)
+
+
+@dataclass
+class RegionPlan:
+    """How the focal-region driver serves each id pair (i, j) (indices into `ids`, i < j): `batched`
+    pairs are columns of cs_b200_solve_region_pairs with `sets[p]` (0-based rows of L0) as id p's region,
+    `per_pair` pairs take the reference's per-pair path (`reasons` says why), `unconnected` pairs have
+    no L0 component touching both regions (R = -1, nothing solved)."""
+    ids: list
+    sets: dict
+    batched: list
+    per_pair: list
+    unconnected: list
+    reasons: dict
+
+
+def _region_cells(cellmap, polymap, points_rc, p):
+    """Id p on the per-pair polygon map (graph.create_pair_polymap), flat column-major cell indices:
+    (cells merged with p's first point, cells relabelled elsewhere).  Raises graph.RegionPolymapError."""
+    from . import graph
+    rr, cc_, ids = points_rc
+    nr = cellmap.shape[0]
+    k = int(np.nonzero(ids == p)[0][0])
+    x = int((cc_[k] - 1) * nr + (rr[k] - 1))
+    none = np.zeros(0, dtype=np.int64)
+    if polymap is None or np.size(polymap) == 0:
+        sel = ids == p
+        return np.unique((cc_[sel] - 1) * nr + (rr[sel] - 1)), none
+    pm = np.asarray(polymap).reshape(-1, order="F")
+    mask = graph.region_relabel(np.asarray(polymap), points_rc, p)
+    own = np.nonzero(pm == pm[x])[0] if pm[x] != 0 else np.array([x])
+    if mask is None:
+        return own, none
+    q = np.nonzero(mask.reshape(-1, order="F"))[0]
+    return (q, none) if mask.reshape(-1, order="F")[x] else (own, q)
+
+
+def plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of):
+    """Decide each region pair's path from L0's node map (`nodemap`, 1-based, 0 = none) and component
+    label per L0 node (`comp_of`, 0-based node index).  A pair is batched when, for both ids, every cell
+    the per-pair polygon map merges is already an L0 node, those nodes hold no other cell, the map changes
+    nothing else, and the two regions share no cell and no node."""
+    from . import graph
+    ids = np.asarray(points_rc[2])
+    pts = list(dict.fromkeys(int(p) for p in ids))
+    node_of = np.asarray(nodemap).reshape(-1, order="F")
+    region, bad = {}, {}
+    for p in pts:
+        try:
+            cells, extra = _region_cells(cellmap, polymap, points_rc, p)
+        except graph.RegionPolymapError:
+            bad[p] = "the reference's error branch (raised by the per-pair path)"
+            continue
+        nodes = node_of[cells]
+        if np.any(nodes == 0):
+            bad[p] = "a region cell is not a node of the raster's graph"
+            continue
+        s = np.unique(nodes)
+        if np.count_nonzero(np.isin(node_of, s)) != len(cells):
+            bad[p] = "the region's nodes hold cells outside the region"
+            continue
+        if len(extra) and (np.any(node_of[extra] == 0) or len(np.unique(node_of[extra])) > 1):
+            bad[p] = "the polygon map merges polygons outside the region"
+            continue
+        region[p] = (s - 1, np.union1d(cells, extra))
+    plan = RegionPlan(pts, {p: r[0] for p, r in region.items()}, [], [], [], {})
+    for i in range(len(pts)):
+        for j in range(i + 1, len(pts)):
+            a, b = pts[i], pts[j]
+            if (a, b) in exclude or (b, a) in exclude:
+                continue
+            why = bad.get(a) or bad.get(b)
+            if why is None and (np.intersect1d(region[a][0], region[b][0]).size or
+                                np.intersect1d(region[a][1], region[b][1]).size):
+                why = "the two regions overlap"
+            if why is not None:
+                plan.per_pair.append((i, j))
+                plan.reasons[(i, j)] = why
+            elif np.intersect1d(comp_of[region[a][0]], comp_of[region[b][0]]).size:
+                plan.batched.append((i, j))
+            else:
+                plan.unconnected.append((i, j))
+    return plan
+
+
+def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink):
+    """src/raster/pairwise.jl:72-135 on one whole-raster operator (see raster_pairwise)."""
+    from . import graph
+    from scipy.sparse import csgraph
+    o = flags.outputflags
+    want_maps = o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
+    per_pair_curr = o.write_cur_maps and not o.write_cum_cur_map_only
+    nodemap = graph.construct_node_map(cellmap, polymap)
+    adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
+    adj.eliminate_zeros()
+    _, comp_of = csgraph.connected_components(adj, directed=False)
+    plan = plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of)
+    pts = plan.ids
+    P = len(pts)
+    R = -np.ones((P, P))
+    out = PairwiseOutput(resistances=None)
+    out.cum_curmap = np.zeros(cellmap.shape)
+    out.max_curmap = np.full(cellmap.shape, NODATA) if o.write_max_cur_maps else None
+
+    def emit(key, vm, cm):
+        if vm is not None:
+            if sink is not None:
+                sink.voltmap(key, vm)
+            else:
+                out.voltmaps[key] = vm
+        if cm is not None:
+            if sink is not None:
+                sink.curmap(key, cm)
+            else:
+                out.curmaps[key] = cm
+
+    if plan.batched:
+        factor, dev_nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                                        avg_res=avg_res, log_transform=o.log_transform_maps)
+        with factor:
+            if not np.array_equal(np.asarray(dev_nodemap), nodemap):
+                raise RuntimeError("device node map differs from the host's")
+            used = sorted({pts[i] for i, _ in plan.batched} | {pts[j] for _, j in plan.batched})
+            slot = {p: s for s, p in enumerate(used)}
+            sets = [plan.sets[p] for p in used]
+            if want_maps:
+                factor.reset_currents()
+            bs = max(1, int(solver.bs))
+            for st in range(0, len(plan.batched), bs):
+                chunk = plan.batched[st:st + bs]
+                res = factor.solve_region_pairs(sets, [slot[pts[i]] for i, _ in chunk],
+                                                [slot[pts[j]] for _, j in chunk], want_volt=o.write_volt_maps,
+                                                want_curr=per_pair_curr, accumulate=want_maps)
+                out.stats.append(factor.stats())
+                out.num_solves += len(chunk)
+                out.iterations += int(res["iters"].sum())
+                for col, (i, j) in enumerate(chunk):
+                    R[i, j] = R[j, i] = float(res["R"][col])
+                    vm = cm = None
+                    if o.write_volt_maps:
+                        vm = _process_grid(_scatter(res["volt"][:, col].astype(np.float64), nodemap), cellmap,
+                                           False, o.set_null_voltages_to_nodata)
+                    if per_pair_curr:
+                        cm = _process_grid(_scatter(res["curr"][:, col].astype(np.float64), nodemap), cellmap,
+                                           o.log_transform_maps, o.set_null_currents_to_nodata)
+                    emit((pts[i], pts[j]), vm, cm)
+            if want_maps:
+                # the per-node accumulation of every batched pair, as core.solve scatters it (cells that are
+                # no node hold 0 in each pair's map: NODATA once log-transformed)
+                npost = float(len(plan.batched))
+                cum, mx = factor.read_currents(want_max=True)
+                cmap = _scatter(cum.astype(np.float64), nodemap)
+                off = nodemap == 0
+                if o.log_transform_maps:
+                    cmap = np.where(off, NODATA * npost, cmap)
+                if o.set_null_currents_to_nodata:
+                    cmap = np.where(cellmap == 0, NODATA * npost, cmap)
+                out.cum_curmap += cmap
+                if out.max_curmap is not None:
+                    mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, _scatter(mx.astype(np.float64), nodemap))
+                    if o.set_null_currents_to_nodata:
+                        mmap = np.where(cellmap == 0, NODATA, mmap)
+                    out.max_curmap = np.maximum(out.max_curmap, mmap)
+    rr, cc_, ids = points_rc
+    for i, j in plan.per_pair:                                   # the reference's own algorithm
+        p1, p2 = pts[i], pts[j]
+        newpoly = graph.create_pair_polymap(cellmap, polymap, points_rc, p1, p2)
+        nm = graph.construct_node_map(cellmap, newpoly)
+        G = graph.laplacian(graph.construct_graph(cellmap, nm, avg_res, four_neighbors))
+        x = int(np.nonzero(ids == p1)[0][0])
+        y = int(np.nonzero(ids == p2)[0][0])
+        pn = np.array([nm[rr[x] - 1, cc_[x] - 1], nm[rr[y] - 1, cc_[y] - 1]])
+        r = single_ground_all_pairs(GraphProblem(G, graph.connected_components(G), pn, np.array([p1, p2]), set(),
+                                                 nm, newpoly, cellmap, solver), flags, sink=sink)
+        R[i, j] = R[j, i] = r.resistances[1, 2]
+        out.num_solves += r.num_solves
+        out.iterations += r.iterations
+        out.voltmaps.update(r.voltmaps)
+        out.curmaps.update(r.curmaps)
+        out.cum_curmap += r.cum_curmap
+        if out.max_curmap is not None:
+            out.max_curmap = np.maximum(out.max_curmap, r.max_curmap)
+    np.fill_diagonal(R, 0.0)
+    full = np.zeros((P + 1, P + 1))
+    full[0, 1:] = pts
+    full[1:, 0] = pts
+    full[1:, 1:] = R
+    out.resistances = full
+    # every pair's map goes into one shared cumulative map, clamped once when it is written
+    # (write_cum_maps -> postprocess_cum_curmap!, src/out.jl:467-479, src/utils.jl:114-120): a cell that
+    # is NODATA in every pair's map stays NODATA instead of adding up to -9999 * pairs
+    out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
+    if out.max_curmap is not None:
+        out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
+    return out
+
+
 def _one_to_all_batched_raster(G, comps, nodemap, newpoly, point_map, unique_point_map, uniq, rr, cc_,
                                strengths, solver):
     """One-to-all without include/exclude lists: iteration p puts a current source on focal node p and

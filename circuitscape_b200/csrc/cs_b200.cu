@@ -126,6 +126,14 @@ struct cs_b200_handle {
   cs_b200_opts opts{};
   cs_b200_stats stats{};
   GraphSlot graphs[4];  // KT = 1,2,4,8
+  // cs_b200_solve_region_pairs: the panel's Dirichlet sets as 2*KT row segments (kernels.cuh k_seg_set).
+  // Region panels mask AP and Z inside the PCG loop, so they get graph slots of their own; those graphs
+  // capture d_rg_seg / d_rg_rows and are dropped whenever the buffers are reallocated.
+  bool rg_on = false;                // the panel being solved is a region panel
+  int* d_rg_seg = nullptr;
+  int* d_rg_rows = nullptr;
+  size_t rg_cap = 0;
+  GraphSlot rgraphs[4];
   // optional per-launch SpMM timing (cs_b200_profile_spmm): event pairs harvested at
   // every host poll, so the pool only has to cover one chunk of iterations.
   int profile = 0;
@@ -1062,11 +1070,40 @@ void launch_vcycle(cs_b200_handle* h, bool level0_presmoothed) {
   }
 }
 
+// region panels: zero the set rows of a panel (Dirichlet mask), or set the set_b rows to v
+template <typename T, int KT>
+void launch_seg_set(cs_b200_handle* h, void* panel, int set_b_only, T v) {
+  k_seg_set<T, KT><<<2 * KT, NT, 0, h->stream>>>((T*)panel, h->d_rg_seg, h->d_rg_rows, set_b_only, v);
+  h->stats.kernel_launches++;
+}
+
+// z = mask M^-1 mask r on a region panel (r is zero on the sets already)
+template <typename T, int KT>
+void mask_z(cs_b200_handle* h) {
+  if (!h->rg_on) return;
+  if (h->mixed) launch_seg_set<float, KT>(h, h->Z32, 0, 0.0f);
+  else launch_seg_set<T, KT>(h, h->Z, 0, T(0));
+}
+
+inline GraphSlot& graph_slot(cs_b200_handle* h, int kt) {
+  return (h->rg_on ? h->rgraphs : h->graphs)[kt_index(kt)];
+}
+
+void drop_graphs(GraphSlot* slots) {
+  for (int i = 0; i < 4; ++i) {
+    if (slots[i].exec) cudaGraphExecDestroy(slots[i].exec);
+    if (slots[i].loop_exec) cudaGraphExecDestroy(slots[i].loop_exec);
+    slots[i] = GraphSlot{};
+  }
+}
+
 template <typename T, int KT>
 void launch_iteration(cs_b200_handle* h) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int g = ew_grid<T, KT>(h);
   launch_spmm<T, KT, SP_CG>(h, (const T*)h->P, (T*)h->AP, nullptr);
+  // region panel: r stays zero on the sets (p is zero there, so p.Ap needs no mask)
+  if (h->rg_on) launch_seg_set<T, KT>(h, h->AP, 0, T(0));
   if (!h->amg) {
     k_cg_update_r<T, KT><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
                                                   (T*)h->R, h->d_ctl, h->d_partials);
@@ -1082,6 +1119,7 @@ void launch_iteration(cs_b200_handle* h) {
                                                             implicit_x0(h->lv32[0]) ? nullptr : (float*)h->X32,
                                                             (float*)h->R32, h->d_ctl);
       launch_vcycle<T, KT>(h, true);
+      mask_z<T, KT>(h);
       k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
                                                              h->d_ctl);
     } else {
@@ -1090,6 +1128,7 @@ void launch_iteration(cs_b200_handle* h) {
                                                         implicit_x0(h->lv[0]) ? nullptr : (T*)h->stage, nullptr,
                                                         h->d_ctl);
       launch_vcycle<T, KT>(h, true);
+      mask_z<T, KT>(h);
       k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
     h->stats.kernel_launches += 2;
@@ -1098,7 +1137,7 @@ void launch_iteration(cs_b200_handle* h) {
 
 template <typename T, int KT>
 int run_chunk(cs_b200_handle* h, int chunk) {
-  GraphSlot& gs = h->graphs[kt_index(KT)];
+  GraphSlot& gs = graph_slot(h, KT);
   if (h->opts.use_graph > 0 && !h->profile) {   // use_graph == 2: host-polled chunks
     if (!gs.exec || gs.chunk != chunk) {
       if (gs.exec) cudaGraphExecDestroy(gs.exec);
@@ -1132,7 +1171,7 @@ int run_chunk(cs_b200_handle* h, int chunk) {
 // clear ctl->nactive; itmax bounds the loop), the host neither polls nor re-launches.
 template <typename T, int KT>
 int run_loop(cs_b200_handle* h) {
-  GraphSlot& gs = h->graphs[kt_index(KT)];
+  GraphSlot& gs = graph_slot(h, KT);
   if (!gs.loop_exec) {
     cudaGraph_t graph;
     CK(h, cudaGraphCreate(&graph, 0));
@@ -1198,11 +1237,13 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     if (h->mixed) {
       k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
       launch_vcycle<T, KT>(h, false);
+      mask_z<T, KT>(h);
       k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
                                                              h->d_ctl);
       h->stats.kernel_launches++;
     } else {
       launch_vcycle<T, KT>(h, false);
+      mask_z<T, KT>(h);
       k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
     h->stats.kernel_launches += 2;
@@ -1219,7 +1260,7 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     CK(h, cudaStreamSynchronize(h->stream));
     if (h->profile) harvest_profile(h);
     if (device_loop) {
-      GraphSlot& gs = h->graphs[kt_index(KT)];
+      GraphSlot& gs = graph_slot(h, KT);
       h->stats.kernel_launches += 1 + gs.loop_kernels * h->h_ctl->iter;
       h->stats.spmm_launches += gs.loop_spmms * h->h_ctl->iter;
       break;
@@ -1229,7 +1270,15 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     if (rc) return rc;
   }
   // true residual  AP = B - A X  (core.jl:640, 648-651)
-  launch_spmm<T, KT, 2>(h, (const T*)h->X, (T*)h->AP, (const T*)h->B);
+  if (h->rg_on) {
+    // masked system: the set rows of B - A X hold the flux, not a residual -> zero them, then the norms
+    launch_spmm<T, KT, SP_RES>(h, (const T*)h->X, (T*)h->AP, (const T*)h->B);
+    launch_seg_set<T, KT>(h, h->AP, 0, T(0));
+    k_resnorm<T, KT><<<g, NT, 0, h->stream>>>(nelem, (size_t)h->n * KT, (const T*)h->AP, (const T*)h->B, h->d_ctl, h->d_partials);
+    h->stats.kernel_launches++;
+  } else {
+    launch_spmm<T, KT, 2>(h, (const T*)h->X, (T*)h->AP, (const T*)h->B);
+  }
   CK(h, cudaGetLastError());
   CK(h, cudaEventRecord(h->ev3, h->stream));
   CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
@@ -1618,6 +1667,127 @@ int solve_pairs_t(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_
   return CS_B200_OK;
 }
 
+// ---- focal-region pairs (cs_b200_solve_region_pairs) ----------------------------------------
+// Column c: L w = 0 off the sets, w = 0 on set_a and set_b, right-hand side -L 1_b, so u = w + 1_b
+// holds set_a at 0 V and set_b at 1 V.  flux = u.L u ; v = u / flux ; R = 1 / flux.
+template <typename T, int KT>
+int region_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const int64_t* set_rows,
+                 const int64_t* set_a, const int64_t* set_b, const double* weight, double rtol,
+                 int64_t itmax, T* R, T* volt, T* curr, int accumulate, int64_t* iters, double* relres,
+                 bool* any_fail, bool* any_maxit, std::string* msg) {
+  const size_t nelem = (size_t)h->n_pad * KT;
+  const int g = ew_grid<T, KT>(h);
+  PanelCtl* hc = h->h_ctl;
+  std::memset(hc, 0, sizeof(PanelCtl));
+  int seg[2 * MAXKT + 1];
+  std::vector<int> rows;
+  seg[0] = 0;
+  for (int c = 0; c < KT; ++c) {
+    hc->src[c] = hc->dst[c] = -1;
+    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
+    for (int side = 0; side < 2; ++side) {
+      const int64_t s = side ? set_b[c0 + c] : set_a[c0 + c];
+      for (int64_t e = set_ptr[s]; e < set_ptr[s + 1]; ++e) rows.push_back((int)set_rows[e]);
+      seg[2 * c + side + 1] = (int)rows.size();
+    }
+  }
+  if (!h->d_rg_seg) CK(h, cudaMalloc(&h->d_rg_seg, (2 * MAXKT + 1) * sizeof(int)));
+  if (rows.size() > h->rg_cap) {
+    CK(h, cudaStreamSynchronize(h->stream));
+    drop_graphs(h->rgraphs);                 // they captured the old address
+    cudaFree(h->d_rg_rows);
+    h->d_rg_rows = nullptr;
+    h->rg_cap = std::max<size_t>(rows.size(), 4096);
+    CK(h, cudaMalloc(&h->d_rg_rows, h->rg_cap * sizeof(int)));
+  }
+  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
+  CK(h, h2d(h, h->d_rg_seg, seg, (2 * KT + 1) * sizeof(int)));
+  CK(h, h2d(h, h->d_rg_rows, rows.data(), rows.size() * sizeof(int)));
+  h->stats.h2d_bytes += sizeof(PanelCtl) + (2.0 * KT + 1 + rows.size()) * sizeof(int);
+  // B = -L 1_b, zero on the sets (and on the pad rows, which the SpMM does not write)
+  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
+  CK(h, cudaMemsetAsync(h->X, 0, nelem * sizeof(T), h->stream));
+  launch_seg_set<T, KT>(h, h->X, 1, T(-1));
+  launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->B, nullptr);
+  launch_seg_set<T, KT>(h, h->B, 0, T(0));
+  h->rg_on = true;
+  int rc = solve_panel<T, KT>(h, rtol, itmax);
+  h->rg_on = false;
+  if (rc) return rc;
+  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  // u = w + 1_b (w is zero on the sets); flux = u.L u, second order in the error of w
+  launch_seg_set<T, KT>(h, h->X, 1, T(1));
+  launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->AP, nullptr);
+  k_flux<T, KT><<<g, NT, 0, h->stream>>>(nelem, (size_t)h->n * KT, (const T*)h->X, (const T*)h->AP, h->d_ctl, h->d_partials);
+  h->stats.kernel_launches++;
+  CK(h, cudaGetLastError());
+  CK(h, cudaMemcpyAsync(hc, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  h->stats.d2h_bytes += sizeof(PanelCtl);
+  for (int c = 0; c < KT; ++c) {
+    const double flux = hc->xdst[c];
+    if (!(flux > 0.0))
+      return set_err(h, CS_B200_ERR_ARG, "region pair %lld: flux into set_b is %g (no conducting path to set_a)",
+                     (long long)(c0 + c), flux);
+    R[c0 + c] = (T)(1.0 / flux);
+  }
+  k_scale_flux<T, KT><<<g, NT, 0, h->stream>>>(nelem, (T*)h->X, h->d_ctl);
+  h->stats.kernel_launches++;
+  if (accumulate || curr) {
+    launch_currents<T, KT>(h, true, 0);
+    k_seg_current<T, KT><<<2 * KT, NT, 0, h->stream>>>((T*)h->AP, h->d_rg_seg, h->d_rg_rows);
+    h->stats.kernel_launches++;
+    if (accumulate) {
+      const int ag = (int)std::max<int64_t>(1, std::min<int64_t>(h->grid_ew, (h->n + NT - 1) / NT));
+      k_cur_accum<T, KT><<<ag, NT, 0, h->stream>>>((int)h->n, (const T*)h->AP, h->d_ctl, (T*)h->d_cum,
+                                                   (T*)h->d_max, h->opts.log_transform);
+      h->stats.kernel_launches++;
+    }
+  }
+  CK(h, cudaGetLastError());
+  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  if (curr) {
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
+                                                    (T*)h->stage, h->d_ctl, 0);
+    h->stats.kernel_launches++;
+    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
+  }
+  if (volt) {
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
+                                                    (T*)h->stage, h->d_ctl, 0);
+    h->stats.kernel_launches++;
+    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
+  }
+  CK(h, cudaStreamSynchronize(h->stream));
+  return CS_B200_OK;
+}
+
+template <typename T>
+int solve_region_pairs_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_t* set_rows, int64_t k,
+                         const int64_t* set_a, const int64_t* set_b, const double* weight, double rtol,
+                         int64_t itmax, T* R, T* volt, T* curr, int accumulate, int64_t* iters,
+                         double* relres) {
+  bool any_fail = false, any_maxit = false;
+  std::string msg;
+  int64_t c0 = 0;
+  while (c0 < k) {
+    const int kt = next_kt(k - c0, h->ktmax);
+    int rc = 0;
+    DISPATCH_KT(kt, (rc = region_panel<T, KT>(h, c0, set_ptr, set_rows, set_a, set_b, weight, rtol, itmax, R,
+                                              volt, curr, accumulate, iters, relres, &any_fail, &any_maxit,
+                                              &msg)));
+    if (rc) return rc;
+    c0 += kt;
+  }
+  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
+  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
+  return CS_B200_OK;
+}
+
 template <typename T>
 int solve_sources_t(cs_b200_handle* h, int64_t k, const int64_t* colptr, const int64_t* rows,
                     const double* vals, const int64_t* ref, const double* weight, double rtol,
@@ -1841,11 +2011,8 @@ __global__ void k_apply_grounds(int n, const int* __restrict__ rowptr, const int
 // and the panels stay.
 static void teardown_operators(cs_b200_handle* h) {
   if (h->stream) cudaStreamSynchronize(h->stream);
-  for (auto& g : h->graphs) {
-    if (g.exec) cudaGraphExecDestroy(g.exec);
-    if (g.loop_exec) cudaGraphExecDestroy(g.loop_exec);
-    g = GraphSlot{};
-  }
+  drop_graphs(h->graphs);
+  drop_graphs(h->rgraphs);
   free_win(h->A0);
   h->A0.has_dinv = 0; h->A0.win_blocks = 0; h->A0.win_nblocks = 0; h->A0.dia_nr = 0; h->A0.dia_ld = 0;
   for (size_t l = 0; l < h->lv.size(); ++l) {
@@ -1908,7 +2075,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1003; }
+int cs_b200_version(void) { return 1004; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2337,6 +2504,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
   cudaFree(h->d_sp_rows); cudaFree(h->d_sp_vals); cudaFree(h->d_sp_ptr);
   cudaFree(h->d_probe); cudaFree(h->d_probe_out);
+  cudaFree(h->d_rg_seg); cudaFree(h->d_rg_rows);
   for (int i = 0; i < 2; ++i) {
     cudaFree(h->io_in[i]); cudaFree(h->io_out[i]);
     cudaEvent_t evs[] = {h->ev_in[i], h->ev_used[i], h->ev_ready[i], h->ev_out[i]};
@@ -2654,6 +2822,50 @@ int cs_b200_solve_pairs_superposed(cs_b200_handle* h, int64_t np, const int64_t*
                                                   (double*)volt, (double*)curr, accumulate, point_iters, relres)
                : solve_pairs_superposed_t<float>(h, np, nodes, k, pi, pj, weight, rtol, itmax, (float*)R,
                                                  (float*)volt, (float*)curr, accumulate, point_iters, relres);
+  end_call(h);
+  return rc;
+}
+
+int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
+                               const int64_t* set_rows, int64_t k, const int64_t* set_a,
+                               const int64_t* set_b, const double* weight, double rtol, int64_t itmax,
+                               void* R, void* volt, void* curr, int accumulate,
+                               int64_t* iters, double* relres) {
+  // the sets are checked before the handle so that malformed input is reported the same way with or
+  // without a device; row ranges need the handle's n
+  if (k < 1 || nsets < 1 || !set_ptr || !set_rows || !set_a || !set_b || !R || !(rtol >= 0) || itmax < 0)
+    return set_err(h, CS_B200_ERR_ARG, "bad solve_region_pairs arguments");
+  if (set_ptr[0] != 0) return set_err(h, CS_B200_ERR_ARG, "set_ptr[0] must be 0");
+  for (int64_t s = 0; s < nsets; ++s) {
+    if (set_ptr[s + 1] <= set_ptr[s]) return set_err(h, CS_B200_ERR_ARG, "set %lld is empty", (long long)s);
+    for (int64_t e = set_ptr[s]; e < set_ptr[s + 1]; ++e) {
+      if (set_rows[e] < 0 || (h && set_rows[e] >= h->n) || set_rows[e] > INT32_MAX)
+        return set_err(h, CS_B200_ERR_ARG, "set %lld: row %lld out of range", (long long)s, (long long)set_rows[e]);
+      if (e > set_ptr[s] && set_rows[e] <= set_rows[e - 1])
+        return set_err(h, CS_B200_ERR_ARG, "set %lld: rows not sorted and unique", (long long)s);
+    }
+  }
+  for (int64_t c = 0; c < k; ++c) {
+    const int64_t a = set_a[c], b = set_b[c];
+    if (a < 0 || a >= nsets || b < 0 || b >= nsets)
+      return set_err(h, CS_B200_ERR_ARG, "column %lld: set index out of range (%lld, %lld)", (long long)c,
+                     (long long)a, (long long)b);
+    // sorted merge: the two sets of a column must not share a row
+    int64_t i = set_ptr[a], j = set_ptr[b];
+    while (i < set_ptr[a + 1] && j < set_ptr[b + 1]) {
+      if (set_rows[i] == set_rows[j])
+        return set_err(h, CS_B200_ERR_ARG, "column %lld: sets %lld and %lld overlap at row %lld", (long long)c,
+                       (long long)a, (long long)b, (long long)set_rows[i]);
+      if (set_rows[i] < set_rows[j]) ++i; else ++j;
+    }
+  }
+  if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
+  begin_call(h);
+  int rc = h->dtype == CS_B200_F64
+               ? solve_region_pairs_t<double>(h, set_ptr, set_rows, k, set_a, set_b, weight, rtol, itmax,
+                                              (double*)R, (double*)volt, (double*)curr, accumulate, iters, relres)
+               : solve_region_pairs_t<float>(h, set_ptr, set_rows, k, set_a, set_b, weight, rtol, itmax,
+                                             (float*)R, (float*)volt, (float*)curr, accumulate, iters, relres);
   end_call(h);
   return rc;
 }

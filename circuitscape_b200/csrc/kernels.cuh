@@ -1900,4 +1900,127 @@ __global__ void k_flush(float* p, size_t n) {
     p[i] = p[i] * 1.0001f + 1.0f;
 }
 
+// ---------------------------------------------------------------------------
+// focal-region pairs (cs_b200_solve_region_pairs).  A panel's Dirichlet sets are 2*KT row
+// segments of `rows`: segment 2c is set_a of column c (0 V), segment 2c+1 its set_b (1 V);
+// seg[] holds the 2*KT+1 offsets.  The segment kernels run one CTA per segment; the sets of
+// one column are disjoint, so no two threads write the same element.
+// ---------------------------------------------------------------------------
+// P[row][s/2] = v for the rows of every segment s (set_b_only = 0) or of the set_b segments only
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_seg_set(T* __restrict__ P, const int* __restrict__ seg, const int* __restrict__ rows, int set_b_only, T v) {
+  const int s = blockIdx.x;
+  if (set_b_only && !(s & 1)) return;
+  const int c = s >> 1;
+  for (int e = seg[s] + threadIdx.x; e < seg[s + 1]; e += NT) P[(size_t)rows[e] * KT + c] = v;
+}
+
+// every row of a set takes its merged node's current.  The set is equipotential, so its internal
+// edges carry nothing and each of its rows only sends (set_b, the highest voltage) or only receives
+// (set_a, the lowest): the merged node's max(inflow, outflow) is the sum of the rows' currents.
+// Fixed-order sum: strided per thread, then a shared-memory tree.
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_seg_current(T* __restrict__ C, const int* __restrict__ seg, const int* __restrict__ rows) {
+  __shared__ double s_sum[NT];
+  const int s = blockIdx.x, c = s >> 1, tid = threadIdx.x;
+  double a = 0.0;
+  for (int e = seg[s] + tid; e < seg[s + 1]; e += NT) a += (double)C[(size_t)rows[e] * KT + c];
+  s_sum[tid] = a;
+  __syncthreads();
+  for (int w = NT / 2; w > 0; w >>= 1) {
+    if (tid < w) s_sum[tid] += s_sum[tid + w];
+    __syncthreads();
+  }
+  const T tot = (T)s_sum[0];
+  for (int e = seg[s] + tid; e < seg[s + 1]; e += NT) C[(size_t)rows[e] * KT + c] = tot;
+}
+
+// true-residual gate of a masked panel:  resid[c] = ||Y[:,c]||^2 , bnorm[c] = ||B[:,c]||^2
+// (Y = B - A X with the set rows zeroed, B zero there already).  Only the first nvalid = n*KT elements
+// count: the SpMM leaves the pad rows of Y as an earlier, wider panel wrote them.
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_resnorm(size_t nelem, size_t nvalid, const T* __restrict__ Y, const T* __restrict__ B, PanelCtl* ctl,
+          double* partials) {
+  constexpr int VEC = Vec<T>::N;
+  CSB_REDUCE_SMEM(2, KT)
+  const size_t stride = (size_t)gridDim.x * NT * VEC;
+  double acc[2][VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) acc[0][i] = acc[1][i] = 0.0;
+  for (size_t e = ((size_t)blockIdx.x * NT + threadIdx.x) * VEC; e < nelem; e += stride) {
+    T y[VEC], b[VEC];
+    vload(Y + e, y);
+    vload(B + e, b);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) {
+      if (e + i >= nvalid) continue;
+      acc[0][i] += (double)y[i] * (double)y[i];
+      acc[1][i] += (double)b[i] * (double)b[i];
+    }
+  }
+  if (grid_reduce<KT, VEC, 2, false>(acc, partials, &ctl->ticket, s_warp, s_tree, s_out)) {
+    if (threadIdx.x < KT) {
+      ctl->resid[threadIdx.x] = s_out[threadIdx.x];
+      ctl->bnorm[threadIdx.x] = s_out[KT + threadIdx.x];
+    }
+  }
+}
+
+// flux into set_b of every column:  xdst[c] = u[:,c] . (A u)[:,c]  over the first nvalid = n*KT elements
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_flux(size_t nelem, size_t nvalid, const T* __restrict__ U, const T* __restrict__ AU, PanelCtl* ctl,
+       double* partials) {
+  constexpr int VEC = Vec<T>::N;
+  CSB_REDUCE_SMEM(1, KT)
+  const size_t stride = (size_t)gridDim.x * NT * VEC;
+  double acc[1][VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) acc[0][i] = 0.0;
+  for (size_t e = ((size_t)blockIdx.x * NT + threadIdx.x) * VEC; e < nelem; e += stride) {
+    T u[VEC], y[VEC];
+    vload(U + e, u);
+    vload(AU + e, y);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i)
+      if (e + i < nvalid) acc[0][i] += (double)u[i] * (double)y[i];
+  }
+  if (grid_reduce<KT, VEC, 1, false>(acc, partials, &ctl->ticket, s_warp, s_tree, s_out))
+    if (threadIdx.x < KT) ctl->xdst[threadIdx.x] = s_out[threadIdx.x];
+}
+
+// X[:,c] /= flux[c]  (the reference's 1 A normalisation)
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_scale_flux(size_t nelem, T* __restrict__ X, const PanelCtl* __restrict__ ctl) {
+  for (size_t e = (size_t)blockIdx.x * NT + threadIdx.x; e < nelem; e += (size_t)gridDim.x * NT)
+    X[e] = (T)((double)X[e] / ctl->xdst[e % KT]);
+}
+
+// cum += sum_c weight[c] f(C[:,c]) and max = max(max, f(C[:,c])) in column order, f = log10 when
+// log_transform (out.jl:100-107, 305-309) -- the accumulation of k_cur_acc, run after the set fix-up
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_cur_accum(int n, const T* __restrict__ C, const PanelCtl* __restrict__ ctl, T* __restrict__ cum,
+            T* __restrict__ mx, int log_transform) {
+  for (int row = blockIdx.x * NT + threadIdx.x; row < n; row += gridDim.x * NT) {
+    double s = 0.0;
+    T m = T(-1.0e30);
+#pragma unroll
+    for (int c = 0; c < KT; ++c) {
+      const double w = ctl->weight[c];
+      if (w == 0.0) continue;
+      const T cur = C[(size_t)row * KT + c];
+      const T val = log_transform ? (cur > T(0) ? (T)log10((double)cur) : T(-9999)) : cur;
+      s += w * (double)val;
+      m = val > m ? val : m;
+    }
+    cum[row] = (T)((double)cum[row] + s);
+    if (mx) mx[row] = m > mx[row] ? m : mx[row];
+  }
+}
+
 }  // namespace csb

@@ -64,6 +64,70 @@ def create_new_polymap(gmap, polymap, points_rc, point_map):
     return newpoly
 
 
+class RegionPolymapError(ValueError):
+    """A focal region touches exactly one user polygon among several points: the reference reads an
+    undefined variable on that branch (src/raster/pairwise.jl:428-430) and stops with UndefVarError."""
+
+
+def region_relabel(polymap, points_rc, pt):
+    """The cells the pairwise polygon map relabels for focal id `pt` (src/raster/pairwise.jl:404-436,
+    with a polygon map): None when the id keeps the map as it is (one point), else a boolean mask.
+    Raises RegionPolymapError on the reference's error branch."""
+    rr, cc, ids = points_rc
+    idx = np.nonzero(np.asarray(ids) == pt)[0]
+    if len(idx) == 1:
+        return None
+    vals_at = polymap[rr[idx] - 1, cc[idx] - 1]
+    if np.all(vals_at == 0):
+        mask = np.zeros(polymap.shape, dtype=bool)
+        mask[rr[idx] - 1, cc[idx] - 1] = True
+        return mask
+    nz = idx[vals_at != 0]
+    if len(nz) == 1:
+        raise RegionPolymapError(f"focal region {pt} touches exactly one polygon cell among its points; "
+                                 "the reference raises UndefVarError here")
+    return np.isin(polymap, polymap[rr[nz] - 1, cc[nz] - 1])
+
+
+def create_pair_polymap(gmap, polymap, points_rc, pt1, pt2):
+    """Polygon map of one focal-region pair (pairwise mode, src/raster/pairwise.jl:369-442): without
+    user polygons the cells of pt1 and pt2 become polygons labelled by their ids; with them, an id whose
+    points all lie outside polygons becomes a new polygon, and an id touching several polygon cells
+    merges every polygon it touches into a new one (pt2 after pt1, so pt2 wins where they overlap)."""
+    rr, cc, ids = points_rc
+    if polymap is None or np.size(polymap) == 0:
+        newpoly = np.zeros(np.shape(gmap), dtype=np.int64)
+        for p in (pt1, pt2):
+            sel = np.asarray(ids) == p
+            newpoly[rr[sel] - 1, cc[sel] - 1] = p
+        return newpoly
+    polymap = np.asarray(polymap)
+    newpoly = np.array(polymap, dtype=np.int64)
+    k = int(polymap.max())
+    for p in (pt1, pt2):
+        mask = region_relabel(polymap, points_rc, p)
+        if mask is not None:
+            k += 1
+            newpoly[mask] = k
+    return newpoly
+
+
+def generate_exclude_pairs(points_rc, inc):
+    """src/raster/pairwise.jl:240-269: the id pairs an include / exclude list leaves out.  An include
+    list also drops the points whose id it does not name.  Returns (points_rc, exclude set)."""
+    ex = set()
+    ids, mat = np.asarray(inc.point_ids), np.asarray(inc.mat)
+    if inc.mode == "include":
+        keep = np.isin(points_rc[2], ids)
+        points_rc = tuple(np.asarray(a)[keep] for a in points_rc)
+        hit = (mat == 0) & (mat.T == 0)
+    else:
+        hit = (mat == 1) & (mat.T == 1)
+    for i, j in zip(*np.nonzero(hit)):
+        ex.add((int(ids[i]), int(ids[j])))
+    return points_rc, ex
+
+
 def construct_graph(gmap, nodemap, avg_res, four_neighbors):
     """Symmetric adjacency of conductances: E, S, SE, NE neighbours, duplicates
     (parallel cell adjacencies of merged nodes) summed."""

@@ -385,6 +385,39 @@ class B200Factor:
             curr = None if curr is None else curr.astype(self.io_dtype)
         return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
 
+    def solve_region_pairs(self, sets, set_a, set_b, weight=None, want_volt=False, want_curr=False,
+                           accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
+        """Focal-region pairs on this operator (cs_b200_solve_region_pairs): column c holds the rows of
+        sets[set_a[c]] at 0 V and those of sets[set_b[c]] at 1 V, then scales to the reference's 1 A
+        normalisation.  sets: list of 0-based row arrays (sorted, unique, non-empty).  Returns the dict
+        of solve_pairs: R = 1 / flux, volt (0 on set_a, R on set_b), curr (every row of a set carries
+        its merged node's current)."""
+        ptr = np.zeros(len(sets) + 1, dtype=np.int64)
+        for s, r in enumerate(sets):
+            ptr[s + 1] = ptr[s] + len(r)
+        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r in sets])
+                                    if len(sets) else np.zeros(0), dtype=np.int64)
+        set_a = np.ascontiguousarray(set_a, dtype=np.int64)
+        set_b = np.ascontiguousarray(set_b, dtype=np.int64)
+        k = len(set_a)
+        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
+        R = np.zeros(k, dtype=self.dtype)
+        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
+        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
+        iters = np.zeros(k, dtype=np.int64)
+        relres = np.zeros(k, dtype=np.float64)
+        rc = self._lib.cs_b200_solve_region_pairs(
+            self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(set_a), _lib._ptr(set_b),
+            _lib._ptr(w), self.solver.rtol if rtol is None else rtol,
+            self.solver.itmax if itmax is None else itmax, _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr),
+            1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+        self._raise(rc, raise_on_residual)
+        if self.io_dtype != self.dtype:
+            R = R.astype(self.io_dtype)
+            volt = None if volt is None else volt.astype(self.io_dtype)
+            curr = None if curr is None else curr.astype(self.io_dtype)
+        return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
+
     def solve_sources(self, columns, ref, probe=None, weight=None, want_volt=False, want_curr=False,
                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
         """Batched solve with sparse right-hand sides, device-resident
@@ -491,6 +524,15 @@ def solve_advanced_batch(g, src, gnd, four_neighbors, device, rtol, itmax, want_
 def construct_cholesky_factor(matrix, solver: CUDASolver, **kw) -> B200Factor:
     """Hook #1 (src/core.jl:379,519-523): once per connected component."""
     return B200Factor(matrix, solver, **kw)
+
+
+def construct_raster_factor(cellmap, polymap, solver: CUDASolver, four_neighbors=False, avg_res=False,
+                            log_transform=False):
+    """The whole-raster operator of a focal-region job and its node map (1-based, 0 = none):
+    B200Factor.from_raster_polygons.  Not one of the three hooks: the region-pair driver needs the
+    handle's cs_b200_solve_region_pairs, which the Solver interface has no method for."""
+    return B200Factor.from_raster_polygons(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                           avg_res=avg_res, log_transform=log_transform)
 
 
 def solve_linear_system(factor: B200Factor, matrix, rhs):

@@ -232,6 +232,20 @@ int cs_b200_solve_pairs_superposed(cs_b200_handle* h, int64_t np, const int64_t*
                                    double rtol, int64_t itmax, void* R, void* volt, void* curr,
                                    int accumulate, int64_t* point_iters, double* relres);
 
+/* Pairwise mode with focal regions (src/raster/pairwise.jl:72-135) on ONE resident operator: column c holds
+ * set_a[c] at 0 V and set_b[c] at 1 V (Dirichlet), solves the interior, R[c] = 1 / flux into set_b[c],
+ * voltages scaled to the reference's 1 A normalisation (0 on set_a, R on set_b).  Sets: CSR over 0-based rows
+ * (set_ptr[nsets+1], set_rows), each non-empty, sorted, unique; the two sets of a column disjoint.
+ * weight / volt / curr / accumulate / iters / relres as cs_b200_solve_pairs; curr and the accumulated maps
+ * give every row of a set its merged-node current.
+ * Bad or overlapping sets, out-of-range rows or set indices and k <= 0 give CS_B200_ERR_ARG before any
+ * device work; so does a column whose flux comes out <= 0 (a pair with no conducting path).            */
+int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
+                               const int64_t* set_rows, int64_t k, const int64_t* set_a,
+                               const int64_t* set_b, const double* weight, double rtol, int64_t itmax,
+                               void* R, void* volt, void* curr, int accumulate,
+                               int64_t* iters, double* relres);
+
 /* Batched solve with SPARSE right-hand sides, device-resident -- the advanced-mode kernel
  * (src/raster/advanced.jl:274-305) for source/ground sets without finite grounds, and
  * the all-to-one loop built on it (src/raster/onetoall.jl:110-118,146-151):
