@@ -1,6 +1,10 @@
 """Float64 references of the operations the CUDA kernels implement, in plain numpy / scipy.
 
     vcycle(levels, r)             the Jacobi-smoothed V(1,1) cycle the device runs as its preconditioner
+    pcg(A, B, precond, rtol, itmax)
+                                  the device's PCG recurrence, column by column: deferred x update, stop
+                                  test, stall guard and per-column freezing (csrc/kernels.cuh
+                                  cg_after_precond, k_cg_*)
     true_relres(A, X, B)          ||B - A X|| / ||B|| per column (the reference's residual gate,
                                   src/core.jl:640-650)
     node_currents(A, v)           per-node currents with the 1e-8 relative zeroing (src/out.jl:178-290)
@@ -54,6 +58,81 @@ def _vcycle(levels, pinv, b, l):
     x = om * dinv * b
     x = x + L["P"] @ _vcycle(levels, pinv, L["R"] @ (b - A @ x), l + 1)
     return x + om * dinv * (b - A @ x)
+
+
+ATOL = float(np.sqrt(np.finfo(np.float64).eps))     # the device's default absolute tolerance
+
+
+def _coldots(U, V):
+    """r.z per column, each column its own contiguous fp64 dot (a column's value does not depend on
+    the other columns of the panel)."""
+    return np.array([np.dot(U[:, c].astype(np.float64), V[:, c].astype(np.float64))
+                     for c in range(U.shape[1])])
+
+
+def pcg(A, B, precond, rtol, itmax, atol=ATOL, stall_limit=40, dtype=np.float64):
+    """The device's preconditioned CG recurrence for B of shape (n,) or (n, k), column by column
+    (csrc/kernels.cuh cg_after_precond, k_cg_init / k_cg_update_r / k_cg_update_xp, k_cg_update_r0 /
+    k_cg_update_xp2, the SP_CG epilogue):
+
+        x = 0, r = b, z = M^-1 r, p = z, rho0 = |r.z|, tol = atol + rtol sqrt(rho0)
+        active  <=>  rho0 > 0 and sqrt(rho0) > tol and itmax > 0
+        per iteration of an active column:
+            alpha = rho / p.Ap  (0 if p.Ap <= 0) ;  r -= alpha Ap ;  z = M^-1 r ;  rho' = |r.z|
+            beta = rho' / rho ;  stall guard: rho' < 0.81 best resets the counter, `stall_limit`
+            iterations without that freeze the column ;  stop: !(sqrt(rho') > tol) or it >= itmax
+            x += alpha p  (the deferred update runs on the stopping iteration too) ;  p = z + beta p
+        a frozen column is never touched again.
+
+    `precond(R)` maps an (n, j) panel to M^-1 R (Jacobi: D^-1 R, whose r.z is the device's r.D^-1 r).
+    `dtype` is the storage type of x, r, p, z and A p; alpha, beta and the dots stay fp64, as on the
+    device.  The device's AMG path uses stall_limit = 40, its Jacobi path 2000.
+
+    Returns (X (n, k), iters (k,), rho (iterations + 1, k), tol (k,)): rho[j, c] is column c's rho
+    after iteration j (rho0 at j = 0), NaN where the column had already stopped."""
+    dtype = np.dtype(dtype)
+    B = np.asarray(B, dtype=dtype)
+    B = B.reshape(B.shape[0], -1)
+    n, k = B.shape
+    X = np.zeros((n, k), dtype=dtype)
+    R = B.copy()
+    Z = np.asarray(precond(R), dtype=dtype).reshape(n, k)
+    P = Z.copy()
+    rho = np.abs(_coldots(R, Z))
+    tol = atol + rtol * np.sqrt(rho)
+    active = (rho > 0) & (np.sqrt(rho) > tol) & (itmax > 0)
+    iters = np.zeros(k, dtype=np.int64)
+    best, stall = rho.copy(), np.zeros(k, dtype=np.int64)
+    hist = [rho.copy()]
+    it = 0
+    while active.any():
+        it += 1
+        c = np.nonzero(active)[0]
+        AP = np.asarray(A @ P[:, c], dtype=dtype).reshape(n, c.size)
+        pap = _coldots(P[:, c], AP)
+        alpha = np.where(pap > 0, rho[c] / np.where(pap > 0, pap, 1.0), 0.0)
+        Rc = R[:, c] - alpha.astype(dtype) * AP
+        Zc = np.asarray(precond(Rc), dtype=dtype).reshape(n, c.size)
+        rn = np.abs(_coldots(Rc, Zc))
+        beta = np.where(rho[c] > 0, rn / np.where(rho[c] > 0, rho[c], 1.0), 0.0)
+        row = np.full(k, np.nan)
+        row[c] = rn
+        hist.append(row)
+        for j, col in enumerate(c):
+            iters[col] = it
+            if rn[j] < 0.81 * best[col]:
+                best[col], stall[col] = rn[j], 0
+            else:
+                stall[col] += 1
+                if stall_limit > 0 and stall[col] >= stall_limit:
+                    active[col] = False
+            if not (np.sqrt(rn[j]) > tol[col]) or it >= itmax:
+                active[col] = False
+        rho[c] = rn
+        X[:, c] += alpha.astype(dtype) * P[:, c]
+        P[:, c] = Zc + beta.astype(dtype) * P[:, c]
+        R[:, c] = Rc
+    return X, iters, np.array(hist), tol
 
 
 def true_relres(A, X, B):
