@@ -28,6 +28,9 @@ namespace {
 
 thread_local std::string g_create_error;
 
+constexpr int PROF_CLASSES = 18;   // cs_b200_profile_classes: 9 kernel classes x (fp64, fp32)
+constexpr int PROF_CGF = 8;        // class of the fused CG step (after the 8 SpMM epilogues)
+
 struct GraphSlot {
   cudaGraphExec_t exec = nullptr;
   int chunk = 0;
@@ -88,6 +91,7 @@ struct cs_b200_handle {
   int ktmax = 8;
   void *X = nullptr, *R = nullptr, *P = nullptr, *AP = nullptr, *B = nullptr, *stage = nullptr;
   void* Z = nullptr;                 // AMG: z = M^-1 r
+  void* P2 = nullptr;                // fused CG step (k_stencil_cg): p of even iterations; P holds the odd ones
   DevCsr A0;                         // view of the finest operator (aliases d_rowptr/...)
   std::vector<DevLevel> lv;          // lv[0] = finest (A aliases A0), lv.back() = coarsest
   double* d_pinv = nullptr;          // dense pseudo-inverse of the coarsest operator
@@ -142,11 +146,12 @@ struct cs_b200_handle {
   double prof_ms = 0.0;
   double prof_bytes = 0.0;   // algorithmic bytes of the timed launches (DESIGN.md §4 formula)
   int64_t prof_launches = 0;
-  // the same per kernel class: slot = 2 * MODE + (fp32 ? 1 : 0), MODE 7 = fused prolongation + sweep
+  // the same per kernel class: slot = 2 * MODE + (fp32 ? 1 : 0), MODE 7 = fused prolongation + sweep,
+  // MODE 8 = fused CG step
   std::vector<int> prof_slot;           // one entry per event pair in flight
   std::vector<double> prof_pair_bytes;
-  double prof_slot_ms[16] = {}, prof_slot_bytes[16] = {};
-  int64_t prof_slot_launches[16] = {};
+  double prof_slot_ms[PROF_CLASSES] = {}, prof_slot_bytes[PROF_CLASSES] = {};
+  int64_t prof_slot_launches[PROF_CLASSES] = {};
   std::string err;
   size_t esize() const { return dtype == CS_B200_F64 ? 8 : 4; }
 };
@@ -749,6 +754,12 @@ int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::
   if (want_amg) {
     rc = setup_amg_device<T>(h, hp, job, dseed);
     if (rc) return rc;
+    if (h->amg && h->A0.dia && !h->P2) {   // second p panel of the fused CG step
+      const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(T);
+      cudaError_t e = cudaMalloc(&h->P2, pe);
+      if (e == cudaSuccess) e = cudaMemsetAsync(h->P2, 0, pe, h->stream);
+      if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (second p panel)", cudaGetErrorString(e));
+    }
   } else {
     csb_dev::seed_discard(job);
   }
@@ -887,7 +898,7 @@ void harvest_profile(cs_b200_handle* h) {
       h->prof_ms += ms;
       h->prof_launches++;
       if (i / 2 < h->prof_slot.size()) {
-        const int sl = h->prof_slot[i / 2] & 15;
+        const int sl = h->prof_slot[i / 2];
         h->prof_slot_ms[sl] += ms;
         h->prof_slot_bytes[sl] += h->prof_pair_bytes[i / 2];
         h->prof_slot_launches[sl]++;
@@ -1097,11 +1108,56 @@ void drop_graphs(GraphSlot* slots) {
   }
 }
 
+// AMG-PCG on a stencil-form finest level runs the fused CG step (kernels.cuh k_stencil_cg) in place of the
+// CG SpMM and k_cg_update_xp2; CS_B200_NO_FUSED_CG keeps the unfused pair for A/B runs
+inline bool fused_cg(const cs_b200_handle* h) {
+  static const bool off = std::getenv("CS_B200_NO_FUSED_CG") != nullptr;
+  return h->amg && h->A0.dia && h->P2 && !off;
+}
+
+// the z panel the CG update reads: the fp32 cycle's output on mixed handles
+template <typename T, int KT, typename TV>
+void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
+  const DevCsr& m = h->A0;
+  const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
+  constexpr int V16 = 16 / (int)sizeof(T);
+  constexpr int CGn = KT / (KT < V16 ? KT : V16);
+  const int rpp = NT / CGn;
+  const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
+                           ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
+  const int sg = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));   // = k_stencil<SP_CG>'s
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (h->profile) {
+    if (h->prof_used + 2 > h->prof_ev.size())
+      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
+    e0 = h->prof_ev[h->prof_used++];
+    e1 = h->prof_ev[h->prof_used++];
+    // 9 diagonals, Z and p_{it-1} in, AP and p_it out; X in + out and p_{it-2} in on every other step
+    const double pe = (double)m.nrows * KT * sizeof(T);
+    const double fb = (double)m.nrows * 9 * sizeof(T) + (double)m.nrows * KT * sizeof(TV) + 3.0 * pe + 1.5 * pe;
+    h->prof_bytes += fb;
+    h->prof_slot.push_back(2 * PROF_CGF + (sizeof(T) == 4 ? 1 : 0));
+    h->prof_pair_bytes.push_back(fb);
+    cudaEventRecord(e0, h->stream);
+  }
+  k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
+                                                     h->d_partials);
+  if (h->profile) cudaEventRecord(e1, h->stream);
+  h->stats.kernel_launches++;
+  h->stats.spmm_launches++;
+}
+
 template <typename T, int KT>
 void launch_iteration(cs_b200_handle* h) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int g = ew_grid<T, KT>(h);
-  launch_spmm<T, KT, SP_CG>(h, (const T*)h->P, (T*)h->AP, nullptr);
+  const bool fused = fused_cg(h);
+  if (fused) {
+    if (h->mixed) launch_stencil_cg<T, KT, float>(h, (const float*)h->Z32);
+    else launch_stencil_cg<T, KT, T>(h, (const T*)h->Z);
+  } else {
+    launch_spmm<T, KT, SP_CG>(h, (const T*)h->P, (T*)h->AP, nullptr);
+  }
   // region panel: r stays zero on the sets (p is zero there, so p.Ap needs no mask)
   if (h->rg_on) launch_seg_set<T, KT>(h, h->AP, 0, T(0));
   if (!h->amg) {
@@ -1112,7 +1168,8 @@ void launch_iteration(cs_b200_handle* h) {
     h->stats.kernel_launches += 2;
   } else {
     // r -= alpha Ap with the finest pre-smoothing folded in; V-cycle; then the deferred
-    // x += alpha p together with p = z + beta p  (9 instead of 11 panel passes)
+    // x += alpha p together with p = z + beta p  (9 instead of 11 panel passes), which the fused
+    // CG step of the next iteration does instead
     if (h->mixed) {
       k_cg_update_r0<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
                                                             (T)h->lv[0].omega, (T*)h->R,
@@ -1120,8 +1177,9 @@ void launch_iteration(cs_b200_handle* h) {
                                                             (float*)h->R32, h->d_ctl);
       launch_vcycle<T, KT>(h, true);
       mask_z<T, KT>(h);
-      k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
-                                                             h->d_ctl);
+      if (!fused)
+        k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
+                                                               h->d_ctl);
     } else {
       k_cg_update_r0<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
                                                         (T)h->lv[0].omega, (T*)h->R,
@@ -1129,10 +1187,20 @@ void launch_iteration(cs_b200_handle* h) {
                                                         h->d_ctl);
       launch_vcycle<T, KT>(h, true);
       mask_z<T, KT>(h);
-      k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
+      if (!fused)
+        k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
-    h->stats.kernel_launches += 2;
+    h->stats.kernel_launches += fused ? 1 : 2;
   }
+}
+
+// after the PCG loop: the x updates the fused CG steps left pending
+template <typename T, int KT>
+void finish_x(cs_b200_handle* h) {
+  if (!fused_cg(h)) return;
+  k_cg_x_tail<T, KT><<<ew_grid<T, KT>(h), NT, 0, h->stream>>>((size_t)h->n_pad * KT, (const T*)h->P2, (const T*)h->P,
+                                                             (T*)h->X, h->d_ctl);
+  h->stats.kernel_launches++;
 }
 
 template <typename T, int KT>
@@ -1229,7 +1297,9 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     h->stats.kernel_launches++;
   } else {
     // x = 0, p = 0, r = b ; z = M^-1 r (V-cycle; its last kernel sets rho0, tolerances,
-    // activity because ctl->init = 1) ; p = z + 0*p
+    // activity because ctl->init = 1) ; p = z + 0*p  (fused CG step: formed by the first step, which
+    // reads the zeroed P as p_{-1} with beta = 0)
+    const bool fused = fused_cg(h);
     CK(h, cudaMemsetAsync(h->X, 0, nelem * sizeof(T), h->stream));
     CK(h, cudaMemsetAsync(h->P, 0, nelem * sizeof(T), h->stream));
     CK(h, cudaMemcpyAsync(h->R, h->B, nelem * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
@@ -1238,15 +1308,17 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
       k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
       launch_vcycle<T, KT>(h, false);
       mask_z<T, KT>(h);
-      k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
-                                                             h->d_ctl);
+      if (!fused)
+        k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
+                                                               h->d_ctl);
       h->stats.kernel_launches++;
     } else {
       launch_vcycle<T, KT>(h, false);
       mask_z<T, KT>(h);
-      k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
+      if (!fused)
+        k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
-    h->stats.kernel_launches += 2;
+    h->stats.kernel_launches += fused ? 1 : 2;
   }
   CK(h, cudaGetLastError());
   const int chunk = h->amg ? std::min(h->opts.check_every, 4) : h->opts.check_every;
@@ -1269,6 +1341,7 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     int rc = run_chunk<T, KT>(h, chunk);
     if (rc) return rc;
   }
+  if (h->amg) finish_x<T, KT>(h);
   // true residual  AP = B - A X  (core.jl:640, 648-651)
   if (h->rg_on) {
     // masked system: the set rows of B - A X hold the flux, not a residual -> zero them, then the norms
@@ -2075,7 +2148,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1004; }
+int cs_b200_version(void) { return 1005; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2498,7 +2571,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   teardown_operators(h);
   if (h->owns_matrix) { cudaFree(h->d_rowptr); cudaFree(h->d_colidx); cudaFree(h->d_vals); }
   cudaFree(h->d_vals0);
-  void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->P, h->AP, h->B, h->stage,
+  void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->P, h->P2, h->AP, h->B, h->stage,
                   h->d_cum, h->d_max, h->d_ctl, h->d_partials, h->d_flush};
   for (void* b : bufs) if (b) cudaFree(b);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
@@ -2569,17 +2642,17 @@ int cs_b200_profile_spmm(cs_b200_handle* h, int enable, double* total_ms, int64_
     h->prof_bytes = 0.0;
     h->prof_slot.clear();
     h->prof_pair_bytes.clear();
-    for (int i = 0; i < 16; ++i) { h->prof_slot_ms[i] = 0.0; h->prof_slot_bytes[i] = 0.0; h->prof_slot_launches[i] = 0; }
+    for (int i = 0; i < PROF_CLASSES; ++i) { h->prof_slot_ms[i] = 0.0; h->prof_slot_bytes[i] = 0.0; h->prof_slot_launches[i] = 0; }
   }
   return CS_B200_OK;
 }
 
-int cs_b200_profile_classes(cs_b200_handle* h, double* ms16, double* bytes16, int64_t* launches16) {
+int cs_b200_profile_classes(cs_b200_handle* h, double* ms18, double* bytes18, int64_t* launches18) {
   if (!h) return CS_B200_ERR_ARG;
-  for (int i = 0; i < 16; ++i) {
-    if (ms16) ms16[i] = h->prof_slot_ms[i];
-    if (bytes16) bytes16[i] = h->prof_slot_bytes[i];
-    if (launches16) launches16[i] = h->prof_slot_launches[i];
+  for (int i = 0; i < PROF_CLASSES; ++i) {
+    if (ms18) ms18[i] = h->prof_slot_ms[i];
+    if (bytes18) bytes18[i] = h->prof_slot_bytes[i];
+    if (launches18) launches18[i] = h->prof_slot_launches[i];
   }
   return CS_B200_OK;
 }

@@ -52,6 +52,10 @@ struct PanelCtl {
   int stall[MAXKT];
   int stall_limit;
   int stalled[MAXKT];
+  // fused CG step (k_stencil_cg): alpha of p_j in slot j mod 3 (j >= -1; slot 2 = 0 stands for the zero
+  // p_{-1}).  A step reads the two slots of the deferred x updates and writes the third, so its CTAs never
+  // read a slot its last CTA rewrites.
+  double alpha_ring[3][MAXKT];
 };
 
 // ---------------------------------------------------------------------------
@@ -201,6 +205,7 @@ __device__ __forceinline__ void cg_after_precond(PanelCtl* ctl, const double* rh
       ctl->active[c] = (rn > 0.0 && sqrt(rn) > tol && ctl->itmax > 0) ? 1 : 0;
       ctl->iters[c] = 0;
       ctl->alpha[c] = 0.0;
+      ctl->alpha_ring[0][c] = ctl->alpha_ring[1][c] = ctl->alpha_ring[2][c] = 0.0;
       ctl->beta[c] = 0.0;
       ctl->best[c] = rn;
       ctl->stall[c] = 0;
@@ -547,25 +552,28 @@ __device__ __forceinline__ void consumer_sync() {   // named barrier 1: consumer
 
 // N contiguous values through the widest aligned vector access (<= 16 B); p is aligned to
 // min(16, N*sizeof(T)) bytes by construction (rows of KT values, column groups of CPT).
-template <typename T, int N>
+// NC: through the read-only path, for data no thread of the kernel writes that the compiler cannot prove so.
+template <typename T, int N, bool NC = false>
 __device__ __forceinline__ void ldvec(const T* p, T (&v)[N]) {
   constexpr int BYTES = N * (int)sizeof(T);
   if constexpr (BYTES >= 16) {
     constexpr int PER = 16 / (int)sizeof(T);
 #pragma unroll
     for (int k = 0; k < N / PER; ++k) {
-      const uint4 t = *reinterpret_cast<const uint4*>(p + k * PER);
+      const uint4* a = reinterpret_cast<const uint4*>(p + k * PER);
+      const uint4 t = NC ? __ldg(a) : *a;
       const T* q = reinterpret_cast<const T*>(&t);
 #pragma unroll
       for (int i = 0; i < PER; ++i) v[k * PER + i] = q[i];
     }
   } else if constexpr (BYTES == 8) {
-    const uint2 t = *reinterpret_cast<const uint2*>(p);
+    const uint2* a = reinterpret_cast<const uint2*>(p);
+    const uint2 t = NC ? __ldg(a) : *a;
     const T* q = reinterpret_cast<const T*>(&t);
 #pragma unroll
     for (int i = 0; i < N; ++i) v[i] = q[i];
   } else {
-    v[0] = p[0];
+    v[0] = NC ? __ldg(p) : p[0];
   }
 }
 template <typename T, int N>
@@ -1071,6 +1079,131 @@ k_stencil(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, const S
 }
 
 // ---------------------------------------------------------------------------
+// Fused CG step of the AMG-PCG loop on a stencil-form finest level, iteration it = ctl->iter:
+//   p_it = z + beta p_{it-1}   formed for the 9 gathered neighbours and for the own row, which goes to Pd
+//   Y    = A p_it ; p.Ap per column ; last CTA: alpha_it exactly as k_stencil<SP_CG>, also into alpha_ring
+//   x    the deferred solution updates, two at a time: on odd it, x = (x + alpha_{it-2} p_{it-2}) + alpha_{it-1}
+//        p_{it-1}, with p_{it-2} read from the own row of Pd before p_it overwrites it
+// p of even iterations lives in Pb[0], of odd ones in Pb[1]: the step reads p_{it-1} at neighbour rows while
+// it writes p_it, so the two cannot share a buffer, and the buffer is picked from ctl->iter on the device
+// (the loop body is captured once).  Tile order, grid and per-thread dot accumulation are those of
+// k_stencil<SP_CG>, and every p and x value is formed with the expressions of k_cg_update_xp2: the partials,
+// alpha and the iterates are bit-identical to the SpMM + update pair this replaces.  k_cg_x_tail applies
+// the updates still pending when the loop ends.  It moves Z, p_{it-1}, the diagonals in and AP, p_it out
+// every step, and X in/out and p_{it-2} in every other step, against the pair's Z, P, X in and X, P out
+// plus the SpMM's diagonals, P in and AP out.
+// ---------------------------------------------------------------------------
+// CTAs per SM of k_stencil_cg: two (128 registers), all the z and p gathers of a row in flight.  At three (80
+// registers) the T = double variants are spill-free but ptxas issues the gathers in smaller batches: on an
+// H100 80GB HBM3 (700 W), fp64 k = 8 with the fp32 z on the 3163^2 raster, one step took 1.96 ms against
+// 1.70 ms at two.  The fp32 k = 4 and 8 variants spill at three.
+constexpr int CGF_MINB = 2;
+
+template <typename T, int KT, typename TV>
+__device__ __forceinline__ void stencil_cg_body(const DiaDev<T>& A, const TV* __restrict__ Z, const T* __restrict__ Pold,
+                                                T* __restrict__ Pd, T* __restrict__ X, T* __restrict__ Y,
+                                                PanelCtl* ctl, double* partials, int it) {
+  constexpr int V16 = 16 / (int)sizeof(T);
+  constexpr int CPT = KT < V16 ? KT : V16;      // panel columns per thread (one 16-byte vector)
+  constexpr int CG = KT / CPT;                  // column groups per row
+  constexpr int RPP = NT / CG;                  // rows per pass of the CTA
+  const int tid = threadIdx.x;
+  const int cg = tid % CG, rl = tid / CG, c0 = cg * CPT;
+  const int n = A.n, nr = A.nr;
+  const int ncol = (n + nr - 1) / nr;
+  const int nrc = (nr + RPP - 1) / RPP;
+  const int ntc = (ncol + ST_TC - 1) / ST_TC;
+  const long long ntiles = (long long)nrc * ntc;
+  const bool pair = it & 1;
+  T be[CPT], a1[CPT], a2[CPT];                  // beta_it ; alpha_{it-1}, alpha_{it-2}
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) {
+    be[i] = (T)ctl->beta[c0 + i];
+    a1[i] = (T)ctl->alpha_ring[(it + 2) % 3][c0 + i];
+    a2[i] = (T)ctl->alpha_ring[(it + 1) % 3][c0 + i];
+  }
+  double dot0[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) dot0[i] = 0.0;
+
+  for (long long t = blockIdx.x; t < ntiles; t += gridDim.x) {
+    const int tc = (int)(t / nrc), rc = (int)(t % nrc);
+    const int r = rc * RPP + rl;
+    if (r >= nr) continue;
+    const int cend = min(ncol, (tc + 1) * ST_TC);
+    for (int c = tc * ST_TC; c < cend; ++c) {
+      const long long row_l = (long long)c * nr + r;
+      if (row_l >= n) break;
+      const int row = (int)row_l;
+      T v[9];
+#pragma unroll
+      for (int s = 0; s < 9; ++s) v[s] = __ldcs(A.vals + (size_t)s * A.ld + row);
+      TV zv[9][CPT];
+      T pv[9][CPT];
+#pragma unroll
+      for (int s = 0; s < 9; ++s) {
+        int j = row + (s / 3 - 1) * nr + (s % 3 - 1);
+        j = max(0, min(n - 1, j));
+        ldvec<TV, CPT>(Z + (size_t)j * KT + c0, zv[s]);
+        ldvec<T, CPT, true>(Pold + (size_t)j * KT + c0, pv[s]);   // Pold != Pd: nothing writes it here
+      }
+      const size_t o = (size_t)row * KT + c0;
+      T xo[CPT], pd[CPT], po[CPT];
+      if (pair) {
+        ldvec<T, CPT>(X + o, xo);
+        ldvec<T, CPT>(Pd + o, pd);
+      }
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) po[i] = pv[4][i];
+#pragma unroll
+      for (int s = 0; s < 9; ++s)
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) pv[s][i] = (T)zv[s][i] + be[i] * pv[s][i];
+      T acc[CPT];
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) acc[i] = T(0);
+#pragma unroll
+      for (int s = 0; s < 9; ++s)
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) acc[i] += v[s] * pv[s][i];
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) dot0[i] += (double)acc[i] * (double)pv[4][i];
+      stvec<T, CPT>(Y + o, acc);
+      stvec<T, CPT>(Pd + o, pv[4]);
+      if (pair) {
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) {
+          xo[i] += a2[i] * pd[i];
+          xo[i] += a1[i] * po[i];
+        }
+        stvec<T, CPT>(X + o, xo);
+      }
+    }
+  }
+  CSB_REDUCE_SMEM(1, KT)
+  double v[1][CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) v[0][i] = dot0[i];
+  if (grid_reduce<KT, CPT, 1, false>(v, partials, &ctl->ticket, s_warp, s_tree, s_out)) {
+    if (tid < KT) {
+      const double pap = s_out[tid];
+      const double al = (ctl->active[tid] && pap > 0.0) ? ctl->rho[tid] / pap : 0.0;
+      ctl->pap[tid] = pap;
+      ctl->alpha[tid] = al;
+      ctl->alpha_ring[it % 3][tid] = al;
+    }
+  }
+}
+
+template <typename T, int KT, typename TV>
+__global__ void __launch_bounds__(NT, CGF_MINB)
+k_stencil_cg(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __restrict__ X, T* __restrict__ Y,
+             PanelCtl* ctl, double* partials) {
+  const int it = ctl->iter;
+  stencil_cg_body<T, KT, TV>(A, Z, (it & 1) ? Pb0 : Pb1, (it & 1) ? Pb1 : Pb0, X, Y, ctl, partials, it);
+}
+
+// ---------------------------------------------------------------------------
 // Upward leg of the V-cycle on a stencil-form level, fused:  prolongate + correct + post-smooth
 //     x1 = x0 + P y          (y: the coarser level's correction, P: ~3 entries per row)
 //     z  = x1 + omega D^-1 (b - A x1)        [+ dot(b, z) -> CG beta / stop test on the finest level]
@@ -1530,6 +1663,40 @@ k_cg_update_xp2(size_t nelem, const TV* __restrict__ Z, T* __restrict__ X, T* __
     }
     vstore(X + e, x);
     vstore(P + e, p);
+  }
+}
+
+// after a loop of K = ctl->iter fused CG steps (k_stencil_cg): the x updates still pending, in order --
+// p_{K-1}, preceded by p_{K-2} when K is odd (the last pair went in at step K - 2)
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_cg_x_tail(size_t nelem, const T* __restrict__ Pb0, const T* __restrict__ Pb1, T* __restrict__ X,
+            const PanelCtl* ctl) {
+  constexpr int VEC = Vec<T>::N;
+  const int K = ctl->iter;
+  const bool two = K & 1;
+  const T* p2 = (K & 1) ? Pb1 : Pb0;         // p_{K-2} (j = -1: the zero p_{-1} with alpha 0)
+  const T* p1 = (K & 1) ? Pb0 : Pb1;         // p_{K-1}
+  const size_t e0 = ((size_t)blockIdx.x * NT + threadIdx.x) * VEC;
+  const size_t stride = (size_t)gridDim.x * NT * VEC;
+  T a1[VEC], a2[VEC];
+#pragma unroll
+  for (int i = 0; i < VEC; ++i) {
+    a1[i] = (T)ctl->alpha_ring[(K + 2) % 3][(e0 + i) % KT];
+    a2[i] = (T)ctl->alpha_ring[(K + 1) % 3][(e0 + i) % KT];
+  }
+  for (size_t e = e0; e < nelem; e += stride) {
+    T x[VEC], q1[VEC], q2[VEC];
+    vload(X + e, x);
+    vload(p1 + e, q1);
+    if (two) {
+      vload(p2 + e, q2);
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) x[i] += a2[i] * q2[i];
+    }
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) x[i] += a1[i] * q1[i];
+    vstore(X + e, x);
   }
 }
 

@@ -258,13 +258,14 @@ class B200Factor:
 
     def profile_classes(self):
         """per kernel class of the timed finest-level launches: {name: (ms, algorithmic bytes, launches)}"""
-        ms = np.zeros(16)
-        by = np.zeros(16)
-        ln = np.zeros(16, dtype=np.int64)
+        names = ["plain", "cg", "residual_gate", "residual", "jacobi", "jacobi_dot", "prolong_add", "prolong_jacobi_fused",
+                 "cg_step_fused"]
+        ms = np.zeros(2 * len(names))
+        by = np.zeros(2 * len(names))
+        ln = np.zeros(2 * len(names), dtype=np.int64)
         _lib.check(self._lib, self._h, self._lib.cs_b200_profile_classes(self._h, _lib._ptr(ms), _lib._ptr(by), _lib._ptr(ln)))
-        names = ["plain", "cg", "residual_gate", "residual", "jacobi", "jacobi_dot", "prolong_add", "prolong_jacobi_fused"]
         return {f"{names[i // 2]}_{'f32' if i % 2 else 'f64'}": (float(ms[i]), float(by[i]), int(ln[i]))
-                for i in range(16) if ln[i]}
+                for i in range(2 * len(names)) if ln[i]}
 
     def profile_bytes(self):
         """algorithmic bytes of the launches timed since profiling was enabled."""

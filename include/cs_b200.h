@@ -348,10 +348,11 @@ int cs_b200_comm_gather_pairs(cs_b200_comm* c, int64_t k_total, const int64_t* m
 int cs_b200_comm_max_double(cs_b200_comm* c, double* v, int count);
 int cs_b200_comm_barrier(cs_b200_comm* c);
 
-/* The same totals per kernel class (read before disabling): 16 slots, slot = 2 * epilogue + (fp32 ? 1 : 0)
+/* The same totals per kernel class (read before disabling): 18 slots, slot = 2 * epilogue + (fp32 ? 1 : 0)
  * with epilogue 0 plain, 1 CG (p.Ap), 2 residual + norms (gate), 3 residual, 4 Jacobi sweep, 5 Jacobi
- * sweep + r.z, 6 prolong-add, 7 fused prolongation + sweep.                                          */
-int cs_b200_profile_classes(cs_b200_handle* h, double* ms16, double* bytes16, int64_t* launches16);
+ * sweep + r.z, 6 prolong-add, 7 fused prolongation + sweep, 8 fused CG step (p = z + beta p, A p, p.Ap,
+ * deferred x update; since ABI 1005, 16 slots before).                                             */
+int cs_b200_profile_classes(cs_b200_handle* h, double* ms18, double* bytes18, int64_t* launches18);
 
 /* Library/ABI version: major*1000 + minor.                                          */
 int cs_b200_version(void);
