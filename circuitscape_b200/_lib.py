@@ -83,6 +83,10 @@ _PROTOS = {
     "cs_b200_solve_region_pairs": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_double, C.c_int64, C.c_void_p,
                                              C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "cs_b200_solve_grounded": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                         C.c_void_p]),
     "cs_b200_solve_sources": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,

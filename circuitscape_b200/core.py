@@ -1083,6 +1083,215 @@ def _all_to_one_batched_raster(G, comps, nodemap, newpoly, point_map, unique_poi
     return served
 
 
+@dataclass
+class OneToAllColumn:
+    """One iteration as a column on the whole-raster operator L0: `ground` (0-based rows, sorted) at 0 V,
+    `vals` injected at `rows` (0-based, sorted), both inside L0 component `comp`; `strength` divides the
+    one-to-all source voltage into the reported value."""
+    i: int
+    comp: int
+    ground: np.ndarray
+    rows: np.ndarray
+    vals: np.ndarray
+    strength: float
+
+
+@dataclass
+class OneToAllPlan:
+    """How CUDASolver(onetoall_raster=True) serves each iteration i (index into `ids`): `columns` are solved
+    on one whole-raster handle; `skipped[i] = (value, emits)` need no solve (`emits`: the iteration still
+    writes all-zero maps, as the loop does when no component is solved); `per_iteration` take the existing
+    loop (`reasons[i]` says why)."""
+    ids: list
+    columns: list
+    skipped: dict
+    per_iteration: list
+    reasons: dict
+
+
+def _local_map_is_global(nodemap, comp_of, ci, newpoly):
+    """Whether construct_local_node_map of component `ci` numbers its cells like L0 restricted to the
+    component (utils.jl:10-30 renumbers column-major; a NODATA cell of a merged polygon can move a node)."""
+    comp = np.nonzero(comp_of == ci)[0] + 1
+    if len(comp) == len(comp_of):
+        return True
+    lm = construct_local_node_map(nodemap, comp, newpoly)
+    rank = np.zeros(len(comp_of) + 1, dtype=np.int64)
+    rank[comp] = np.arange(1, len(comp) + 1)
+    return np.array_equal(lm, rank[nodemap])
+
+
+def plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths=None, included_pairs=None):
+    """Sort the iterations of onetoall_kernel from L0's node map (`nodemap`, 1-based, 0 = none, built from
+    `newpoly`) and component label per L0 node (`comp_of`, 0-based node index).  Works on the focal cells
+    only; reproduces the loop's source / ground maps (onetoall.jl:93-118), sources_and_grounds_from_maps
+    with rmvgnd / rmvsrc, the component picked through row i of points_rc (sic, onetoall.jl:120) and the
+    sum tests of advanced.jl:186-196."""
+    rr, cc_, ids = (np.asarray(a) for a in points_rc)
+    uniq = list(dict.fromkeys(int(p) for p in ids))
+    plan = OneToAllPlan(uniq, [], {}, [], {})
+    if included_pairs is not None:
+        for i in range(len(uniq)):
+            plan.per_iteration.append(i)
+            plan.reasons[i] = "an include/exclude list: the loop builds each iteration's node map (onetoall.jl:88-90)"
+        return plan
+    nr, nc = gmap.shape
+    flat = ((cc_ - 1) * nr + (rr - 1)).astype(np.int64)          # column-major cell of each point row
+    node_of = np.asarray(nodemap).reshape(-1, order="F")
+    pm = {}                                                      # point_map: the last row on a cell wins
+    for x, p in zip(flat.tolist(), ids.tolist()):
+        pm[x] = int(p)
+    upm = {}                                                     # unique_point_map: each id's first cell
+    for p in uniq:
+        upm[int(flat[int(np.nonzero(ids == p)[0][0])])] = p
+    smap = None
+    if strengths is not None:                                    # onetoall.jl:93-101 (raises like the loop)
+        st = np.array(strengths, dtype=np.float64)
+        st[np.array([pm[x] for x in flat.tolist()]) == 0, 1] = 1
+        sm = np.zeros(gmap.shape)
+        sm[rr - 1, cc_ - 1] = st[:, 1]
+        smf = sm.reshape(-1, order="F")
+        smap = {x: float(smf[x]) for x in pm}
+    pm_sum = sum(pm.values())
+    rowmajor = lambda x: (x % nr) * nc + x // nr                 # np.add.at visits cells in C order
+    lm_ok = {}
+    for i, n in enumerate(uniq):
+        if pm_sum == n:                                          # no other focal node left
+            plan.skipped[i] = (-1.0, False)
+            continue
+        strv = 1.0
+        if one_to_all:
+            strv = float(strengths[i, 1]) if strengths is not None else 1.0
+            src = [(x, strv) for x, p in upm.items() if p == n]
+            gnd = [x for x, p in pm.items() if p != n and p > 0]
+        else:
+            if smap is not None:
+                src = [(x, v) for x, v in smap.items() if upm.get(x) != n]
+            else:
+                src = [(x, 1.0) for x, p in upm.items() if p != 0 and pm[x] != n]
+            gnd = [x for x, p in pm.items() if p == n]
+        s = {}
+        for x, v in sorted(src, key=lambda t: rowmajor(t[0])):
+            if v != 0 and node_of[x] != 0:
+                s[int(node_of[x]) - 1] = s.get(int(node_of[x]) - 1, 0.0) + v
+        s = {k: v for k, v in s.items() if v != 0}
+        g = {int(node_of[x]) - 1 for x in gnd if node_of[x] != 0}
+        if one_to_all:
+            g -= set(s)                                          # rmvgnd
+        else:
+            s = {k: v for k, v in s.items() if k not in g}       # rmvsrc
+        check_node = int(node_of[flat[i]])                       # (sic) row i of points_rc
+        if check_node == 0:
+            plan.skipped[i] = (-1.0, True)
+            continue
+        ci = int(comp_of[check_node - 1])
+        rows = np.array(sorted(k for k in s if comp_of[k] == ci), dtype=np.int64)
+        vals = np.array([s[k] for k in rows.tolist()], dtype=np.float64)
+        ground = np.array(sorted(k for k in g if comp_of[k] == ci), dtype=np.int64)
+        if vals.sum() == 0 or len(ground) == 0:                  # advanced.jl:194-196: nothing solved
+            plan.skipped[i] = (-1.0, True)
+            continue
+        if ci not in lm_ok:
+            lm_ok[ci] = _local_map_is_global(nodemap, comp_of, ci, newpoly)
+        if not lm_ok[ci]:
+            plan.per_iteration.append(i)
+            plan.reasons[i] = "the component's local node map numbers cells unlike L0 (utils.jl:10-30)"
+            continue
+        plan.columns.append(OneToAllColumn(i, ci, ground, rows, vals, strv))
+    return plan
+
+
+def _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solver, four_neighbors, avg_res):
+    """Solve the plan's columns on one whole-raster handle.  one-to-all and all-to-one iterations with
+    several ground rows: cs_b200_solve_grounded (Dirichlet rows at the grounds); all-to-one with one ground
+    row: the singular form of cs_b200_solve_sources (ref = the ground), whose voltages outside the
+    component are zeroed here.  Node currents go into the handle's cumulative / max vectors.
+    -> ({i: (value, voltmap | None, curmap | None)}, cumulative map, max map | None, iterations)."""
+    want_v = o.write_volt_maps
+    want_c = o.write_cur_maps or o.write_cum_cur_map_only
+    served = {}
+    factor, dev_nodemap = S.construct_raster_factor(gmap, newpoly, solver, four_neighbors=four_neighbors,
+                                                    avg_res=avg_res, log_transform=False)
+    iters = 0
+    with factor:
+        if not np.array_equal(np.asarray(dev_nodemap), nodemap):
+            raise RuntimeError("device node map differs from the host's")
+        factor.reset_currents()
+        singular = lambda c: (not one_to_all) and len(c.ground) == 1
+        bs = max(1, int(solver.bs))
+        for kind in (False, True):
+            cols = [c for c in plan.columns if singular(c) == kind]
+            for st in range(0, len(cols), bs):
+                chunk = cols[st:st + bs]
+                if kind:
+                    res = factor.solve_sources(
+                        [(np.r_[c.rows, c.ground], np.r_[c.vals, -c.vals.sum()]) for c in chunk],
+                        [int(c.ground[0]) for c in chunk], want_volt=want_v, want_curr=want_c, accumulate=True)
+                else:
+                    res = factor.solve_grounded([c.ground for c in chunk], np.arange(len(chunk)),
+                                                [(c.rows, c.vals) for c in chunk], want_volt=want_v,
+                                                want_curr=want_c, accumulate=True)
+                iters += int(res["iters"].sum())
+                for col, c in enumerate(chunk):
+                    val = 0.0
+                    if one_to_all:
+                        val = float(res["src_volt"][col]) / c.strength
+                        val = -1.0 if np.isclose(val, 0) else val               # advanced.jl:252-263
+                    out = comp_of != c.comp
+                    vm = cm = None
+                    if want_v:
+                        v = np.asarray(res["volt"][:, col], dtype=np.float64).copy()
+                        v[out] = 0.0
+                        vm = _scatter(v, nodemap)
+                    if want_c:
+                        cur = np.asarray(res["curr"][:, col], dtype=np.float64).copy()
+                        cur[out] = 0.0
+                        cm = _scatter(cur, nodemap)
+                    served[c.i] = (val, vm, cm)
+        cum, mx = factor.read_currents(want_max=o.write_max_cur_maps)
+    cmap = _scatter(np.asarray(cum, dtype=np.float64), nodemap)
+    mmap = None if mx is None or not plan.columns else _scatter(np.asarray(mx, dtype=np.float64), nodemap)
+    return served, cmap, mmap, iters
+
+
+def _onetoall_output(plan, device, gmap, o, out=None, res=None):
+    """The results of the iterations the plan keeps out of the loop, into `out` / `res`; with out=None a
+    new, finished OneToAllOutput (the loop's NODATA clamp of the cumulative map included)."""
+    finish = out is None
+    if finish:
+        out = OneToAllOutput(resistances=None)
+        out.cum_curmap = np.zeros(gmap.shape)
+        out.max_curmap = np.full(gmap.shape, NODATA) if o.write_max_cur_maps else None
+        res = np.zeros(len(plan.ids))
+    served = device.get("served", {})
+    for i, n in enumerate(plan.ids):
+        if i in plan.skipped:
+            res[i], emits = plan.skipped[i]
+            if not emits:
+                continue
+            if o.write_volt_maps:
+                out.voltmaps[n] = np.zeros(gmap.shape)
+            if o.write_cur_maps or o.write_cum_cur_map_only:
+                out.curmaps[n] = np.zeros(gmap.shape)
+            if out.max_curmap is not None:
+                out.max_curmap = np.maximum(out.max_curmap, 0.0)
+        elif i in served:
+            res[i], vm, cm = served[i]
+            out.num_solves += 1
+            if vm is not None:
+                out.voltmaps[n] = vm
+            if cm is not None:
+                out.curmaps[n] = cm
+    if device:
+        out.cum_curmap += device["cum"]
+        if out.max_curmap is not None and device["max"] is not None:
+            out.max_curmap = np.maximum(out.max_curmap, device["max"])
+    if finish:
+        out.resistances = np.column_stack([plan.ids, res])
+        out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
+    return out
+
+
 def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all=None,
                     four_neighbors=False, avg_res=False) -> OneToAllOutput:
     """src/raster/onetoall.jl:13-167.  One advanced-mode solve per focal id: one-to-all = unit
@@ -1110,6 +1319,19 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
     newpoly = graph.create_new_polymap(gmap, polymap, points_rc, point_map)
     nodemap = graph.construct_node_map(gmap, newpoly)
     adj = graph.construct_graph(gmap, nodemap, avg_res, four_neighbors)
+    device, plan = {}, None
+    if getattr(solver, "onetoall_raster", False):       # precedence over batch_one_to_all / batch_all_to_one
+        from scipy.sparse import csgraph
+        a = adj.copy()
+        a.eliminate_zeros()
+        comp_of = csgraph.connected_components(a, directed=False)[1]
+        plan = plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths, inc)
+        if plan.columns:
+            device = dict(zip(("served", "cum", "max", "iters"),
+                              _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solver,
+                                                four_neighbors, avg_res)))
+        if not plan.per_iteration:
+            return _onetoall_output(plan, device, gmap, o)
     comps = graph.connected_components(adj)
     G = graph.laplacian(adj)
     first = {p: int(np.nonzero(ids == p)[0][0]) for p in uniq}
@@ -1122,15 +1344,17 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
     res = np.zeros(len(uniq))
     strength_map = np.zeros(gmap.shape) if strengths is not None else None
     batched = {}
-    if (not one_to_all) and inc is None and getattr(solver, "batch_all_to_one", False):
+    if (not one_to_all) and inc is None and plan is None and getattr(solver, "batch_all_to_one", False):
         batched = _all_to_one_batched_raster(G, comps, nodemap, newpoly, point_map, unique_point_map, uniq,
                                              rr, cc_, strengths, solver, o)
     batched1 = {}
-    if one_to_all and inc is None and getattr(solver, "batch_one_to_all", False):
+    if one_to_all and inc is None and plan is None and getattr(solver, "batch_one_to_all", False):
         batched1 = _one_to_all_batched_raster(G, comps, nodemap, newpoly, point_map, unique_point_map, uniq,
                                               rr, cc_, strengths, solver)
     resident_factors = {}          # CUDASolver(resident_grounds=True): one device factor per component
     for i, n in enumerate(uniq):
+        if plan is not None and i not in plan.reasons:              # served by the plan (_onetoall_output)
+            continue
         pm, nm, npoly = point_map.copy(), nodemap, newpoly
         if inc is not None:
             for j, other in enumerate(inc.point_ids):
@@ -1219,6 +1443,8 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
             out.max_curmap = np.maximum(out.max_curmap, outcurr)
     for f in resident_factors.values():
         f.close()
+    if plan is not None:
+        _onetoall_output(plan, device, gmap, o, out, res)
     out.resistances = np.column_stack([uniq, res])
     out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
     return out

@@ -1861,6 +1861,120 @@ int solve_region_pairs_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_
   return CS_B200_OK;
 }
 
+// ---- direct-ground columns (cs_b200_solve_grounded) -----------------------------------------
+// Column c: the rows of its ground set are Dirichlet rows at 0 V (segment 2c of the region-panel table;
+// segment 2c+1, the region panels' set_b, is empty), b = its sparse sources, masked; A_c v = b.  No flux
+// or scaling step, and no set fix-up of the currents: every ground row is a node of its own.
+template <typename T, int KT>
+int grounded_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const int64_t* set_rows,
+                   const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
+                   const double* weight, double rtol, int64_t itmax, T* src_volt, T* volt, T* curr,
+                   int accumulate, int64_t* iters, double* relres, bool* any_fail, bool* any_maxit,
+                   std::string* msg) {
+  const size_t nelem = (size_t)h->n_pad * KT;
+  PanelCtl* hc = h->h_ctl;
+  std::memset(hc, 0, sizeof(PanelCtl));
+  int seg[2 * MAXKT + 1];
+  int ent_ptr[MAXKT + 1];
+  std::vector<int> rows;
+  seg[0] = 0;
+  const int64_t e0 = src_ptr[c0];
+  for (int c = 0; c < KT; ++c) {
+    hc->src[c] = -1;
+    hc->dst[c] = src_rows[src_ptr[c0 + c]];          // k_pair_extract probes the first source row
+    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
+    const int64_t s = gset[c0 + c];
+    for (int64_t e = set_ptr[s]; e < set_ptr[s + 1]; ++e) rows.push_back((int)set_rows[e]);
+    seg[2 * c + 1] = seg[2 * c + 2] = (int)rows.size();
+    ent_ptr[c] = (int)(src_ptr[c0 + c] - e0);
+  }
+  ent_ptr[KT] = (int)(src_ptr[c0 + KT] - e0);
+  const size_t nent = (size_t)ent_ptr[KT];
+  if (!h->d_rg_seg) CK(h, cudaMalloc(&h->d_rg_seg, (2 * MAXKT + 1) * sizeof(int)));
+  if (rows.size() > h->rg_cap) {
+    CK(h, cudaStreamSynchronize(h->stream));
+    drop_graphs(h->rgraphs);                 // they captured the old address
+    cudaFree(h->d_rg_rows);
+    h->d_rg_rows = nullptr;
+    h->rg_cap = std::max<size_t>(rows.size(), 4096);
+    CK(h, cudaMalloc(&h->d_rg_rows, h->rg_cap * sizeof(int)));
+  }
+  if (nent > h->sp_cap) {
+    cudaFree(h->d_sp_rows); cudaFree(h->d_sp_vals);
+    h->d_sp_rows = nullptr; h->d_sp_vals = nullptr;
+    h->sp_cap = std::max<size_t>(nent, 1024);
+    CK(h, cudaMalloc(&h->d_sp_rows, h->sp_cap * sizeof(long long)));
+    CK(h, cudaMalloc(&h->d_sp_vals, h->sp_cap * sizeof(double)));
+  }
+  if (!h->d_sp_ptr) CK(h, cudaMalloc(&h->d_sp_ptr, (MAXKT + 1) * sizeof(int)));
+  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
+  CK(h, h2d(h, h->d_rg_seg, seg, (2 * KT + 1) * sizeof(int)));
+  CK(h, h2d(h, h->d_rg_rows, rows.data(), rows.size() * sizeof(int)));
+  CK(h, h2d(h, h->d_sp_ptr, ent_ptr, (KT + 1) * sizeof(int)));
+  CK(h, h2d(h, h->d_sp_rows, src_rows + e0, nent * sizeof(long long)));
+  CK(h, h2d(h, h->d_sp_vals, src_vals + e0, nent * sizeof(double)));
+  h->stats.h2d_bytes += sizeof(PanelCtl) + (2.0 * KT + 1 + rows.size() + KT + 1) * sizeof(int) + nent * 16.0;
+  // B = sum of the sources, zero on the ground rows (the entry point rejects a source there) and pad rows
+  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
+  k_sparse_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_sp_ptr, h->d_sp_rows, h->d_sp_vals);
+  h->stats.kernel_launches++;
+  launch_seg_set<T, KT>(h, h->B, 0, T(0));
+  h->rg_on = true;
+  int rc = solve_panel<T, KT>(h, rtol, itmax);
+  h->rg_on = false;
+  if (rc) return rc;
+  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
+  h->stats.kernel_launches++;
+  if (accumulate || curr) launch_currents<T, KT>(h, curr != nullptr, accumulate);
+  CK(h, cudaGetLastError());
+  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  if (curr) {
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
+                                                    (T*)h->stage, h->d_ctl, 0);
+    h->stats.kernel_launches++;
+    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
+  }
+  if (volt) {
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
+                                                    (T*)h->stage, h->d_ctl, 0);
+    h->stats.kernel_launches++;
+    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
+  }
+  CK(h, cudaMemcpyAsync(hc, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  h->stats.d2h_bytes += sizeof(PanelCtl);
+  if (src_volt)
+    for (int c = 0; c < KT; ++c) src_volt[c0 + c] = (T)hc->xdst[c];
+  return CS_B200_OK;
+}
+
+template <typename T>
+int solve_grounded_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_t* set_rows, int64_t k,
+                     const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
+                     const double* weight, double rtol, int64_t itmax, T* src_volt, T* volt, T* curr,
+                     int accumulate, int64_t* iters, double* relres) {
+  bool any_fail = false, any_maxit = false;
+  std::string msg;
+  int64_t c0 = 0;
+  while (c0 < k) {
+    const int kt = next_kt(k - c0, h->ktmax);
+    int rc = 0;
+    DISPATCH_KT(kt, (rc = grounded_panel<T, KT>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals,
+                                                weight, rtol, itmax, src_volt, volt, curr, accumulate, iters,
+                                                relres, &any_fail, &any_maxit, &msg)));
+    if (rc) return rc;
+    c0 += kt;
+  }
+  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
+  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
+  return CS_B200_OK;
+}
+
 template <typename T>
 int solve_sources_t(cs_b200_handle* h, int64_t k, const int64_t* colptr, const int64_t* rows,
                     const double* vals, const int64_t* ref, const double* weight, double rtol,
@@ -2148,7 +2262,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1005; }
+int cs_b200_version(void) { return 1006; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2899,15 +3013,8 @@ int cs_b200_solve_pairs_superposed(cs_b200_handle* h, int64_t np, const int64_t*
   return rc;
 }
 
-int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
-                               const int64_t* set_rows, int64_t k, const int64_t* set_a,
-                               const int64_t* set_b, const double* weight, double rtol, int64_t itmax,
-                               void* R, void* volt, void* curr, int accumulate,
-                               int64_t* iters, double* relres) {
-  // the sets are checked before the handle so that malformed input is reported the same way with or
-  // without a device; row ranges need the handle's n
-  if (k < 1 || nsets < 1 || !set_ptr || !set_rows || !set_a || !set_b || !R || !(rtol >= 0) || itmax < 0)
-    return set_err(h, CS_B200_ERR_ARG, "bad solve_region_pairs arguments");
+// the sets of one CSR (set_ptr[nsets+1], set_rows): non-empty, sorted, unique, rows in range
+static int check_sets(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows) {
   if (set_ptr[0] != 0) return set_err(h, CS_B200_ERR_ARG, "set_ptr[0] must be 0");
   for (int64_t s = 0; s < nsets; ++s) {
     if (set_ptr[s + 1] <= set_ptr[s]) return set_err(h, CS_B200_ERR_ARG, "set %lld is empty", (long long)s);
@@ -2918,6 +3025,19 @@ int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* 
         return set_err(h, CS_B200_ERR_ARG, "set %lld: rows not sorted and unique", (long long)s);
     }
   }
+  return CS_B200_OK;
+}
+
+int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
+                               const int64_t* set_rows, int64_t k, const int64_t* set_a,
+                               const int64_t* set_b, const double* weight, double rtol, int64_t itmax,
+                               void* R, void* volt, void* curr, int accumulate,
+                               int64_t* iters, double* relres) {
+  // the sets are checked before the handle so that malformed input is reported the same way with or
+  // without a device; row ranges need the handle's n
+  if (k < 1 || nsets < 1 || !set_ptr || !set_rows || !set_a || !set_b || !R || !(rtol >= 0) || itmax < 0)
+    return set_err(h, CS_B200_ERR_ARG, "bad solve_region_pairs arguments");
+  if (int rc = check_sets(h, nsets, set_ptr, set_rows)) return rc;
   for (int64_t c = 0; c < k; ++c) {
     const int64_t a = set_a[c], b = set_b[c];
     if (a < 0 || a >= nsets || b < 0 || b >= nsets)
@@ -2939,6 +3059,47 @@ int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* 
                                               (double*)R, (double*)volt, (double*)curr, accumulate, iters, relres)
                : solve_region_pairs_t<float>(h, set_ptr, set_rows, k, set_a, set_b, weight, rtol, itmax,
                                              (float*)R, (float*)volt, (float*)curr, accumulate, iters, relres);
+  end_call(h);
+  return rc;
+}
+
+int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
+                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
+                           const double* src_vals, const double* weight, double rtol, int64_t itmax,
+                           void* src_volt, void* volt, void* curr, int accumulate, int64_t* iters,
+                           double* relres) {
+  // everything is checked before the handle, as in cs_b200_solve_region_pairs; row ranges need its n
+  if (k < 1 || nsets < 1 || !set_ptr || !set_rows || !gset || !src_ptr || !src_rows || !src_vals ||
+      !(rtol >= 0) || itmax < 0)
+    return set_err(h, CS_B200_ERR_ARG, "bad solve_grounded arguments");
+  if (int rc = check_sets(h, nsets, set_ptr, set_rows)) return rc;
+  if (src_ptr[0] != 0) return set_err(h, CS_B200_ERR_ARG, "src_ptr[0] must be 0");
+  for (int64_t c = 0; c < k; ++c) {
+    const int64_t s = gset[c];
+    if (s < 0 || s >= nsets)
+      return set_err(h, CS_B200_ERR_ARG, "column %lld: set index %lld out of range", (long long)c, (long long)s);
+    if (src_ptr[c + 1] <= src_ptr[c])
+      return set_err(h, CS_B200_ERR_ARG, "column %lld has no sources", (long long)c);
+    if (src_ptr[c + 1] - src_ptr[0] > INT32_MAX)
+      return set_err(h, CS_B200_ERR_ARG, "too many source entries");
+    for (int64_t e = src_ptr[c]; e < src_ptr[c + 1]; ++e) {
+      const int64_t r = src_rows[e];
+      if (r < 0 || (h && r >= h->n) || r > INT32_MAX)
+        return set_err(h, CS_B200_ERR_ARG, "column %lld: source row %lld out of range", (long long)c, (long long)r);
+      if (std::binary_search(set_rows + set_ptr[s], set_rows + set_ptr[s + 1], r))
+        return set_err(h, CS_B200_ERR_ARG, "column %lld: source row %lld is on its ground set %lld", (long long)c,
+                       (long long)r, (long long)s);
+    }
+  }
+  if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
+  begin_call(h);
+  int rc = h->dtype == CS_B200_F64
+               ? solve_grounded_t<double>(h, set_ptr, set_rows, k, gset, src_ptr, src_rows, src_vals, weight, rtol,
+                                          itmax, (double*)src_volt, (double*)volt, (double*)curr, accumulate, iters,
+                                          relres)
+               : solve_grounded_t<float>(h, set_ptr, set_rows, k, gset, src_ptr, src_rows, src_vals, weight, rtol,
+                                         itmax, (float*)src_volt, (float*)volt, (float*)curr, accumulate, iters,
+                                         relres);
   end_call(h);
   return rc;
 }

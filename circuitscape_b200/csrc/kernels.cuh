@@ -2071,7 +2071,8 @@ __global__ void k_flush(float* p, size_t n) {
 // focal-region pairs (cs_b200_solve_region_pairs).  A panel's Dirichlet sets are 2*KT row
 // segments of `rows`: segment 2c is set_a of column c (0 V), segment 2c+1 its set_b (1 V);
 // seg[] holds the 2*KT+1 offsets.  The segment kernels run one CTA per segment; the sets of
-// one column are disjoint, so no two threads write the same element.
+// one column are disjoint, so no two threads write the same element.  cs_b200_solve_grounded
+// uses the same table with segment 2c = column c's ground set and segment 2c+1 empty.
 // ---------------------------------------------------------------------------
 // P[row][s/2] = v for the rows of every segment s (set_b_only = 0) or of the set_b segments only
 template <typename T, int KT>

@@ -49,6 +49,8 @@ class CUDASolver:
     batch_one_to_all: bool = False   # one-to-all: one solve per iteration on ONE grounded operator
     resident_grounds: bool = False   # advanced mode: keep the component's factor, move the grounds on the
                                      # device (cs_b200_set_grounds) instead of a new handle per solve
+    onetoall_raster: bool = False    # one-to-all / all-to-one iterations as columns on one whole-raster
+                                     # handle (core.plan_onetoall); takes precedence over batch_*
 
     @property
     def dtype(self):
@@ -418,6 +420,47 @@ class B200Factor:
             volt = None if volt is None else volt.astype(self.io_dtype)
             curr = None if curr is None else curr.astype(self.io_dtype)
         return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
+
+    def solve_grounded(self, sets, gset, sources, weight=None, want_volt=False, want_curr=False,
+                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
+        """Advanced-mode columns with direct grounds on this operator (cs_b200_solve_grounded): column c
+        holds the rows of sets[gset[c]] at 0 V and injects sources[c] = (rows, values) (0-based rows, none
+        on the column's ground set).  sets: list of 0-based row arrays (sorted, unique, non-empty).
+        Returns dict with src_volt (v at each column's first source row), volt, curr (every ground row is
+        a node of its own), iters, relres."""
+        ptr = np.zeros(len(sets) + 1, dtype=np.int64)
+        for s, r in enumerate(sets):
+            ptr[s + 1] = ptr[s] + len(r)
+        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r in sets])
+                                    if len(sets) else np.zeros(0), dtype=np.int64)
+        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        k = len(gset)
+        assert len(sources) == k
+        sptr = np.zeros(k + 1, dtype=np.int64)
+        for c, (r, _) in enumerate(sources):
+            sptr[c + 1] = sptr[c] + len(r)
+        srows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r, _ in sources])
+                                     if k else np.zeros(0), dtype=np.int64)
+        svals = np.ascontiguousarray(np.concatenate([np.asarray(v, dtype=np.float64) for _, v in sources])
+                                     if k else np.zeros(0), dtype=np.float64)
+        assert len(srows) == len(svals) == sptr[-1]
+        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
+        sv = np.zeros(k, dtype=self.dtype)
+        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
+        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
+        iters = np.zeros(k, dtype=np.int64)
+        relres = np.zeros(k, dtype=np.float64)
+        rc = self._lib.cs_b200_solve_grounded(
+            self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(gset), _lib._ptr(sptr),
+            _lib._ptr(srows), _lib._ptr(svals), _lib._ptr(w), self.solver.rtol if rtol is None else rtol,
+            self.solver.itmax if itmax is None else itmax, _lib._ptr(sv), _lib._ptr(volt), _lib._ptr(curr),
+            1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+        self._raise(rc, raise_on_residual)
+        if self.io_dtype != self.dtype:
+            sv = sv.astype(self.io_dtype)
+            volt = None if volt is None else volt.astype(self.io_dtype)
+            curr = None if curr is None else curr.astype(self.io_dtype)
+        return dict(src_volt=sv, volt=volt, curr=curr, iters=iters, relres=relres)
 
     def solve_sources(self, columns, ref, probe=None, weight=None, want_volt=False, want_curr=False,
                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):

@@ -246,6 +246,21 @@ int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* 
                                void* R, void* volt, void* curr, int accumulate,
                                int64_t* iters, double* relres);
 
+/* Advanced-mode columns with direct grounds on ONE resident operator (src/raster/advanced.jl:274-305 with
+ * Inf grounds only; the one-to-all loop src/raster/onetoall.jl:106-118).  Column c: the rows of set gset[c]
+ * are held at 0 V (each its own node), b = sum_e src_vals[e] e_{src_rows[e]} over src_ptr[c]..src_ptr[c+1]-1,
+ * A_c v = b on the rest.  src_volt[c] = v at src_rows[src_ptr[c]].  weight / volt / curr / accumulate /
+ * iters / relres as cs_b200_solve_pairs.  Sets as in cs_b200_solve_region_pairs (CSR over 0-based rows,
+ * non-empty, sorted, unique); src_ptr[k+1] with src_ptr[0] = 0.  A column without sources, a source on its
+ * own ground set, bad sets, rows or set indices, or k <= 0 give CS_B200_ERR_ARG before any device work.
+ * Sources in a component that holds none of the column's ground rows make the system inconsistent: the
+ * caller must not pass them (the gate reports such a column as CS_B200_ERR_RESIDUAL / _MAXITER).          */
+int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
+                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
+                           const double* src_vals, const double* weight, double rtol, int64_t itmax,
+                           void* src_volt, void* volt, void* curr, int accumulate, int64_t* iters,
+                           double* relres);
+
 /* Batched solve with SPARSE right-hand sides, device-resident -- the advanced-mode kernel
  * (src/raster/advanced.jl:274-305) for source/ground sets without finite grounds, and
  * the all-to-one loop built on it (src/raster/onetoall.jl:110-118,146-151):
