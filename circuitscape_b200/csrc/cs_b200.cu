@@ -14,6 +14,7 @@
 #include <cstring>
 #include <limits>
 #include <string>
+#include <type_traits>
 #include <vector>
 
 #include "amg_host.hpp"
@@ -1363,31 +1364,85 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
   return CS_B200_OK;
 }
 
-int gather_panel_status(cs_b200_handle* h, int kt, int64_t c0, int64_t* iters, double* relres,
-                        int64_t itmax, bool* any_fail, bool* any_maxit, std::string* msg) {
-  for (int c = 0; c < kt; ++c) {
-    const PanelCtl& ct = *h->h_ctl;
-    const double bn = ct.bnorm[c];
-    const double rr = bn > 0 ? std::sqrt(ct.resid[c] / bn) : 0.0;
-    if (iters) iters[c0 + c] = ct.iters[c];
-    if (relres) relres[c0 + c] = rr;
-    h->stats.iterations += ct.iters[c];
-    if (!(rr < h->opts.resid_gate)) {
-      if (!*any_fail) {
-        char buf[256];
-        snprintf(buf, sizeof buf,
-                 "CUDA PCG solver residual %g exceeds tolerance %g for column %lld (%d iterations)",
-                 rr, h->opts.resid_gate, (long long)(c0 + c + 1), ct.iters[c]);
-        *msg = buf;
-      }
-      *any_fail = true;
-    }
-    // a column frozen by the stagnation guard above its tolerance is reported like one that ran into
-    // itmax: results written, CS_B200_ERR_MAXITER, the true-residual gate decides (core.jl:639-641)
-    if ((ct.iters[c] >= itmax || ct.stalled[c]) && std::sqrt(ct.rho[c]) > ct.tol[c]) *any_maxit = true;
-  }
-  return 0;
+int next_kt(int64_t remaining, int ktmax) {
+  int kt = ktmax;
+  while (kt > remaining) kt >>= 1;
+  return kt < 1 ? 1 : kt;
 }
+
+#define DISPATCH_KT(kt, CALL)                    \
+  switch (kt) {                                  \
+    case 1: { constexpr int KT = 1; CALL; } break; \
+    case 2: { constexpr int KT = 2; CALL; } break; \
+    case 4: { constexpr int KT = 4; CALL; } break; \
+    default: { constexpr int KT = 8; CALL; } break; \
+  }
+
+// The column driver of the batched solve entries: walks a call's columns in panels, collects every
+// column's residual-gate and itmax status, and maps them to the call's return code.
+struct ColumnDriver {
+  cs_b200_handle* h;
+  bool any_fail = false, any_maxit = false;
+  std::string msg;   // the first column over the residual gate
+
+  // columns c_begin .. c_end-1 in panels of next_kt width: panel(KT, c0) with KT a std::integral_constant;
+  // stops at the first panel that fails
+  template <typename Panel>
+  int run(int64_t c_begin, int64_t c_end, Panel&& panel) {
+    for (int64_t c0 = c_begin; c0 < c_end;) {
+      const int kt = next_kt(c_end - c0, h->ktmax);
+      int rc = 0;
+      DISPATCH_KT(kt, (rc = panel(std::integral_constant<int, KT>{}, c0)));
+      if (rc) return rc;
+      c0 += kt;
+    }
+    return CS_B200_OK;
+  }
+
+  // solve_panel on the staged panel of columns c0 .. c0+KT-1 (under its Dirichlet segments when masked), then
+  // gather its status
+  template <typename T, int KT>
+  int solve(int64_t c0, double rtol, int64_t itmax, int64_t* iters, double* relres, bool masked = false) {
+    h->rg_on = masked;
+    const int rc = solve_panel<T, KT>(h, rtol, itmax);
+    h->rg_on = false;
+    if (!rc) gather(KT, c0, iters, relres, itmax);
+    return rc;
+  }
+
+  // the status of the panel whose solve_panel just returned (columns c0 .. c0+kt-1)
+  void gather(int kt, int64_t c0, int64_t* iters, double* relres, int64_t itmax) {
+    for (int c = 0; c < kt; ++c) {
+      const PanelCtl& ct = *h->h_ctl;
+      const double bn = ct.bnorm[c];
+      const double rr = bn > 0 ? std::sqrt(ct.resid[c] / bn) : 0.0;
+      if (iters) iters[c0 + c] = ct.iters[c];
+      if (relres) relres[c0 + c] = rr;
+      h->stats.iterations += ct.iters[c];
+      if (!(rr < h->opts.resid_gate)) {
+        if (!any_fail) {
+          char buf[256];
+          snprintf(buf, sizeof buf,
+                   "CUDA PCG solver residual %g exceeds tolerance %g for column %lld (%d iterations)",
+                   rr, h->opts.resid_gate, (long long)(c0 + c + 1), ct.iters[c]);
+          msg = buf;
+        }
+        any_fail = true;
+      }
+      // a column frozen by the stagnation guard above its tolerance is reported like one that ran into
+      // itmax: results written, CS_B200_ERR_MAXITER, the true-residual gate decides (core.jl:639-641)
+      if ((ct.iters[c] >= itmax || ct.stalled[c]) && std::sqrt(ct.rho[c]) > ct.tol[c]) any_maxit = true;
+    }
+  }
+
+  // the call's return code: rc of a failed panel, else the residual gate, else the itmax stop
+  int verdict(int rc) const {
+    if (rc) return rc;
+    if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
+    if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
+    return CS_B200_OK;
+  }
+};
 
 // node currents of the panel in X (src/out.jl:178-290): branch-current maxima, then max(inflow, outflow)
 // per node with the 1e-8 zeroing, accumulated into the cumulative / max vectors (src/out.jl:100-107)
@@ -1409,60 +1464,155 @@ void launch_currents(cs_b200_handle* h, bool want_curr, int accumulate) {
   h->stats.kernel_launches += 2;
 }
 
-int next_kt(int64_t remaining, int ktmax) {
-  int kt = ktmax;
-  while (kt > remaining) kt >>= 1;
-  return kt < 1 ? 1 : kt;
-}
+// ---- panel staging and downloads shared by the column kinds ------------------------------------
+struct ColCtl {
+  long long src, dst;
+  double weight;
+};
 
-template <typename T, int KT>
-int pairs_panel(cs_b200_handle* h, int64_t c0, const int64_t* src, const int64_t* dst,
-                const double* weight, double rtol, int64_t itmax, T* R, T* volt, T* curr,
-                int accumulate, int64_t* iters, double* relres, bool* any_fail, bool* any_maxit,
-                std::string* msg) {
-  const size_t nelem = (size_t)h->n_pad * KT;
+inline double col_weight(const double* weight, int64_t c) { return weight ? weight[c] : 1.0; }
+
+// the panel's control block: zeroed, column c's src / dst / weight from col(c), uploaded
+template <typename Col>
+int upload_ctl(cs_b200_handle* h, int kt, Col&& col) {
   PanelCtl* hc = h->h_ctl;
   std::memset(hc, 0, sizeof(PanelCtl));
-  for (int c = 0; c < KT; ++c) {
-    hc->src[c] = src[c0 + c];
-    hc->dst[c] = dst[c0 + c];
-    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
+  for (int c = 0; c < kt; ++c) {
+    const ColCtl v = col(c);
+    hc->src[c] = v.src;
+    hc->dst[c] = v.dst;
+    hc->weight[c] = v.weight;
   }
   CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
   h->stats.h2d_bytes += sizeof(PanelCtl);
-  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
-  k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
-  h->stats.kernel_launches++;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  if (rc) return rc;
-  k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
-  h->stats.kernel_launches++;
-  if (accumulate || curr) {
-    launch_currents<T, KT>(h, curr != nullptr, accumulate);
-  }
-  CK(h, cudaGetLastError());
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
-  if (curr) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  if (volt) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
-                                                    (T*)h->stage, h->d_ctl, 1);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  // status gathered from the host copy taken inside solve_panel; xsrc/xdst need a re-read
-  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  return CS_B200_OK;
+}
+
+// host copy of the control block as the kernels after solve_panel left it
+int read_ctl(cs_b200_handle* h) {
   CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   h->stats.d2h_bytes += sizeof(PanelCtl);
+  return CS_B200_OK;
+}
+
+// d_sp_*: the panel's sparse right-hand sides for k_sparse_rhs.  ptr: the kt+1 column offsets into
+// rows / vals.  The capacity is recorded only once every buffer of the family is allocated.
+int upload_sparse_rhs(cs_b200_handle* h, int kt, const int64_t* ptr, const int64_t* rows, const double* vals) {
+  int ent_ptr[MAXKT + 1];
+  for (int c = 0; c <= kt; ++c) ent_ptr[c] = (int)(ptr[c] - ptr[0]);
+  const size_t nent = (size_t)ent_ptr[kt];
+  if (!h->d_sp_ptr || nent > h->sp_cap) {
+    cudaFree(h->d_sp_ptr); cudaFree(h->d_sp_rows); cudaFree(h->d_sp_vals);
+    h->d_sp_ptr = nullptr; h->d_sp_rows = nullptr; h->d_sp_vals = nullptr;
+    h->sp_cap = 0;
+    const size_t cap = std::max<size_t>(nent, 1024);
+    CK(h, cudaMalloc(&h->d_sp_ptr, (MAXKT + 1) * sizeof(int)));
+    CK(h, cudaMalloc(&h->d_sp_rows, cap * sizeof(long long)));
+    CK(h, cudaMalloc(&h->d_sp_vals, cap * sizeof(double)));
+    h->sp_cap = cap;
+  }
+  CK(h, h2d(h, h->d_sp_ptr, ent_ptr, (kt + 1) * sizeof(int)));
+  CK(h, h2d(h, h->d_sp_rows, rows + ptr[0], nent * sizeof(long long)));
+  CK(h, h2d(h, h->d_sp_vals, vals + ptr[0], nent * sizeof(double)));
+  h->stats.h2d_bytes += (kt + 1) * sizeof(int) + nent * 16.0;
+  return CS_B200_OK;
+}
+
+// d_rg_*: the panel's Dirichlet sets as the 2*kt row segments of k_seg_set -- segment 2c the rows of set
+// set_a[c], segment 2c+1 those of set_b[c] (empty without set_b).  Growing the buffers drops the region
+// graphs, which captured their addresses; the capacity is recorded once both buffers are allocated.
+int upload_set_segments(cs_b200_handle* h, int kt, const int64_t* set_ptr, const int64_t* set_rows,
+                        const int64_t* set_a, const int64_t* set_b) {
+  int seg[2 * MAXKT + 1];
+  std::vector<int> rows;
+  seg[0] = 0;
+  for (int s = 0; s < 2 * kt; ++s) {
+    const int64_t* sets = (s & 1) ? set_b : set_a;
+    if (sets)
+      for (int64_t e = set_ptr[sets[s / 2]]; e < set_ptr[sets[s / 2] + 1]; ++e) rows.push_back((int)set_rows[e]);
+    seg[s + 1] = (int)rows.size();
+  }
+  if (!h->d_rg_seg || rows.size() > h->rg_cap) {
+    CK(h, cudaStreamSynchronize(h->stream));
+    drop_graphs(h->rgraphs);
+    cudaFree(h->d_rg_seg); cudaFree(h->d_rg_rows);
+    h->d_rg_seg = nullptr; h->d_rg_rows = nullptr;
+    h->rg_cap = 0;
+    const size_t cap = std::max<size_t>(rows.size(), 4096);
+    CK(h, cudaMalloc(&h->d_rg_seg, (2 * MAXKT + 1) * sizeof(int)));
+    CK(h, cudaMalloc(&h->d_rg_rows, cap * sizeof(int)));
+    h->rg_cap = cap;
+  }
+  CK(h, h2d(h, h->d_rg_seg, seg, (2 * kt + 1) * sizeof(int)));
+  CK(h, h2d(h, h->d_rg_rows, rows.data(), rows.size() * sizeof(int)));
+  h->stats.h2d_bytes += (2.0 * kt + 1 + rows.size()) * sizeof(int);
+  return CS_B200_OK;
+}
+
+// d_probe*: the probe rows of cs_b200_solve_sources and room for one panel of their voltages; the
+// capacity is recorded once both buffers are allocated
+int upload_probe(cs_b200_handle* h, int64_t nprobe, const int64_t* probe) {
+  const size_t need = (size_t)nprobe;
+  if (need > h->probe_cap) {
+    cudaFree(h->d_probe); cudaFree(h->d_probe_out);
+    h->d_probe = nullptr; h->d_probe_out = nullptr;
+    h->probe_cap = 0;
+    CK(h, cudaMalloc(&h->d_probe, need * sizeof(long long)));
+    CK(h, cudaMalloc(&h->d_probe_out, need * MAXKT * sizeof(double)));
+    h->probe_cap = need;
+  }
+  CK(h, h2d(h, h->d_probe, probe, need * sizeof(long long)));
+  return CS_B200_OK;
+}
+
+// the panel's node currents (AP) and voltages (X; less each column's xsrc when volt_shift) into columns
+// c0 .. c0+KT-1 of the caller's column-major arrays, through the staging buffer; either may be null.
+// Checks the launches queued before it first.
+template <typename T, int KT>
+int download_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int volt_shift) {
+  CK(h, cudaGetLastError());
+  const int tg = (int)std::min<size_t>(4096, ((size_t)h->n_pad * KT + 255) / 256);
+  auto download = [&](const void* panel, int shift, T* out) -> int {
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)panel, (T*)h->stage,
+                                                    h->d_ctl, shift);
+    h->stats.kernel_launches++;
+    CK(h, cudaMemcpyAsync(out + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
+    return CS_B200_OK;
+  };
+  if (curr)
+    if (int rc = download(h->AP, 0, curr)) return rc;
+  if (volt)
+    if (int rc = download(h->X, volt_shift, volt)) return rc;
+  return CS_B200_OK;
+}
+
+// the node currents of launch_currents (into AP for curr, into the maps when accumulating), then download_outputs
+template <typename T, int KT>
+int currents_and_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int accumulate, int volt_shift) {
+  if (accumulate || curr) launch_currents<T, KT>(h, curr != nullptr, accumulate);
+  return download_outputs<T, KT>(h, c0, curr, volt, volt_shift);
+}
+
+// ---- the column kinds ------------------------------------------------------------------------
+template <typename T, int KT>
+int pairs_panel(cs_b200_handle* h, int64_t c0, const int64_t* src, const int64_t* dst,
+                const double* weight, double rtol, int64_t itmax, T* R, T* volt, T* curr,
+                int accumulate, int64_t* iters, double* relres, ColumnDriver& cols) {
+  if (int rc = upload_ctl(h, KT, [&](int c) {
+        return ColCtl{src[c0 + c], dst[c0 + c], col_weight(weight, c0 + c)};
+      }))
+    return rc;
+  CK(h, cudaMemsetAsync(h->B, 0, (size_t)h->n_pad * KT * sizeof(T), h->stream));
+  k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
+  h->stats.kernel_launches++;
+  if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres)) return rc;
+  k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
+  h->stats.kernel_launches++;
+  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 1)) return rc;
+  if (int rc = read_ctl(h)) return rc;   // xsrc / xdst of k_pair_extract
   for (int c = 0; c < KT; ++c) R[c0 + c] = (T)(h->h_ctl->xdst[c] - h->h_ctl->xsrc[c]);
   return CS_B200_OK;
 }
@@ -1473,41 +1623,14 @@ template <typename T, int KT>
 int sources_panel(cs_b200_handle* h, int64_t c0, const int64_t* colptr, const int64_t* rows,
                   const double* vals, const int64_t* ref, const double* weight, double rtol,
                   int64_t itmax, int64_t nprobe, T* probe_volt, T* volt, T* curr, int accumulate,
-                  int64_t* iters, double* relres, bool* any_fail, bool* any_maxit, std::string* msg) {
-  const size_t nelem = (size_t)h->n_pad * KT;
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
-  int ent_ptr[MAXKT + 1];
-  const int64_t e0 = colptr[c0];
-  for (int c = 0; c < KT; ++c) {
-    hc->src[c] = ref[c0 + c];
-    hc->dst[c] = -1;
-    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
-    ent_ptr[c] = (int)(colptr[c0 + c] - e0);
-  }
-  ent_ptr[KT] = (int)(colptr[c0 + KT] - e0);
-  const size_t nent = (size_t)ent_ptr[KT];
-  if (nent > h->sp_cap) {
-    cudaFree(h->d_sp_rows); cudaFree(h->d_sp_vals);
-    h->d_sp_rows = nullptr; h->d_sp_vals = nullptr;
-    h->sp_cap = std::max<size_t>(nent, 1024);
-    CK(h, cudaMalloc(&h->d_sp_rows, h->sp_cap * sizeof(long long)));
-    CK(h, cudaMalloc(&h->d_sp_vals, h->sp_cap * sizeof(double)));
-  }
-  if (!h->d_sp_ptr) CK(h, cudaMalloc(&h->d_sp_ptr, (MAXKT + 1) * sizeof(int)));
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
-  CK(h, h2d(h, h->d_sp_ptr, ent_ptr, (KT + 1) * sizeof(int)));
-  if (nent) {
-    CK(h, h2d(h, h->d_sp_rows, rows + e0, nent * sizeof(long long)));
-    CK(h, h2d(h, h->d_sp_vals, vals + e0, nent * sizeof(double)));
-  }
-  h->stats.h2d_bytes += sizeof(PanelCtl) + nent * 16.0;
-  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
+                  int64_t* iters, double* relres, ColumnDriver& cols) {
+  if (int rc = upload_ctl(h, KT, [&](int c) { return ColCtl{ref[c0 + c], -1, col_weight(weight, c0 + c)}; }))
+    return rc;
+  if (int rc = upload_sparse_rhs(h, KT, colptr + c0, rows, vals)) return rc;
+  CK(h, cudaMemsetAsync(h->B, 0, (size_t)h->n_pad * KT * sizeof(T), h->stream));
   k_sparse_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_sp_ptr, h->d_sp_rows, h->d_sp_vals);
   h->stats.kernel_launches++;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  if (rc) return rc;
-  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres)) return rc;
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
   h->stats.kernel_launches++;
   if (nprobe > 0 && probe_volt) {
@@ -1518,59 +1641,23 @@ int sources_panel(cs_b200_handle* h, int64_t c0, const int64_t* colptr, const in
                           cudaMemcpyDeviceToHost, h->stream));
     h->stats.d2h_bytes += (double)nprobe * KT * sizeof(T);
   }
-  if (accumulate || curr) {
-    launch_currents<T, KT>(h, curr != nullptr, accumulate);
-  }
-  CK(h, cudaGetLastError());
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
-  if (curr) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  if (volt) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
-                                                    (T*)h->stage, h->d_ctl, 1);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
+  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 1)) return rc;
   CK(h, cudaStreamSynchronize(h->stream));
   return CS_B200_OK;
 }
-
-template <typename T>
-int solve_sources_t(cs_b200_handle* h, int64_t k, const int64_t* colptr, const int64_t* rows,
-                    const double* vals, const int64_t* ref, const double* weight, double rtol,
-                    int64_t itmax, int64_t nprobe, const int64_t* probe, T* probe_volt, T* volt,
-                    T* curr, int accumulate, int64_t* iters, double* relres);
 
 // ---- superposition driver (cs_b200_solve_pairs_superposed) ----------------------------------
 // panel of point solves  A u_x = e_{nodes[x]} - e_{nodes[0]}  for x = x0 .. x0+KT-1 (1-based among
 // the focal nodes); the shifted solutions land in columns x0-1 .. of U (column-major, ld = n_pad)
 template <typename T, int KT>
 int point_panel(cs_b200_handle* h, int64_t x0, const int64_t* nodes, double rtol, int64_t itmax, T* U,
-                int64_t* point_iters, bool* any_fail, bool* any_maxit, std::string* msg) {
+                int64_t* point_iters, ColumnDriver& cols) {
   const size_t nelem = (size_t)h->n_pad * KT;
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
-  for (int c = 0; c < KT; ++c) {
-    hc->src[c] = nodes[0];
-    hc->dst[c] = nodes[x0 + c];
-    hc->weight[c] = 1.0;
-  }
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
-  h->stats.h2d_bytes += sizeof(PanelCtl);
+  if (int rc = upload_ctl(h, KT, [&](int c) { return ColCtl{nodes[0], nodes[x0 + c], 1.0}; })) return rc;
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
   k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
   h->stats.kernel_launches++;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  if (rc) return rc;
-  gather_panel_status(h, KT, 0, nullptr, nullptr, itmax, any_fail, any_maxit, msg);
+  if (int rc = cols.solve<T, KT>(0, rtol, itmax, nullptr, nullptr)) return rc;
   if (point_iters)
     for (int c = 0; c < KT; ++c) point_iters[x0 - 1 + c] = h->h_ctl->iters[c];
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
@@ -1587,23 +1674,20 @@ int point_panel(cs_b200_handle* h, int64_t x0, const int64_t* nodes, double rtol
 template <typename T, int KT>
 int combine_panel(cs_b200_handle* h, int64_t c0, const int64_t* nodes, const int64_t* pi, const int64_t* pj,
                   const double* weight, const T* U, int* d_ci, int* d_cj, T* R, T* volt, T* curr,
-                  int accumulate, double* relres, int64_t itmax, bool* any_fail, bool* any_maxit,
-                  std::string* msg) {
+                  int accumulate, double* relres, int64_t itmax, ColumnDriver& cols) {
   const size_t nelem = (size_t)h->n_pad * KT;
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
+  if (int rc = upload_ctl(h, KT, [&](int c) {
+        return ColCtl{nodes[pi[c0 + c]], nodes[pj[c0 + c]], col_weight(weight, c0 + c)};
+      }))
+    return rc;
   int ci[MAXKT], cj[MAXKT];
   for (int c = 0; c < KT; ++c) {
-    hc->src[c] = nodes[pi[c0 + c]];
-    hc->dst[c] = nodes[pj[c0 + c]];
-    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
     ci[c] = (int)pi[c0 + c] - 1;      // point 0 is the reference: its solution is identically 0
     cj[c] = (int)pj[c0 + c] - 1;
   }
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
   CK(h, h2d(h, d_ci, ci, KT * sizeof(int)));
   CK(h, h2d(h, d_cj, cj, KT * sizeof(int)));
-  h->stats.h2d_bytes += sizeof(PanelCtl) + 2.0 * KT * sizeof(int);
+  h->stats.h2d_bytes += 2.0 * KT * sizeof(int);
   const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
   k_combine<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n_pad, U, d_ci, d_cj, (T*)h->X);
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
@@ -1612,43 +1696,15 @@ int combine_panel(cs_b200_handle* h, int64_t c0, const int64_t* nodes, const int
   launch_spmm<T, KT, SP_RESNORM>(h, (const T*)h->X, (T*)h->AP, (const T*)h->B);
   h->stats.kernel_launches += 2;
   CK(h, cudaGetLastError());
-  CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(h, cudaStreamSynchronize(h->stream));
-  gather_panel_status(h, KT, c0, nullptr, relres, itmax, any_fail, any_maxit, msg);
+  if (int rc = read_ctl(h)) return rc;
+  cols.gather(KT, c0, nullptr, relres, itmax);
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
   h->stats.kernel_launches++;
-  if (accumulate || curr) {
-    launch_currents<T, KT>(h, curr != nullptr, accumulate);
-  }
-  CK(h, cudaGetLastError());
-  if (curr) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  if (volt) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
-                                                    (T*)h->stage, h->d_ctl, 1);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(h, cudaStreamSynchronize(h->stream));
-  h->stats.d2h_bytes += sizeof(PanelCtl);
+  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 1)) return rc;
+  if (int rc = read_ctl(h)) return rc;
   for (int c = 0; c < KT; ++c) R[c0 + c] = (T)(h->h_ctl->xdst[c] - h->h_ctl->xsrc[c]);
   return CS_B200_OK;
 }
-
-template <typename T>
-int solve_pairs_superposed_t(cs_b200_handle* h, int64_t np, const int64_t* nodes, int64_t k,
-                             const int64_t* pi, const int64_t* pj, const double* weight, double rtol,
-                             int64_t itmax, T* R, T* volt, T* curr, int accumulate,
-                             int64_t* point_iters, double* relres);
 
 int ensure_io_pipeline(cs_b200_handle* h) {
   if (h->s_in) return CS_B200_OK;
@@ -1681,13 +1737,10 @@ int rhs_upload(cs_b200_handle* h, int ip, int64_t c0, int kt, const T* rhs) {
 
 template <typename T, int KT>
 int rhs_panel(cs_b200_handle* h, int ip, int64_t c0, T* lhs, double rtol, int64_t itmax,
-              int64_t* iters, double* relres, bool* any_fail, bool* any_maxit, std::string* msg) {
+              int64_t* iters, double* relres, ColumnDriver& cols) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int s = ip & 1;
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
-  for (int c = 0; c < KT; ++c) hc->src[c] = hc->dst[c] = -1;
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
+  if (int rc = upload_ctl(h, KT, [](int) { return ColCtl{-1, -1, 0.0}; })) return rc;
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
   const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
   CK(h, cudaStreamWaitEvent(h->stream, h->ev_in[s], 0));
@@ -1695,9 +1748,7 @@ int rhs_panel(cs_b200_handle* h, int ip, int64_t c0, T* lhs, double rtol, int64_
                                                   (T*)h->B, KT);
   CK(h, cudaEventRecord(h->ev_used[s], h->stream));
   h->stats.kernel_launches++;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  if (rc) return rc;
-  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres)) return rc;
   if (ip >= 2) CK(h, cudaStreamWaitEvent(h->stream, h->ev_out[s], 0));   // slot's last download done
   k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
                                                   (T*)h->io_out[s], h->d_ctl, 0);
@@ -1711,35 +1762,6 @@ int rhs_panel(cs_b200_handle* h, int ip, int64_t c0, T* lhs, double rtol, int64_
   return CS_B200_OK;
 }
 
-#define DISPATCH_KT(kt, CALL)                    \
-  switch (kt) {                                  \
-    case 1: { constexpr int KT = 1; CALL; } break; \
-    case 2: { constexpr int KT = 2; CALL; } break; \
-    case 4: { constexpr int KT = 4; CALL; } break; \
-    default: { constexpr int KT = 8; CALL; } break; \
-  }
-
-template <typename T>
-int solve_pairs_t(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
-                  const double* weight, double rtol, int64_t itmax, T* R, T* volt, T* curr,
-                  int accumulate, int64_t* iters, double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
-  int64_t c0 = 0;
-  while (c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    int rc = 0;
-    DISPATCH_KT(kt, (rc = pairs_panel<T, KT>(h, c0, src, dst, weight, rtol, itmax, R, volt, curr,
-                                             accumulate, iters, relres, &any_fail, &any_maxit,
-                                             &msg)));
-    if (rc) return rc;
-    c0 += kt;
-  }
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
-  return CS_B200_OK;
-}
-
 // ---- focal-region pairs (cs_b200_solve_region_pairs) ----------------------------------------
 // Column c: L w = 0 off the sets, w = 0 on set_a and set_b, right-hand side -L 1_b, so u = w + 1_b
 // holds set_a at 0 V and set_b at 1 V.  flux = u.L u ; v = u / flux ; R = 1 / flux.
@@ -1747,58 +1769,27 @@ template <typename T, int KT>
 int region_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const int64_t* set_rows,
                  const int64_t* set_a, const int64_t* set_b, const double* weight, double rtol,
                  int64_t itmax, T* R, T* volt, T* curr, int accumulate, int64_t* iters, double* relres,
-                 bool* any_fail, bool* any_maxit, std::string* msg) {
+                 ColumnDriver& cols) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int g = ew_grid<T, KT>(h);
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
-  int seg[2 * MAXKT + 1];
-  std::vector<int> rows;
-  seg[0] = 0;
-  for (int c = 0; c < KT; ++c) {
-    hc->src[c] = hc->dst[c] = -1;
-    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
-    for (int side = 0; side < 2; ++side) {
-      const int64_t s = side ? set_b[c0 + c] : set_a[c0 + c];
-      for (int64_t e = set_ptr[s]; e < set_ptr[s + 1]; ++e) rows.push_back((int)set_rows[e]);
-      seg[2 * c + side + 1] = (int)rows.size();
-    }
-  }
-  if (!h->d_rg_seg) CK(h, cudaMalloc(&h->d_rg_seg, (2 * MAXKT + 1) * sizeof(int)));
-  if (rows.size() > h->rg_cap) {
-    CK(h, cudaStreamSynchronize(h->stream));
-    drop_graphs(h->rgraphs);                 // they captured the old address
-    cudaFree(h->d_rg_rows);
-    h->d_rg_rows = nullptr;
-    h->rg_cap = std::max<size_t>(rows.size(), 4096);
-    CK(h, cudaMalloc(&h->d_rg_rows, h->rg_cap * sizeof(int)));
-  }
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
-  CK(h, h2d(h, h->d_rg_seg, seg, (2 * KT + 1) * sizeof(int)));
-  CK(h, h2d(h, h->d_rg_rows, rows.data(), rows.size() * sizeof(int)));
-  h->stats.h2d_bytes += sizeof(PanelCtl) + (2.0 * KT + 1 + rows.size()) * sizeof(int);
+  if (int rc = upload_ctl(h, KT, [&](int c) { return ColCtl{-1, -1, col_weight(weight, c0 + c)}; })) return rc;
+  if (int rc = upload_set_segments(h, KT, set_ptr, set_rows, set_a + c0, set_b + c0)) return rc;
   // B = -L 1_b, zero on the sets (and on the pad rows, which the SpMM does not write)
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
   CK(h, cudaMemsetAsync(h->X, 0, nelem * sizeof(T), h->stream));
   launch_seg_set<T, KT>(h, h->X, 1, T(-1));
   launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->B, nullptr);
   launch_seg_set<T, KT>(h, h->B, 0, T(0));
-  h->rg_on = true;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  h->rg_on = false;
-  if (rc) return rc;
-  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres, true)) return rc;
   // u = w + 1_b (w is zero on the sets); flux = u.L u, second order in the error of w
   launch_seg_set<T, KT>(h, h->X, 1, T(1));
   launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->AP, nullptr);
   k_flux<T, KT><<<g, NT, 0, h->stream>>>(nelem, (size_t)h->n * KT, (const T*)h->X, (const T*)h->AP, h->d_ctl, h->d_partials);
   h->stats.kernel_launches++;
   CK(h, cudaGetLastError());
-  CK(h, cudaMemcpyAsync(hc, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(h, cudaStreamSynchronize(h->stream));
-  h->stats.d2h_bytes += sizeof(PanelCtl);
+  if (int rc = read_ctl(h)) return rc;
   for (int c = 0; c < KT; ++c) {
-    const double flux = hc->xdst[c];
+    const double flux = h->h_ctl->xdst[c];
     if (!(flux > 0.0))
       return set_err(h, CS_B200_ERR_ARG, "region pair %lld: flux into set_b is %g (no conducting path to set_a)",
                      (long long)(c0 + c), flux);
@@ -1817,47 +1808,8 @@ int region_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const in
       h->stats.kernel_launches++;
     }
   }
-  CK(h, cudaGetLastError());
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
-  if (curr) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  if (volt) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
+  if (int rc = download_outputs<T, KT>(h, c0, curr, volt, 0)) return rc;
   CK(h, cudaStreamSynchronize(h->stream));
-  return CS_B200_OK;
-}
-
-template <typename T>
-int solve_region_pairs_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_t* set_rows, int64_t k,
-                         const int64_t* set_a, const int64_t* set_b, const double* weight, double rtol,
-                         int64_t itmax, T* R, T* volt, T* curr, int accumulate, int64_t* iters,
-                         double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
-  int64_t c0 = 0;
-  while (c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    int rc = 0;
-    DISPATCH_KT(kt, (rc = region_panel<T, KT>(h, c0, set_ptr, set_rows, set_a, set_b, weight, rtol, itmax, R,
-                                              volt, curr, accumulate, iters, relres, &any_fail, &any_maxit,
-                                              &msg)));
-    if (rc) return rc;
-    c0 += kt;
-  }
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
   return CS_B200_OK;
 }
 
@@ -1869,142 +1821,26 @@ template <typename T, int KT>
 int grounded_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const int64_t* set_rows,
                    const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
                    const double* weight, double rtol, int64_t itmax, T* src_volt, T* volt, T* curr,
-                   int accumulate, int64_t* iters, double* relres, bool* any_fail, bool* any_maxit,
-                   std::string* msg) {
-  const size_t nelem = (size_t)h->n_pad * KT;
-  PanelCtl* hc = h->h_ctl;
-  std::memset(hc, 0, sizeof(PanelCtl));
-  int seg[2 * MAXKT + 1];
-  int ent_ptr[MAXKT + 1];
-  std::vector<int> rows;
-  seg[0] = 0;
-  const int64_t e0 = src_ptr[c0];
-  for (int c = 0; c < KT; ++c) {
-    hc->src[c] = -1;
-    hc->dst[c] = src_rows[src_ptr[c0 + c]];          // k_pair_extract probes the first source row
-    hc->weight[c] = weight ? weight[c0 + c] : 1.0;
-    const int64_t s = gset[c0 + c];
-    for (int64_t e = set_ptr[s]; e < set_ptr[s + 1]; ++e) rows.push_back((int)set_rows[e]);
-    seg[2 * c + 1] = seg[2 * c + 2] = (int)rows.size();
-    ent_ptr[c] = (int)(src_ptr[c0 + c] - e0);
-  }
-  ent_ptr[KT] = (int)(src_ptr[c0 + KT] - e0);
-  const size_t nent = (size_t)ent_ptr[KT];
-  if (!h->d_rg_seg) CK(h, cudaMalloc(&h->d_rg_seg, (2 * MAXKT + 1) * sizeof(int)));
-  if (rows.size() > h->rg_cap) {
-    CK(h, cudaStreamSynchronize(h->stream));
-    drop_graphs(h->rgraphs);                 // they captured the old address
-    cudaFree(h->d_rg_rows);
-    h->d_rg_rows = nullptr;
-    h->rg_cap = std::max<size_t>(rows.size(), 4096);
-    CK(h, cudaMalloc(&h->d_rg_rows, h->rg_cap * sizeof(int)));
-  }
-  if (nent > h->sp_cap) {
-    cudaFree(h->d_sp_rows); cudaFree(h->d_sp_vals);
-    h->d_sp_rows = nullptr; h->d_sp_vals = nullptr;
-    h->sp_cap = std::max<size_t>(nent, 1024);
-    CK(h, cudaMalloc(&h->d_sp_rows, h->sp_cap * sizeof(long long)));
-    CK(h, cudaMalloc(&h->d_sp_vals, h->sp_cap * sizeof(double)));
-  }
-  if (!h->d_sp_ptr) CK(h, cudaMalloc(&h->d_sp_ptr, (MAXKT + 1) * sizeof(int)));
-  CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
-  CK(h, h2d(h, h->d_rg_seg, seg, (2 * KT + 1) * sizeof(int)));
-  CK(h, h2d(h, h->d_rg_rows, rows.data(), rows.size() * sizeof(int)));
-  CK(h, h2d(h, h->d_sp_ptr, ent_ptr, (KT + 1) * sizeof(int)));
-  CK(h, h2d(h, h->d_sp_rows, src_rows + e0, nent * sizeof(long long)));
-  CK(h, h2d(h, h->d_sp_vals, src_vals + e0, nent * sizeof(double)));
-  h->stats.h2d_bytes += sizeof(PanelCtl) + (2.0 * KT + 1 + rows.size() + KT + 1) * sizeof(int) + nent * 16.0;
+                   int accumulate, int64_t* iters, double* relres, ColumnDriver& cols) {
+  // k_pair_extract probes the first source row
+  if (int rc = upload_ctl(h, KT, [&](int c) {
+        return ColCtl{-1, src_rows[src_ptr[c0 + c]], col_weight(weight, c0 + c)};
+      }))
+    return rc;
+  if (int rc = upload_set_segments(h, KT, set_ptr, set_rows, gset + c0, nullptr)) return rc;
+  if (int rc = upload_sparse_rhs(h, KT, src_ptr + c0, src_rows, src_vals)) return rc;
   // B = sum of the sources, zero on the ground rows (the entry point rejects a source there) and pad rows
-  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
+  CK(h, cudaMemsetAsync(h->B, 0, (size_t)h->n_pad * KT * sizeof(T), h->stream));
   k_sparse_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_sp_ptr, h->d_sp_rows, h->d_sp_vals);
   h->stats.kernel_launches++;
   launch_seg_set<T, KT>(h, h->B, 0, T(0));
-  h->rg_on = true;
-  int rc = solve_panel<T, KT>(h, rtol, itmax);
-  h->rg_on = false;
-  if (rc) return rc;
-  gather_panel_status(h, KT, c0, iters, relres, itmax, any_fail, any_maxit, msg);
+  if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres, true)) return rc;
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
   h->stats.kernel_launches++;
-  if (accumulate || curr) launch_currents<T, KT>(h, curr != nullptr, accumulate);
-  CK(h, cudaGetLastError());
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
-  if (curr) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(curr + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  if (volt) {
-    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->X,
-                                                    (T*)h->stage, h->d_ctl, 0);
-    h->stats.kernel_launches++;
-    CK(h, cudaMemcpyAsync(volt + (size_t)c0 * h->n, h->stage, (size_t)h->n * KT * sizeof(T),
-                          cudaMemcpyDeviceToHost, h->stream));
-    h->stats.d2h_bytes += (double)h->n * KT * sizeof(T);
-  }
-  CK(h, cudaMemcpyAsync(hc, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
-  CK(h, cudaStreamSynchronize(h->stream));
-  h->stats.d2h_bytes += sizeof(PanelCtl);
+  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 0)) return rc;
+  if (int rc = read_ctl(h)) return rc;
   if (src_volt)
-    for (int c = 0; c < KT; ++c) src_volt[c0 + c] = (T)hc->xdst[c];
-  return CS_B200_OK;
-}
-
-template <typename T>
-int solve_grounded_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_t* set_rows, int64_t k,
-                     const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
-                     const double* weight, double rtol, int64_t itmax, T* src_volt, T* volt, T* curr,
-                     int accumulate, int64_t* iters, double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
-  int64_t c0 = 0;
-  while (c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    int rc = 0;
-    DISPATCH_KT(kt, (rc = grounded_panel<T, KT>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals,
-                                                weight, rtol, itmax, src_volt, volt, curr, accumulate, iters,
-                                                relres, &any_fail, &any_maxit, &msg)));
-    if (rc) return rc;
-    c0 += kt;
-  }
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
-  return CS_B200_OK;
-}
-
-template <typename T>
-int solve_sources_t(cs_b200_handle* h, int64_t k, const int64_t* colptr, const int64_t* rows,
-                    const double* vals, const int64_t* ref, const double* weight, double rtol,
-                    int64_t itmax, int64_t nprobe, const int64_t* probe, T* probe_volt, T* volt,
-                    T* curr, int accumulate, int64_t* iters, double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
-  if (nprobe > 0 && probe_volt) {
-    const size_t need = (size_t)nprobe;
-    if (need > h->probe_cap) {
-      cudaFree(h->d_probe); cudaFree(h->d_probe_out);
-      h->d_probe = nullptr; h->d_probe_out = nullptr;
-      h->probe_cap = need;
-      CK(h, cudaMalloc(&h->d_probe, need * sizeof(long long)));
-      CK(h, cudaMalloc(&h->d_probe_out, need * MAXKT * sizeof(double)));
-    }
-    CK(h, h2d(h, h->d_probe, probe, need * sizeof(long long)));
-  }
-  int64_t c0 = 0;
-  while (c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    int rc = 0;
-    DISPATCH_KT(kt, (rc = sources_panel<T, KT>(h, c0, colptr, rows, vals, ref, weight, rtol, itmax,
-                                               nprobe, probe_volt, volt, curr, accumulate, iters,
-                                               relres, &any_fail, &any_maxit, &msg)));
-    if (rc) return rc;
-    c0 += kt;
-  }
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
+    for (int c = 0; c < KT; ++c) src_volt[c0 + c] = (T)h->h_ctl->xdst[c];
   return CS_B200_OK;
 }
 
@@ -2012,9 +1848,7 @@ template <typename T>
 int solve_pairs_superposed_t(cs_b200_handle* h, int64_t np, const int64_t* nodes, int64_t k,
                              const int64_t* pi, const int64_t* pj, const double* weight, double rtol,
                              int64_t itmax, T* R, T* volt, T* curr, int accumulate,
-                             int64_t* point_iters, double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
+                             int64_t* point_iters, double* relres, ColumnDriver& cols) {
   T* U = nullptr;
   int *d_ci = nullptr, *d_cj = nullptr;
   const size_t ubytes = (size_t)h->n_pad * (size_t)(np - 1) * sizeof(T);
@@ -2028,62 +1862,41 @@ int solve_pairs_superposed_t(cs_b200_handle* h, int64_t np, const int64_t* nodes
     return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s allocating %zu bytes for the point solutions",
                    cudaGetErrorString(e), ubytes);
   }
-  int rc = 0;
-  int64_t x0 = 1;
-  while (!rc && x0 < np) {
-    const int kt = next_kt(np - x0, h->ktmax);
-    DISPATCH_KT(kt, (rc = point_panel<T, KT>(h, x0, nodes, rtol, itmax, U, point_iters, &any_fail,
-                                             &any_maxit, &msg)));
-    x0 += kt;
-  }
-  int64_t c0 = 0;
-  while (!rc && c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    DISPATCH_KT(kt, (rc = combine_panel<T, KT>(h, c0, nodes, pi, pj, weight, U, d_ci, d_cj, R, volt, curr,
-                                               accumulate, relres, itmax, &any_fail, &any_maxit, &msg)));
-    c0 += kt;
-  }
+  int rc = cols.run(1, np, [&](auto kt, int64_t x0) {
+    return point_panel<T, kt>(h, x0, nodes, rtol, itmax, U, point_iters, cols);
+  });
+  if (!rc)
+    rc = cols.run(0, k, [&](auto kt, int64_t c0) {
+      return combine_panel<T, kt>(h, c0, nodes, pi, pj, weight, U, d_ci, d_cj, R, volt, curr, accumulate, relres,
+                                  itmax, cols);
+    });
   cudaStreamSynchronize(h->stream);
   cleanup();
-  if (rc) return rc;
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
-  return CS_B200_OK;
+  return rc;
 }
 
 template <typename T>
 int solve_rhs_t(cs_b200_handle* h, int64_t k, const T* rhs, T* lhs, double rtol, int64_t itmax,
-                int64_t* iters, double* relres) {
-  bool any_fail = false, any_maxit = false;
-  std::string msg;
+                int64_t* iters, double* relres, ColumnDriver& cols) {
   int rc = ensure_io_pipeline(h);
   if (rc) return rc;
   // the upload stream must not overtake work of an earlier call that still reads the slots
   CK(h, cudaEventRecord(h->ev_used[0], h->stream));
   CK(h, cudaStreamWaitEvent(h->s_in, h->ev_used[0], 0));
-  int64_t c0 = 0;
   int ip = 0;
   rc = rhs_upload<T>(h, 0, 0, next_kt(k, h->ktmax), rhs);
-  while (!rc && c0 < k) {
-    const int kt = next_kt(k - c0, h->ktmax);
-    const int64_t c1 = c0 + kt;
-    if (c1 < k) {   // next panel's upload overlaps this panel's solve
-      rc = rhs_upload<T>(h, ip + 1, c1, next_kt(k - c1, h->ktmax), rhs);
-      if (rc) break;
-    }
-    DISPATCH_KT(kt, (rc = rhs_panel<T, KT>(h, ip, c0, lhs, rtol, itmax, iters, relres, &any_fail,
-                                           &any_maxit, &msg)));
-    c0 = c1;
-    ++ip;
-  }
+  if (!rc)
+    rc = cols.run(0, k, [&](auto kt, int64_t c0) {
+      const int64_t c1 = c0 + kt;
+      if (c1 < k)   // next panel's upload overlaps this panel's solve
+        if (int urc = rhs_upload<T>(h, ip + 1, c1, next_kt(k - c1, h->ktmax), rhs)) return urc;
+      return rhs_panel<T, kt>(h, ip++, c0, lhs, rtol, itmax, iters, relres, cols);
+    });
   // drain both copy streams whatever happened: the caller owns rhs/lhs again on return
   cudaStreamSynchronize(h->s_in);
   cudaStreamSynchronize(h->s_out);
   cudaStreamSynchronize(h->stream);
-  if (rc) return rc;
-  if (any_fail) return set_err(h, CS_B200_ERR_RESIDUAL, "%s", msg.c_str());
-  if (any_maxit) return set_err(h, CS_B200_ERR_MAXITER, "itmax reached (or the recurrence stagnated) before rtol");
-  return CS_B200_OK;
+  return rc;
 }
 
 void begin_call(cs_b200_handle* h) {
@@ -2100,6 +1913,18 @@ void end_call(cs_b200_handle* h) {
   float ms = 0;
   cudaEventElapsedTime(&ms, h->ev0, h->ev1);
   h->stats.solve_ms = ms;
+}
+
+// a batched solve entry's call: solve(T{}, cols) in the handle's element type T, then the verdict of the
+// column driver, between begin_call and end_call
+template <typename Solve>
+int solve_call(cs_b200_handle* h, Solve&& solve) {
+  if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
+  begin_call(h);
+  ColumnDriver cols{h};
+  const int rc = cols.verdict(h->dtype == CS_B200_F64 ? solve(double{}, cols) : solve(float{}, cols));
+  end_call(h);
+  return rc;
 }
 
 int ensure_flush(cs_b200_handle* h) {
@@ -2931,12 +2756,10 @@ int cs_b200_solve_rhs(cs_b200_handle* h, int64_t k, const void* rhs, void* lhs, 
                       int64_t itmax, int64_t* iters, double* relres) {
   if (!h || k < 1 || !rhs || !lhs || !(rtol >= 0) || itmax < 0)
     return set_err(h, CS_B200_ERR_ARG, "bad solve_rhs arguments");
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_rhs_t<double>(h, k, (const double*)rhs, (double*)lhs, rtol, itmax, iters, relres)
-               : solve_rhs_t<float>(h, k, (const float*)rhs, (float*)lhs, rtol, itmax, iters, relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return solve_rhs_t<T>(h, k, (const T*)rhs, (T*)lhs, rtol, itmax, iters, relres, cols);
+  });
 }
 
 int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
@@ -2948,14 +2771,13 @@ int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const 
     if (src[c] < 0 || src[c] >= h->n || dst[c] < 0 || dst[c] >= h->n || src[c] == dst[c])
       return set_err(h, CS_B200_ERR_ARG, "pair %lld: src/dst out of range or equal (%lld, %lld)",
                      (long long)c, (long long)src[c], (long long)dst[c]);
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_pairs_t<double>(h, k, src, dst, weight, rtol, itmax, (double*)R,
-                                       (double*)volt, (double*)curr, accumulate, iters, relres)
-               : solve_pairs_t<float>(h, k, src, dst, weight, rtol, itmax, (float*)R, (float*)volt,
-                                      (float*)curr, accumulate, iters, relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      return pairs_panel<T, kt>(h, c0, src, dst, weight, rtol, itmax, (T*)R, (T*)volt, (T*)curr, accumulate,
+                                iters, relres, cols);
+    });
+  });
 }
 
 int cs_b200_solve_sources(cs_b200_handle* h, int64_t k, const int64_t* colptr, const int64_t* rows,
@@ -2976,16 +2798,15 @@ int cs_b200_solve_sources(cs_b200_handle* h, int64_t k, const int64_t* colptr, c
       return set_err(h, CS_B200_ERR_ARG, "entry %lld: row %lld out of range", (long long)e, (long long)rows[e]);
   for (int64_t i = 0; i < nprobe; ++i)
     if (probe[i] < 0 || probe[i] >= h->n) return set_err(h, CS_B200_ERR_ARG, "probe row out of range");
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_sources_t<double>(h, k, colptr, rows, vals, ref, weight, rtol, itmax, nprobe, probe,
-                                         (double*)probe_volt, (double*)volt, (double*)curr, accumulate,
-                                         iters, relres)
-               : solve_sources_t<float>(h, k, colptr, rows, vals, ref, weight, rtol, itmax, nprobe, probe,
-                                        (float*)probe_volt, (float*)volt, (float*)curr, accumulate, iters,
-                                        relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    if (nprobe > 0 && probe_volt)
+      if (int rc = upload_probe(h, nprobe, probe)) return rc;
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      return sources_panel<T, kt>(h, c0, colptr, rows, vals, ref, weight, rtol, itmax, nprobe, (T*)probe_volt,
+                                  (T*)volt, (T*)curr, accumulate, iters, relres, cols);
+    });
+  });
 }
 
 int cs_b200_solve_pairs_superposed(cs_b200_handle* h, int64_t np, const int64_t* nodes, int64_t k,
@@ -3003,14 +2824,11 @@ int cs_b200_solve_pairs_superposed(cs_b200_handle* h, int64_t np, const int64_t*
   for (int64_t c = 0; c < k; ++c)
     if (pi[c] < 0 || pi[c] >= np || pj[c] < 0 || pj[c] >= np || nodes[pi[c]] == nodes[pj[c]])
       return set_err(h, CS_B200_ERR_ARG, "pair %lld: indices out of range or equal nodes", (long long)c);
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_pairs_superposed_t<double>(h, np, nodes, k, pi, pj, weight, rtol, itmax, (double*)R,
-                                                  (double*)volt, (double*)curr, accumulate, point_iters, relres)
-               : solve_pairs_superposed_t<float>(h, np, nodes, k, pi, pj, weight, rtol, itmax, (float*)R,
-                                                 (float*)volt, (float*)curr, accumulate, point_iters, relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return solve_pairs_superposed_t<T>(h, np, nodes, k, pi, pj, weight, rtol, itmax, (T*)R, (T*)volt, (T*)curr,
+                                       accumulate, point_iters, relres, cols);
+  });
 }
 
 // the sets of one CSR (set_ptr[nsets+1], set_rows): non-empty, sorted, unique, rows in range
@@ -3052,15 +2870,13 @@ int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* 
       if (set_rows[i] < set_rows[j]) ++i; else ++j;
     }
   }
-  if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_region_pairs_t<double>(h, set_ptr, set_rows, k, set_a, set_b, weight, rtol, itmax,
-                                              (double*)R, (double*)volt, (double*)curr, accumulate, iters, relres)
-               : solve_region_pairs_t<float>(h, set_ptr, set_rows, k, set_a, set_b, weight, rtol, itmax,
-                                             (float*)R, (float*)volt, (float*)curr, accumulate, iters, relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      return region_panel<T, kt>(h, c0, set_ptr, set_rows, set_a, set_b, weight, rtol, itmax, (T*)R, (T*)volt,
+                                 (T*)curr, accumulate, iters, relres, cols);
+    });
+  });
 }
 
 int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
@@ -3091,17 +2907,13 @@ int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_
                        (long long)r, (long long)s);
     }
   }
-  if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
-  begin_call(h);
-  int rc = h->dtype == CS_B200_F64
-               ? solve_grounded_t<double>(h, set_ptr, set_rows, k, gset, src_ptr, src_rows, src_vals, weight, rtol,
-                                          itmax, (double*)src_volt, (double*)volt, (double*)curr, accumulate, iters,
-                                          relres)
-               : solve_grounded_t<float>(h, set_ptr, set_rows, k, gset, src_ptr, src_rows, src_vals, weight, rtol,
-                                         itmax, (float*)src_volt, (float*)volt, (float*)curr, accumulate, iters,
-                                         relres);
-  end_call(h);
-  return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      return grounded_panel<T, kt>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals, weight, rtol,
+                                   itmax, (T*)src_volt, (T*)volt, (T*)curr, accumulate, iters, relres, cols);
+    });
+  });
 }
 
 }  // extern "C"

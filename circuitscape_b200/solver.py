@@ -70,6 +70,19 @@ class CUDASolver:
         return self.dtype
 
 
+def _opt(a, dtype):
+    """None, or `a` as a contiguous array of `dtype` (the optional per-column inputs)."""
+    return None if a is None else np.ascontiguousarray(a, dtype=dtype)
+
+
+def _csr(ragged, dtype):
+    """A ragged list of 1-D arrays as CSR: (ptr (len + 1,) int64, the arrays concatenated as `dtype`)."""
+    ptr = np.zeros(len(ragged) + 1, dtype=np.int64)
+    ptr[1:] = np.cumsum([len(a) for a in ragged])
+    vals = np.concatenate([np.asarray(a, dtype=dtype) for a in ragged]) if len(ragged) else np.zeros(0)
+    return ptr, np.ascontiguousarray(vals, dtype=dtype)
+
+
 class SolverResidualError(RuntimeError):
     """The reference's `error("... residual $r exceeds tolerance 1e-4 ...")`
     (src/core.jl:641,650)."""
@@ -239,6 +252,19 @@ class B200Factor:
         self.close()
 
     # -- calls ------------------------------------------------------------
+    def _limits(self, rtol, itmax):
+        """rtol and itmax of one call: the solver's unless given."""
+        return (self.solver.rtol if rtol is None else rtol, self.solver.itmax if itmax is None else itmax)
+
+    def _columns(self, k, want_volt, want_curr):
+        """Per-column outputs of a batched solve: volt, curr (n, k) F-ordered or None, iters, relres."""
+        cols = lambda want: np.empty((self.n, k), dtype=self.dtype, order="F") if want else None
+        return cols(want_volt), cols(want_curr), np.zeros(k, dtype=np.int64), np.zeros(k, dtype=np.float64)
+
+    def _io(self, a):
+        """`a` (or None) in the caller's element type io_dtype."""
+        return a.astype(self.io_dtype) if a is not None and self.io_dtype != self.dtype else a
+
     def stats(self):
         st = _lib.Stats()
         self._lib.cs_b200_get_stats(self._h, C.byref(st))
@@ -327,13 +353,11 @@ class B200Factor:
         assert x.flags.f_contiguous and x.shape == b.shape and x.dtype == b.dtype
         iters = np.zeros(k, dtype=np.int64)
         relres = np.zeros(k, dtype=np.float64)
-        rc = self._lib.cs_b200_solve_rhs(self._h, k, _lib._ptr(b), _lib._ptr(x),
-                                         self.solver.rtol if rtol is None else rtol,
-                                         self.solver.itmax if itmax is None else itmax,
+        rc = self._lib.cs_b200_solve_rhs(self._h, k, _lib._ptr(b), _lib._ptr(x), *self._limits(rtol, itmax),
                                          _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if out is None and self.io_dtype != self.dtype:
-            x = x.astype(self.io_dtype)
+        if out is None:
+            x = self._io(x)
         return (x[:, 0] if vec else x), iters, relres
 
     def solve_pairs(self, src, dst, weight=None, want_volt=False, want_curr=False,
@@ -343,23 +367,14 @@ class B200Factor:
         src = np.ascontiguousarray(src, dtype=np.int64)
         dst = np.ascontiguousarray(dst, dtype=np.int64)
         k = len(src)
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
         R = np.zeros(k, dtype=self.dtype)
-        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
-        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
-        iters = np.zeros(k, dtype=np.int64)
-        relres = np.zeros(k, dtype=np.float64)
-        rc = self._lib.cs_b200_solve_pairs(self._h, k, _lib._ptr(src), _lib._ptr(dst), _lib._ptr(w),
-                                           self.solver.rtol if rtol is None else rtol,
-                                           self.solver.itmax if itmax is None else itmax,
-                                           _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr),
-                                           1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+        volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
+        rc = self._lib.cs_b200_solve_pairs(self._h, k, _lib._ptr(src), _lib._ptr(dst),
+                                           _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax),
+                                           _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0,
+                                           _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if self.io_dtype != self.dtype:
-            R = R.astype(self.io_dtype)
-            volt = None if volt is None else volt.astype(self.io_dtype)
-            curr = None if curr is None else curr.astype(self.io_dtype)
-        return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
+        return dict(R=self._io(R), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
     def solve_pairs_superposed(self, nodes, pi, pj, weight=None, want_volt=False, want_curr=False,
                                accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
@@ -370,23 +385,15 @@ class B200Factor:
         pi = np.ascontiguousarray(pi, dtype=np.int64)
         pj = np.ascontiguousarray(pj, dtype=np.int64)
         k = len(pi)
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
         R = np.zeros(k, dtype=self.dtype)
-        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
-        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
+        volt, curr, _, relres = self._columns(k, want_volt, want_curr)
         iters = np.zeros(max(len(nodes) - 1, 1), dtype=np.int64)
-        relres = np.zeros(k, dtype=np.float64)
         rc = self._lib.cs_b200_solve_pairs_superposed(
-            self._h, len(nodes), _lib._ptr(nodes), k, _lib._ptr(pi), _lib._ptr(pj), _lib._ptr(w),
-            self.solver.rtol if rtol is None else rtol, self.solver.itmax if itmax is None else itmax,
-            _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters),
-            _lib._ptr(relres))
+            self._h, len(nodes), _lib._ptr(nodes), k, _lib._ptr(pi), _lib._ptr(pj),
+            _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax), _lib._ptr(R), _lib._ptr(volt),
+            _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if self.io_dtype != self.dtype:
-            R = R.astype(self.io_dtype)
-            volt = None if volt is None else volt.astype(self.io_dtype)
-            curr = None if curr is None else curr.astype(self.io_dtype)
-        return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
+        return dict(R=self._io(R), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
     def solve_region_pairs(self, sets, set_a, set_b, weight=None, want_volt=False, want_curr=False,
                            accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
@@ -395,31 +402,18 @@ class B200Factor:
         normalisation.  sets: list of 0-based row arrays (sorted, unique, non-empty).  Returns the dict
         of solve_pairs: R = 1 / flux, volt (0 on set_a, R on set_b), curr (every row of a set carries
         its merged node's current)."""
-        ptr = np.zeros(len(sets) + 1, dtype=np.int64)
-        for s, r in enumerate(sets):
-            ptr[s + 1] = ptr[s] + len(r)
-        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r in sets])
-                                    if len(sets) else np.zeros(0), dtype=np.int64)
+        ptr, rows = _csr(sets, np.int64)
         set_a = np.ascontiguousarray(set_a, dtype=np.int64)
         set_b = np.ascontiguousarray(set_b, dtype=np.int64)
         k = len(set_a)
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
         R = np.zeros(k, dtype=self.dtype)
-        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
-        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
-        iters = np.zeros(k, dtype=np.int64)
-        relres = np.zeros(k, dtype=np.float64)
+        volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
         rc = self._lib.cs_b200_solve_region_pairs(
             self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(set_a), _lib._ptr(set_b),
-            _lib._ptr(w), self.solver.rtol if rtol is None else rtol,
-            self.solver.itmax if itmax is None else itmax, _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr),
-            1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+            _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax), _lib._ptr(R), _lib._ptr(volt),
+            _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if self.io_dtype != self.dtype:
-            R = R.astype(self.io_dtype)
-            volt = None if volt is None else volt.astype(self.io_dtype)
-            curr = None if curr is None else curr.astype(self.io_dtype)
-        return dict(R=R, volt=volt, curr=curr, iters=iters, relres=relres)
+        return dict(R=self._io(R), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
     def solve_grounded(self, sets, gset, sources, weight=None, want_volt=False, want_curr=False,
                        accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
@@ -428,39 +422,22 @@ class B200Factor:
         on the column's ground set).  sets: list of 0-based row arrays (sorted, unique, non-empty).
         Returns dict with src_volt (v at each column's first source row), volt, curr (every ground row is
         a node of its own), iters, relres."""
-        ptr = np.zeros(len(sets) + 1, dtype=np.int64)
-        for s, r in enumerate(sets):
-            ptr[s + 1] = ptr[s] + len(r)
-        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r in sets])
-                                    if len(sets) else np.zeros(0), dtype=np.int64)
+        ptr, rows = _csr(sets, np.int64)
         gset = np.ascontiguousarray(gset, dtype=np.int64)
         k = len(gset)
         assert len(sources) == k
-        sptr = np.zeros(k + 1, dtype=np.int64)
-        for c, (r, _) in enumerate(sources):
-            sptr[c + 1] = sptr[c] + len(r)
-        srows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r, _ in sources])
-                                     if k else np.zeros(0), dtype=np.int64)
-        svals = np.ascontiguousarray(np.concatenate([np.asarray(v, dtype=np.float64) for _, v in sources])
-                                     if k else np.zeros(0), dtype=np.float64)
+        sptr, srows = _csr([r for r, _ in sources], np.int64)
+        _, svals = _csr([v for _, v in sources], np.float64)
         assert len(srows) == len(svals) == sptr[-1]
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
         sv = np.zeros(k, dtype=self.dtype)
-        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
-        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
-        iters = np.zeros(k, dtype=np.int64)
-        relres = np.zeros(k, dtype=np.float64)
+        volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
         rc = self._lib.cs_b200_solve_grounded(
             self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(gset), _lib._ptr(sptr),
-            _lib._ptr(srows), _lib._ptr(svals), _lib._ptr(w), self.solver.rtol if rtol is None else rtol,
-            self.solver.itmax if itmax is None else itmax, _lib._ptr(sv), _lib._ptr(volt), _lib._ptr(curr),
-            1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+            _lib._ptr(srows), _lib._ptr(svals), _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax),
+            _lib._ptr(sv), _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters),
+            _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if self.io_dtype != self.dtype:
-            sv = sv.astype(self.io_dtype)
-            volt = None if volt is None else volt.astype(self.io_dtype)
-            curr = None if curr is None else curr.astype(self.io_dtype)
-        return dict(src_volt=sv, volt=volt, curr=curr, iters=iters, relres=relres)
+        return dict(src_volt=self._io(sv), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
     def solve_sources(self, columns, ref, probe=None, weight=None, want_volt=False, want_curr=False,
                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
@@ -469,36 +446,21 @@ class B200Factor:
         (0-based rows); ref[c]: row whose voltage is subtracted (the ground).  Returns dict
         with probe_volt (k, len(probe))|None, volt, curr, iters, relres."""
         k = len(columns)
-        colptr = np.zeros(k + 1, dtype=np.int64)
-        for c, (r, _) in enumerate(columns):
-            colptr[c + 1] = colptr[c] + len(r)
-        rows = np.ascontiguousarray(np.concatenate([np.asarray(r, dtype=np.int64) for r, _ in columns])
-                                    if k else np.zeros(0), dtype=np.int64)
-        vals = np.ascontiguousarray(np.concatenate([np.asarray(v, dtype=np.float64) for _, v in columns])
-                                    if k else np.zeros(0), dtype=np.float64)
+        colptr, rows = _csr([r for r, _ in columns], np.int64)
+        _, vals = _csr([v for _, v in columns], np.float64)
         ref = np.ascontiguousarray(ref, dtype=np.int64)
         assert len(ref) == k and len(rows) == len(vals) == colptr[-1]
-        w = None if weight is None else np.ascontiguousarray(weight, dtype=np.float64)
-        pr = None if probe is None else np.ascontiguousarray(probe, dtype=np.int64)
+        pr = _opt(probe, np.int64)
         npr = 0 if pr is None else len(pr)
         pv = np.zeros((k, npr), dtype=self.dtype) if npr else None
-        volt = np.empty((self.n, k), dtype=self.dtype, order="F") if want_volt else None
-        curr = np.empty((self.n, k), dtype=self.dtype, order="F") if want_curr else None
-        iters = np.zeros(k, dtype=np.int64)
-        relres = np.zeros(k, dtype=np.float64)
+        volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
         rc = self._lib.cs_b200_solve_sources(self._h, k, _lib._ptr(colptr), _lib._ptr(rows), _lib._ptr(vals),
-                                             _lib._ptr(ref), _lib._ptr(w),
-                                             self.solver.rtol if rtol is None else rtol,
-                                             self.solver.itmax if itmax is None else itmax,
-                                             npr, _lib._ptr(pr), _lib._ptr(pv), _lib._ptr(volt),
-                                             _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters),
-                                             _lib._ptr(relres))
+                                             _lib._ptr(ref), _lib._ptr(_opt(weight, np.float64)),
+                                             *self._limits(rtol, itmax), npr, _lib._ptr(pr), _lib._ptr(pv),
+                                             _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0,
+                                             _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
-        if self.io_dtype != self.dtype:
-            pv = None if pv is None else pv.astype(self.io_dtype)
-            volt = None if volt is None else volt.astype(self.io_dtype)
-            curr = None if curr is None else curr.astype(self.io_dtype)
-        return dict(probe_volt=pv, volt=volt, curr=curr, iters=iters, relres=relres)
+        return dict(probe_volt=self._io(pv), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
     def read_currents(self, want_max=True):
         cum = np.empty(self.n, dtype=self.dtype)
