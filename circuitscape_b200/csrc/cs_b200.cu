@@ -819,6 +819,27 @@ CsrDev<T> view(const DevCsr& m) {
   return CsrDev<T>{m.rowptr, m.colidx, (const T*)m.vals, m.bstart, m.nblocks, m.nrows};
 }
 
+// the stencil kernels stage their operands through the shared-memory pipeline (kernels.cuh k_stencil_pipe,
+// k_stencil_cg_pipe); CS_B200_NO_STENCIL_PIPE keeps the register-gather kernels for A/B runs
+inline bool stencil_pipe() {
+  static const bool off = std::getenv("CS_B200_NO_STENCIL_PIPE") != nullptr;
+  return !off;
+}
+
+// k_stencil<T, KT, MODE> on grid sg, through the pipeline unless it is switched off
+template <typename T, int KT, int MODE>
+void launch_stencil(cs_b200_handle* h, const DiaDev<T>& a, const T* X, T* Y, const SpmmEpi<T>& ep, int sg) {
+  if (!stencil_pipe()) {
+    k_stencil<T, KT, MODE><<<sg, NT, 0, h->stream>>>(a, X, Y, ep);
+    return;
+  }
+  constexpr int SMEM = StPipe<T, KT, MODE>::D::BYTES;
+  static bool once[64] = {};   // per device: the attribute lives in the device's context
+  bool& set = once[h->device & 63];
+  if (!set) { cudaFuncSetAttribute(k_stencil_pipe<T, KT, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  k_stencil_pipe<T, KT, MODE><<<sg, NT, SMEM, h->stream>>>(a, X, Y, ep);
+}
+
 // Y = op(M X) with the fused epilogue MODE (kernels.cuh).  `timed`: counts as a launch of
 // the dominant kernel for the per-launch profile (finest-level operator only).
 template <typename T, int KT, int MODE>
@@ -855,7 +876,7 @@ void launch_spmm_on(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const 
       const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
                                ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
       const int sg = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));
-      k_stencil<T, KT, MODE><<<sg, NT, 0, h->stream>>>(a, X, Y, ep);
+      launch_stencil<T, KT, MODE>(h, a, X, Y, ep, sg);
     }
   } else if (m.win_meta) {
     const WinCsr<T> w{m.win_meta, m.blob, m.has_dinv, m.rowptr, m.colidx, (const T*)m.vals, m.win_nblocks};
@@ -959,7 +980,7 @@ void launch_stencil_res0(cs_b200_handle* h, DevLevel& L, const T* B, T* Tout, bo
     h->prof_pair_bytes.push_back(fb);
     cudaEventRecord(e0, h->stream);
   }
-  k_stencil<T, KT, SP_RES0><<<sg, NT, 0, h->stream>>>(a, nullptr, Tout, ep);
+  launch_stencil<T, KT, SP_RES0>(h, a, nullptr, Tout, ep, sg);
   if (prof) cudaEventRecord(e1, h->stream);
   h->stats.kernel_launches++;
   if (timed) h->stats.spmm_launches++;
@@ -1141,8 +1162,17 @@ void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
     h->prof_pair_bytes.push_back(fb);
     cudaEventRecord(e0, h->stream);
   }
-  k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
-                                                     h->d_partials);
+  if (stencil_pipe()) {
+    constexpr int SMEM = StPipeCg<T, KT, TV>::D::BYTES;
+    static bool once[64] = {};
+    bool& set = once[h->device & 63];
+    if (!set) { cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+    k_stencil_cg_pipe<T, KT, TV><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP,
+                                                              h->d_ctl, h->d_partials);
+  } else {
+    k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
+                                                       h->d_partials);
+  }
   if (h->profile) cudaEventRecord(e1, h->stream);
   h->stats.kernel_launches++;
   h->stats.spmm_launches++;

@@ -1204,6 +1204,410 @@ k_stencil_cg(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __r
 }
 
 // ---------------------------------------------------------------------------
+// Pipelined stencil sweeps (k_stencil_pipe, k_stencil_cg_pipe).  Tiles, tile walk, grid, thread map, each thread's
+// order of (tile, column) steps, the 9-slot FMA order and every epilogue are those of k_stencil / k_stencil_cg, so
+// the outputs and the per-CTA partial sums are bit-identical to theirs.  What changes is how operands arrive: a
+// CTA's tiles form one flat sequence of load steps -- tile (tc, rc) loads the raster columns 16 tc - 1 ... ce
+// (ce = the tile's last column + 1) -- and every load step is filled by cp.async S steps ahead of its use, across
+// tile boundaries.  The step that loads column c + 1 computes column c.  Two rings in dynamic shared memory:
+//   panel ring (S + 3 slots): rows [c nr + r0 - 1, c nr + r0 + RPP] of each gathered panel, one contiguous range:
+//     the +-1 neighbours of a row are rows of the same slot, the +-nr ones the same rows of the slots of c -+ 1
+//   own ring (S + 1 slots): the 9 diagonal runs of the RPP rows of column c and the own-row streams the step reads
+// A slot is rewritten three (panel) or one (own) step after its last read, behind the step's barrier.  Rows
+// outside [0, n) are zero-filled by the copy (src-size 0): such a neighbour has a zero diagonal, and 0 x 0 adds
+// nothing to a sum, as 0 x (the clamped row) does in the register kernels.  Every thread takes part in every copy
+// and barrier; rows past nr or n only mask their compute and stores.
+// Depth S: the largest (<= ST_SMAX) whose rings fit the shared memory of MINB CTAs per SM.  On an H100 80GB HBM3
+// (700 W), 3163^2 raster, k = 8: the fused CG step (fp64, fp32 z; S = 2 at 3 CTAs/SM, 80 registers) 1.425 ms per
+// step against 1.656 ms for k_stencil_cg, the fp32 level-0 residual (S = 4 at 3 CTAs/SM) 383 us against 418 us.
+// Other S x CTAs/SM points were not measured.
+// ---------------------------------------------------------------------------
+constexpr int ST_SMAX = 4;
+constexpr int st_a16(int b) { return (b + 15) & ~15; }
+
+template <int PANEL, int OWN, int MINB> struct StDepth {
+  static constexpr int BUDGET = 228 * 1024 / MINB - 1024 - 3 * 1024;   // less the per-CTA reserve, static buffers
+  static constexpr int FIT = (BUDGET - 3 * PANEL - OWN) / (PANEL + OWN);
+  static constexpr int S = FIT < 1 ? 1 : (FIT > ST_SMAX ? ST_SMAX : FIT);
+  static constexpr int BYTES = (S + 3) * PANEL + (S + 1) * OWN;
+};
+
+template <int B>
+__device__ __forceinline__ void cp_async_zfill(void* dst, const void* src, bool ok) {
+  const int sz = ok ? B : 0;
+  if constexpr (B == 16)
+    asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(smem_u32(dst)), "l"(src), "r"(sz) : "memory");
+  else
+    asm volatile("cp.async.ca.shared.global [%0], [%1], %2, %3;" ::"r"(smem_u32(dst)), "l"(src), "n"(B), "r"(sz)
+                 : "memory");
+}
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+template <int N> __device__ __forceinline__ void cp_async_wait() {
+  asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
+}
+
+// rows [g0, g0 + NROWS) of a panel of W values per row, zero outside [0, n); chunks of min(16, row) bytes
+template <typename U, int W, int NROWS>
+__device__ __forceinline__ void cp_rows(U* dst, const U* src, long long g0, int n) {
+  constexpr int RB = W * (int)sizeof(U);
+  constexpr int CH = RB < 16 ? RB : 16;
+  constexpr int CPR = RB / CH;
+  constexpr int NCH = NROWS * CPR;
+#pragma unroll 1
+  for (int q0 = 0; q0 < NCH; q0 += NT) {
+    const int q = q0 + (int)threadIdx.x;
+    if (NCH % NT == 0 || q < NCH) {
+      const long long g = g0 + q / CPR;
+      const bool ok = g >= 0 && g < n;
+      cp_async_zfill<CH>(reinterpret_cast<char*>(dst) + q * CH,
+                         reinterpret_cast<const char*>(src + (ok ? g : 0) * W) + (q % CPR) * CH, ok);
+    }
+  }
+}
+
+// the 9 diagonal runs of rows [row0, row0 + RPP), slot-major, zero past n
+template <typename T, int RPP>
+__device__ __forceinline__ void cp_diag(T* dst, const DiaDev<T>& A, long long row0) {
+  constexpr int NCH = 9 * RPP;
+#pragma unroll 1
+  for (int q0 = 0; q0 < NCH; q0 += NT) {
+    const int q = q0 + (int)threadIdx.x;
+    if (NCH % NT == 0 || q < NCH) {
+      const long long g = row0 + q % RPP;
+      const bool ok = g < A.n;
+      cp_async_zfill<(int)sizeof(T)>(dst + q, A.vals + (size_t)(q / RPP) * A.ld + (ok ? g : 0), ok);
+    }
+  }
+}
+
+// one load step of a CTA's sequence: tile t, raster column c in [cs - 1, ce]
+struct StStep {
+  long long t;
+  int cs, ce, c, r0;
+  __device__ __forceinline__ void start(long long t_, int nrc, int ncol, int rpp) {
+    t = t_;
+    r0 = (int)(t % nrc) * rpp;
+    cs = (int)(t / nrc) * ST_TC;
+    ce = min(ncol, cs + ST_TC);
+    c = cs - 1;
+  }
+  __device__ __forceinline__ void next(int nrc, int ncol, int rpp) {
+    if (++c > ce) start(t + gridDim.x, nrc, ncol, rpp);
+  }
+};
+
+// issue(step, panel slot, own slot) fills the slots of a load step; compute(step, panel slot, own slot) runs on the
+// step that loaded column step.c, for column step.c - 1, reading panel slots (slot - 2, slot - 1, slot) mod S + 3
+template <int S, int RPP, class Issue, class Compute>
+__device__ __forceinline__ void stencil_pipe(int n, int nr, Issue&& issue, Compute&& compute) {
+  constexpr int RP = S + 3, RO = S + 1;
+  const int ncol = (n + nr - 1) / nr;
+  const int nrc = (nr + RPP - 1) / RPP;
+  const long long ntiles = (long long)nrc * ((ncol + ST_TC - 1) / ST_TC);
+  StStep ld, st;
+  ld.start(blockIdx.x, nrc, ncol, RPP);
+  st = ld;
+  int lp = 0, lo = 0, sp = 0, so = 0;
+#pragma unroll 1
+  for (int k = 0; k < S; ++k) {
+    if (ld.t < ntiles) issue(ld, lp, lo);
+    cp_async_commit();
+    ld.next(nrc, ncol, RPP);
+    lp = lp + 1 == RP ? 0 : lp + 1;
+    lo = lo + 1 == RO ? 0 : lo + 1;
+  }
+#pragma unroll 1
+  while (st.t < ntiles) {
+    cp_async_wait<S - 1>();
+    __syncthreads();                 // this step's slots are filled; every reader of the slots refilled below is done
+    if (ld.t < ntiles) issue(ld, lp, lo);
+    cp_async_commit();
+    ld.next(nrc, ncol, RPP);
+    lp = lp + 1 == RP ? 0 : lp + 1;
+    lo = lo + 1 == RO ? 0 : lo + 1;
+    if (st.c > st.cs) compute(st, sp, so);
+    st.next(nrc, ncol, RPP);
+    sp = sp + 1 == RP ? 0 : sp + 1;
+    so = so + 1 == RO ? 0 : so + 1;
+  }
+  cp_async_wait<0>();
+}
+
+template <typename T, int KT, int MODE> struct StPipe {
+  static constexpr int V16 = 16 / (int)sizeof(T);
+  static constexpr int CPT = KT < V16 ? KT : V16;
+  static constexpr int RPP = NT / (KT / CPT);
+  static constexpr bool NEEDB = (MODE == SP_RESNORM || MODE == SP_RES || MODE == SP_JACOBI || MODE == SP_JACOBI_DOT);
+  static constexpr bool NEEDD = (MODE == SP_JACOBI || MODE == SP_JACOBI_DOT);
+  // panel slot: X (B for SP_RES0) rows, then for SP_RES0 1/diag rows ; own slot: diagonals, B rows, 1/diag
+  static constexpr int PX = st_a16((RPP + 2) * KT * (int)sizeof(T));
+  static constexpr int PANEL = PX + (MODE == SP_RES0 ? st_a16((RPP + 2) * (int)sizeof(T)) : 0);
+  static constexpr int OD = st_a16(9 * RPP * (int)sizeof(T));
+  static constexpr int OB = NEEDB ? st_a16(RPP * KT * (int)sizeof(T)) : 0;
+  static constexpr int OWN = OD + OB + (NEEDD ? st_a16(RPP * (int)sizeof(T)) : 0);
+  using D = StDepth<PANEL, OWN, 3>;
+};
+
+// k_stencil, operands through the shared-memory pipeline.  Three CTAs per SM as k_stencil.
+template <typename T, int KT, int MODE>
+__global__ void __launch_bounds__(NT, 3)
+k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, const SpmmEpi<T> ep) {
+  using SP = StPipe<T, KT, MODE>;
+  constexpr int CPT = SP::CPT, RPP = SP::RPP, S = SP::D::S;
+  constexpr int RP = S + 3;
+  extern __shared__ __align__(128) unsigned char st_sm[];
+  unsigned char* const pring = st_sm;
+  unsigned char* const oring = st_sm + RP * SP::PANEL;
+  const int tid = threadIdx.x;
+  const int cg = tid % (KT / CPT), rl = tid / (KT / CPT), c0 = cg * CPT;
+  const int n = A.n, nr = A.nr;
+  double dot0[CPT], dot1[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) dot0[i] = dot1[i] = 0.0;
+
+  const T* const G = MODE == SP_RES0 ? ep.B : X;     // the gathered panel
+  auto issue = [&](const StStep& s, int lp, int lo) {
+    unsigned char* ps = pring + lp * SP::PANEL;
+    const long long g0 = (long long)s.c * nr + s.r0 - 1;
+    cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), G, g0, n);
+    if (MODE == SP_RES0) cp_rows<T, 1, RPP + 2>(reinterpret_cast<T*>(ps + SP::PX), ep.dinv, g0, n);
+    if (s.c > s.cs) {
+      unsigned char* os = oring + lo * SP::OWN;
+      const long long row0 = (long long)(s.c - 1) * nr + s.r0;
+      cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
+      if (SP::NEEDB) cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), ep.B, row0, n);
+      if (SP::NEEDD) cp_rows<T, 1, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OB), ep.dinv, row0, n);
+    }
+  };
+  auto compute = [&](const StStep& s, int sp, int so) {
+    const int c = s.c - 1, r = s.r0 + rl;
+    const long long row_l = (long long)c * nr + r;
+    if (r >= nr || row_l >= n) return;
+    const int row = (int)row_l;
+    const T* xs[3];
+    const T* ws[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const int k = sp + d + RP - 2;
+      const unsigned char* p = pring + (k >= RP ? k - RP : k) * SP::PANEL;
+      xs[d] = reinterpret_cast<const T*>(p);
+      ws[d] = reinterpret_cast<const T*>(p + SP::PX);
+    }
+    const unsigned char* os = oring + so * SP::OWN;
+    const T* dg = reinterpret_cast<const T*>(os);
+    T acc[CPT], xo[CPT];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) acc[i] = T(0);
+#pragma unroll
+    for (int s9 = 0; s9 < 9; ++s9) {
+      T xv[CPT];
+      ldvec<T, CPT>(xs[s9 / 3] + (rl + s9 % 3) * KT + c0, xv);
+      if (s9 == 4) {
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) xo[i] = xv[i];
+      }
+      const T vs = MODE == SP_RES0 ? dg[s9 * RPP + rl] * (ep.omega * ws[s9 / 3][rl + s9 % 3]) : dg[s9 * RPP + rl];
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) acc[i] += vs * xv[i];
+    }
+    const size_t o = (size_t)row * KT + c0;
+    T out[CPT], bb[CPT];
+    if (SP::NEEDB) ldvec<T, CPT>(reinterpret_cast<const T*>(os + SP::OD) + rl * KT + c0, bb);
+    T dv = T(0);
+    if (SP::NEEDD) dv = ep.omega * reinterpret_cast<const T*>(os + SP::OD + SP::OB)[rl];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) {
+      if (MODE == SP_PLAIN) {
+        out[i] = acc[i];
+      } else if (MODE == SP_CG) {
+        out[i] = acc[i];
+        dot0[i] += (double)acc[i] * (double)xo[i];
+      } else if (MODE == SP_RESNORM) {
+        const T rr = bb[i] - acc[i];
+        out[i] = rr;
+        dot0[i] += (double)rr * (double)rr;
+        dot1[i] += (double)bb[i] * (double)bb[i];
+      } else if (MODE == SP_RES) {
+        out[i] = bb[i] - acc[i];
+      } else if (MODE == SP_RES0) {
+        out[i] = xo[i] - acc[i];
+      } else {
+        const T yn = xo[i] + dv * (bb[i] - acc[i]);
+        out[i] = yn;
+        if (MODE == SP_JACOBI_DOT) dot0[i] += (double)bb[i] * (double)yn;
+      }
+    }
+    stvec<T, CPT>(Y + o, out);
+  };
+  stencil_pipe<S, RPP>(n, nr, issue, compute);
+
+  if (MODE == SP_CG) {
+    CSB_REDUCE_SMEM(1, KT)
+    double v[1][CPT];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) v[0][i] = dot0[i];
+    if (grid_reduce<KT, CPT, 1, false>(v, ep.partials, &ep.ctl->ticket, s_warp, s_tree, s_out)) {
+      if (tid < KT) {
+        const double pap = s_out[tid];
+        ep.ctl->pap[tid] = pap;
+        ep.ctl->alpha[tid] = (ep.ctl->active[tid] && pap > 0.0) ? ep.ctl->rho[tid] / pap : 0.0;
+      }
+    }
+  } else if (MODE == SP_RESNORM) {
+    CSB_REDUCE_SMEM(2, KT)
+    double v[2][CPT];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) { v[0][i] = dot0[i]; v[1][i] = dot1[i]; }
+    if (grid_reduce<KT, CPT, 2, false>(v, ep.partials, &ep.ctl->ticket, s_warp, s_tree, s_out)) {
+      if (tid < KT) {
+        ep.ctl->resid[tid] = s_out[tid];
+        ep.ctl->bnorm[tid] = s_out[KT + tid];
+      }
+    }
+  } else if (MODE == SP_JACOBI_DOT) {
+    CSB_REDUCE_SMEM(1, KT)
+    double v[1][CPT];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) v[0][i] = dot0[i];
+    if (grid_reduce<KT, CPT, 1, false>(v, ep.partials, &ep.ctl->ticket, s_warp, s_tree, s_out))
+      cg_after_precond<KT>(ep.ctl, s_out);
+  }
+}
+
+// k_stencil_cg, operands through the shared-memory pipeline: panel slot p_{it-1} and Z rows, own slot the diagonals
+// and, on odd iterations, the X and Pd (p_{it-2}) rows.  Without the register arrays of the gathers it runs at
+// CGP_MINB CTAs per SM.
+constexpr int CGP_MINB = 3;
+
+template <typename T, int KT, typename TV> struct StPipeCg {
+  static constexpr int V16 = 16 / (int)sizeof(T);
+  static constexpr int CPT = KT < V16 ? KT : V16;
+  static constexpr int RPP = NT / (KT / CPT);
+  static constexpr int PP = st_a16((RPP + 2) * KT * (int)sizeof(T));
+  static constexpr int PANEL = PP + st_a16((RPP + 2) * KT * (int)sizeof(TV));
+  static constexpr int OD = st_a16(9 * RPP * (int)sizeof(T));
+  static constexpr int OX = st_a16(RPP * KT * (int)sizeof(T));
+  static constexpr int OWN = OD + 2 * OX;
+  using D = StDepth<PANEL, OWN, CGP_MINB>;
+};
+
+template <typename T, int KT, typename TV>
+__global__ void __launch_bounds__(NT, CGP_MINB)
+k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __restrict__ X, T* __restrict__ Y,
+                  PanelCtl* ctl, double* partials) {
+  using SP = StPipeCg<T, KT, TV>;
+  constexpr int CPT = SP::CPT, RPP = SP::RPP, S = SP::D::S;
+  constexpr int RP = S + 3;
+  extern __shared__ __align__(128) unsigned char st_sm[];
+  unsigned char* const pring = st_sm;
+  unsigned char* const oring = st_sm + RP * SP::PANEL;
+  const int it = ctl->iter;
+  const T* const Pold = (it & 1) ? Pb0 : Pb1;      // Pold != Pd: nothing writes it here
+  T* const Pd = (it & 1) ? Pb1 : Pb0;
+  const int tid = threadIdx.x;
+  const int cg = tid % (KT / CPT), rl = tid / (KT / CPT), c0 = cg * CPT;
+  const int n = A.n, nr = A.nr;
+  const bool pair = it & 1;
+  T be[CPT], a1[CPT], a2[CPT];                  // beta_it ; alpha_{it-1}, alpha_{it-2}
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) {
+    be[i] = (T)ctl->beta[c0 + i];
+    a1[i] = (T)ctl->alpha_ring[(it + 2) % 3][c0 + i];
+    a2[i] = (T)ctl->alpha_ring[(it + 1) % 3][c0 + i];
+  }
+  double dot0[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) dot0[i] = 0.0;
+
+  auto issue = [&](const StStep& s, int lp, int lo) {
+    unsigned char* ps = pring + lp * SP::PANEL;
+    const long long g0 = (long long)s.c * nr + s.r0 - 1;
+    cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), Pold, g0, n);
+    cp_rows<TV, KT, RPP + 2>(reinterpret_cast<TV*>(ps + SP::PP), Z, g0, n);
+    if (s.c > s.cs) {
+      unsigned char* os = oring + lo * SP::OWN;
+      const long long row0 = (long long)(s.c - 1) * nr + s.r0;
+      cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
+      if (pair) {
+        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), X, row0, n);
+        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OX), Pd, row0, n);
+      }
+    }
+  };
+  auto compute = [&](const StStep& s, int sp, int so) {
+    const int c = s.c - 1, r = s.r0 + rl;
+    const long long row_l = (long long)c * nr + r;
+    if (r >= nr || row_l >= n) return;
+    const int row = (int)row_l;
+    const T* ps[3];
+    const TV* zs[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const int k = sp + d + RP - 2;
+      const unsigned char* p = pring + (k >= RP ? k - RP : k) * SP::PANEL;
+      ps[d] = reinterpret_cast<const T*>(p);
+      zs[d] = reinterpret_cast<const TV*>(p + SP::PP);
+    }
+    const unsigned char* os = oring + so * SP::OWN;
+    const T* dg = reinterpret_cast<const T*>(os);
+    T acc[CPT], po[CPT], pc[CPT];
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) acc[i] = T(0);
+#pragma unroll
+    for (int s9 = 0; s9 < 9; ++s9) {
+      T pv[CPT];
+      TV zv[CPT];
+      ldvec<T, CPT>(ps[s9 / 3] + (rl + s9 % 3) * KT + c0, pv);
+      ldvec<TV, CPT>(zs[s9 / 3] + (rl + s9 % 3) * KT + c0, zv);
+      if (s9 == 4) {
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) po[i] = pv[i];
+      }
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) pv[i] = (T)zv[i] + be[i] * pv[i];
+      if (s9 == 4) {
+#pragma unroll
+        for (int i = 0; i < CPT; ++i) pc[i] = pv[i];
+      }
+      const T vs = dg[s9 * RPP + rl];
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) acc[i] += vs * pv[i];
+    }
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) dot0[i] += (double)acc[i] * (double)pc[i];
+    const size_t o = (size_t)row * KT + c0;
+    stvec<T, CPT>(Y + o, acc);
+    stvec<T, CPT>(Pd + o, pc);
+    if (pair) {
+      T xo[CPT], pd[CPT];
+      ldvec<T, CPT>(reinterpret_cast<const T*>(os + SP::OD) + rl * KT + c0, xo);
+      ldvec<T, CPT>(reinterpret_cast<const T*>(os + SP::OD + SP::OX) + rl * KT + c0, pd);
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) {
+        xo[i] += a2[i] * pd[i];
+        xo[i] += a1[i] * po[i];
+      }
+      stvec<T, CPT>(X + o, xo);
+    }
+  };
+  stencil_pipe<S, RPP>(n, nr, issue, compute);
+
+  CSB_REDUCE_SMEM(1, KT)
+  double v[1][CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) v[0][i] = dot0[i];
+  if (grid_reduce<KT, CPT, 1, false>(v, partials, &ctl->ticket, s_warp, s_tree, s_out)) {
+    if (tid < KT) {
+      const double pap = s_out[tid];
+      const double al = (ctl->active[tid] && pap > 0.0) ? ctl->rho[tid] / pap : 0.0;
+      ctl->pap[tid] = pap;
+      ctl->alpha[tid] = al;
+      ctl->alpha_ring[it % 3][tid] = al;
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------
 // Upward leg of the V-cycle on a stencil-form level, fused:  prolongate + correct + post-smooth
 //     x1 = x0 + P y          (y: the coarser level's correction, P: ~3 entries per row)
 //     z  = x1 + omega D^-1 (b - A x1)        [+ dot(b, z) -> CG beta / stop test on the finest level]

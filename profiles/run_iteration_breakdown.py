@@ -90,12 +90,19 @@ def finest_bytes(levels, prolong_form):
     else:
         halo = (rps + 2) / rps
         prol = n * (halo * (d32 + 4 + 32 + d32) + 9 * 4 + d32)
+    # the stencil kernels under either name: k_stencil[_cg]_pipe (shared-memory pipeline) or the register-gather
+    # form (CS_B200_NO_STENCIL_PIPE)
+    cg_step = n * (9 * 8 + d32 + 3 * d64 + 1.5 * d64)
+    res0 = n * (9 * 4 + d32 + 4 + d32)
     return {
         "k_stencil<double,8,1>": n * (9 * 8 + d64 + d64),               # CG SpMM: diagonals, P, AP
+        "k_stencil_pipe<double,8,1>": n * (9 * 8 + d64 + d64),
         # fused CG step: diagonals, Z32, p_{it-1} in, AP, p_it out; X in/out + p_{it-2} in every other step
-        "k_stencil_cg<double,8,float>": n * (9 * 8 + d32 + 3 * d64 + 1.5 * d64),
+        "k_stencil_cg<double,8,float>": cg_step,
+        "k_stencil_cg_pipe<double,8,float>": cg_step,
         "k_cg_update_r0<double,8,float>": n * (d64 + 8 + 2 * d64 + d32),  # AP, 1/diag, R in/out, R32
-        "k_stencil<float,8,7>": n * (9 * 4 + d32 + 4 + d32),            # residual with implicit x0: diagonals, b, 1/diag, t
+        "k_stencil<float,8,7>": res0,                                   # residual with implicit x0: diagonals, b, 1/diag, t
+        "k_stencil_pipe<float,8,7>": res0,
         "k_spmm_win<float,8,0,*>#1": nnz_r * 6 + n1 * 2 + n * d32 + n1 * d32,
         "k_stencil_prolong_jacobi<float,8,5,*>": prol,
         "k_cg_update_xp2<double,8,float>": n * (d32 + 4 * d64),         # Z32, X in/out, P in/out
@@ -141,6 +148,8 @@ def main():
     # one iteration starts with the fp64 CG SpMM (or the fused CG step); the bench call runs 3 warm-up iterations +
     # reps, plus set-up kernels
     starts = [i for i, e in enumerate(evs) if short(e.name).startswith(("k_stencil<double,8,1>", "k_stencil_cg<double,8,",
+                                                                        "k_stencil_pipe<double,8,1>",
+                                                                        "k_stencil_cg_pipe<double,8,",
                                                                         "k_spmm_win<double,8,1,"))]
     iters = [evs[starts[j]:starts[j + 1]] for j in range(len(starts) - 1)]
     iters = iters[3:] if len(iters) > a.reps else iters             # drop the warm-up iterations
