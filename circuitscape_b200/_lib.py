@@ -62,6 +62,7 @@ _PROTOS = {
     "cs_b200_level_info": (C.c_int, [_H, C.c_int, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64),
                                      C.POINTER(C.c_int64), C.POINTER(C.c_double), C.POINTER(C.c_int)]),
     "cs_b200_level_csr": (C.c_int, [_H, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cs_b200_level_stencil": (C.c_int, [_H, C.c_int, C.POINTER(C.c_int)]),
     "cs_b200_create_from_raster_poly": (C.c_int, [C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                   C.c_int, C.POINTER(Opts), C.POINTER(_H), C.POINTER(C.c_int64),
                                                   C.POINTER(C.c_int64), C.c_void_p]),

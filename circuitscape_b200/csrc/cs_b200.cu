@@ -58,10 +58,12 @@ struct DevCsr {
   int has_dinv = 0;
   int64_t win_blocks = 0;
   int win_nblocks = 0;
-  // stencil (DIA) form (kernels.cuh k_stencil): 9 diagonals, ld apart; null => CSR kernels
+  // stencil (DIA) form (kernels.cuh k_stencil): 9 diagonals, ld apart, or with dia_half the 5 upper ones
+  // (slots 4 ... 8) of a bitwise symmetric operator; null => CSR kernels
   void* dia = nullptr;
   size_t dia_ld = 0;
   int dia_nr = 0;
+  int dia_half = 0;
   // ELL-4 copy of a prolongator with <= 4 entries per row (k_stencil_prolong_jacobi); null otherwise
   int* ell_col = nullptr;
   void* ell_val = nullptr;
@@ -261,6 +263,7 @@ int upload_csr(cs_b200_handle* h, const csb_amg::Csr& m, DevCsr& d, bool windowe
 void free_win(DevCsr& d) {
   cudaFree(d.win_meta); cudaFree(d.blob); cudaFree(d.dia); cudaFree(d.ell_col); cudaFree(d.ell_val);
   d.win_meta = nullptr; d.blob = nullptr; d.dia = nullptr; d.ell_col = nullptr; d.ell_val = nullptr;
+  d.dia_half = 0;
 }
 
 void free_csr(DevCsr& d) {
@@ -515,6 +518,34 @@ int device_windows(cs_b200_handle* h, DevCsr& d, int64_t ncols_pad, const T* d_d
   return CS_B200_OK;
 }
 
+// the stencil kernels stage their operands through the shared-memory pipeline (kernels.cuh k_stencil_pipe,
+// k_stencil_cg_pipe); CS_B200_NO_STENCIL_PIPE keeps the register-gather kernels for A/B runs
+inline bool stencil_pipe() {
+  static const bool off = std::getenv("CS_B200_NO_STENCIL_PIPE") != nullptr;
+  return !off;
+}
+
+// a bitwise symmetric stencil is stored as its 5 upper diagonals (setup_device.hpp halve_dia);
+// CS_B200_FULL_STENCIL keeps all 9 for A/B runs, and so does the register-gather path, which reads 9
+inline bool full_stencil() {
+  static const bool on = std::getenv("CS_B200_FULL_STENCIL") != nullptr;
+  return on || !stencil_pipe();
+}
+
+// the kernels' view of a stencil-form operator
+template <typename T>
+DiaDev<T> dia_view(const DevCsr& m) {
+  return DiaDev<T>{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr, m.dia_half};
+}
+
+// The register-gather kernels (k_stencil, k_stencil_cg) read all 9 slots.  full_stencil() keeps every
+// operator at 9 slots on that path, so a half-form operator reaching them is a broken invariant, and a
+// launch would read past the 5 stored runs: stop instead.
+[[noreturn]] inline void refuse_half(const char* kernel) {
+  std::fprintf(stderr, "cs_b200: %s was handed a half-form (5-slot) stencil; it reads 9 slots\n", kernel);
+  std::abort();
+}
+
 // stencil (DIA) form of a square operator, if its pattern allows it (opts.stencil: 0 auto, 1, -1 never)
 template <typename T>
 int device_stencil(cs_b200_handle* h, DevCsr& d) {
@@ -526,6 +557,10 @@ int device_stencil(cs_b200_handle* h, DevCsr& d) {
   size_t ld = 0;
   int rc = csb_dev::build_dia<T>(h->stream, d.rowptr, d.colidx, (const T*)d.vals, d.nrows, &dia, &nr, &ld, h->err);
   if (rc) return rc_dev(h, rc);
+  if (dia && !full_stencil()) {
+    rc = csb_dev::halve_dia<T>(h->stream, &dia, d.nrows, nr, ld, &d.dia_half, h->err);
+    if (rc) { cudaFree(dia); return rc_dev(h, rc); }
+  }
   d.dia = dia;
   d.dia_nr = nr;
   d.dia_ld = ld;
@@ -819,25 +854,25 @@ CsrDev<T> view(const DevCsr& m) {
   return CsrDev<T>{m.rowptr, m.colidx, (const T*)m.vals, m.bstart, m.nblocks, m.nrows};
 }
 
-// the stencil kernels stage their operands through the shared-memory pipeline (kernels.cuh k_stencil_pipe,
-// k_stencil_cg_pipe); CS_B200_NO_STENCIL_PIPE keeps the register-gather kernels for A/B runs
-inline bool stencil_pipe() {
-  static const bool off = std::getenv("CS_B200_NO_STENCIL_PIPE") != nullptr;
-  return !off;
+template <typename T, int KT, int MODE, bool HALF>
+void launch_stencil_pipe(cs_b200_handle* h, const DiaDev<T>& a, const T* X, T* Y, const SpmmEpi<T>& ep, int sg) {
+  constexpr int SMEM = StPipe<T, KT, MODE, HALF>::D::BYTES;
+  static bool once[64] = {};   // per device: the attribute lives in the device's context
+  bool& set = once[h->device & 63];
+  if (!set) { cudaFuncSetAttribute(k_stencil_pipe<T, KT, MODE, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  k_stencil_pipe<T, KT, MODE, HALF><<<sg, NT, SMEM, h->stream>>>(a, X, Y, ep);
 }
 
 // k_stencil<T, KT, MODE> on grid sg, through the pipeline unless it is switched off
 template <typename T, int KT, int MODE>
 void launch_stencil(cs_b200_handle* h, const DiaDev<T>& a, const T* X, T* Y, const SpmmEpi<T>& ep, int sg) {
   if (!stencil_pipe()) {
+    if (a.half) refuse_half("k_stencil");
     k_stencil<T, KT, MODE><<<sg, NT, 0, h->stream>>>(a, X, Y, ep);
     return;
   }
-  constexpr int SMEM = StPipe<T, KT, MODE>::D::BYTES;
-  static bool once[64] = {};   // per device: the attribute lives in the device's context
-  bool& set = once[h->device & 63];
-  if (!set) { cudaFuncSetAttribute(k_stencil_pipe<T, KT, MODE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
-  k_stencil_pipe<T, KT, MODE><<<sg, NT, SMEM, h->stream>>>(a, X, Y, ep);
+  if (a.half) launch_stencil_pipe<T, KT, MODE, true>(h, a, X, Y, ep, sg);
+  else launch_stencil_pipe<T, KT, MODE, false>(h, a, X, Y, ep, sg);
 }
 
 // Y = op(M X) with the fused epilogue MODE (kernels.cuh).  `timed`: counts as a launch of
@@ -869,7 +904,7 @@ void launch_spmm_on(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const 
   const SpmmEpi<T> ep{B, dinv, (T)omega, h->d_ctl, h->d_partials};
   if (m.dia && MODE != SP_ADD) {
     if constexpr (MODE != SP_ADD) {
-      const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
+      const DiaDev<T> a = dia_view<T>(m);
       constexpr int V16 = 16 / (int)sizeof(T);
       constexpr int CGn = KT / (KT < V16 ? KT : V16);
       const int rpp = NT / CGn;
@@ -958,7 +993,7 @@ inline bool implicit_x0(const DevLevel& L) {
 template <typename T, int KT>
 void launch_stencil_res0(cs_b200_handle* h, DevLevel& L, const T* B, T* Tout, bool timed) {
   const DevCsr& m = L.A;
-  const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
+  const DiaDev<T> a = dia_view<T>(m);
   const SpmmEpi<T> ep{B, (const T*)L.dinv, (T)L.omega, h->d_ctl, h->d_partials};
   constexpr int V16 = 16 / (int)sizeof(T);
   constexpr int CGn = KT / (KT < V16 ? KT : V16);
@@ -991,7 +1026,7 @@ void launch_stencil_res0(cs_b200_handle* h, DevLevel& L, const T* B, T* Tout, bo
 template <typename T, int KT, int MODE>
 void launch_prolong_jacobi(cs_b200_handle* h, DevLevel& L, const T* Yc, const T* X0, T* Yout, const T* B, bool timed) {
   const DevCsr& m = L.A;
-  const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
+  const DiaDev<T> a = dia_view<T>(m);
   const CsrP<T> p{L.P.rowptr, L.P.colidx, (const T*)L.P.vals, L.P.ell_col, (const T*)L.P.ell_val, L.P.ell_ld};
   const SpmmEpi<T> ep{B, (const T*)L.dinv, (T)L.omega, h->d_ctl, h->d_partials};
   using S = PjShape<T, KT>;
@@ -1137,11 +1172,21 @@ inline bool fused_cg(const cs_b200_handle* h) {
   return h->amg && h->A0.dia && h->P2 && !off;
 }
 
+template <typename T, int KT, typename TV, bool HALF>
+void launch_stencil_cg_pipe(cs_b200_handle* h, const DiaDev<T>& a, const TV* Z, int sg) {
+  constexpr int SMEM = StPipeCg<T, KT, TV, HALF>::D::BYTES;
+  static bool once[64] = {};
+  bool& set = once[h->device & 63];
+  if (!set) { cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  k_stencil_cg_pipe<T, KT, TV, HALF><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP,
+                                                                  h->d_ctl, h->d_partials);
+}
+
 // the z panel the CG update reads: the fp32 cycle's output on mixed handles
 template <typename T, int KT, typename TV>
 void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
   const DevCsr& m = h->A0;
-  const DiaDev<T> a{(const T*)m.dia, m.dia_ld, m.nrows, m.dia_nr};
+  const DiaDev<T> a = dia_view<T>(m);
   constexpr int V16 = 16 / (int)sizeof(T);
   constexpr int CGn = KT / (KT < V16 ? KT : V16);
   const int rpp = NT / CGn;
@@ -1163,13 +1208,10 @@ void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
     cudaEventRecord(e0, h->stream);
   }
   if (stencil_pipe()) {
-    constexpr int SMEM = StPipeCg<T, KT, TV>::D::BYTES;
-    static bool once[64] = {};
-    bool& set = once[h->device & 63];
-    if (!set) { cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
-    k_stencil_cg_pipe<T, KT, TV><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP,
-                                                              h->d_ctl, h->d_partials);
+    if (a.half) launch_stencil_cg_pipe<T, KT, TV, true>(h, a, Z, sg);
+    else launch_stencil_cg_pipe<T, KT, TV, false>(h, a, Z, sg);
   } else {
+    if (a.half) refuse_half("k_stencil_cg");
     k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
                                                        h->d_partials);
   }
@@ -1480,7 +1522,7 @@ template <typename T, int KT>
 void launch_currents(cs_b200_handle* h, bool want_curr, int accumulate) {
   const int grid = (int)std::min<int64_t>(h->grid_spmm, (h->n + (NT / KT) - 1) / (NT / KT));
   if (h->A0.dia) {
-    const DiaDev<T> a{(const T*)h->A0.dia, h->A0.dia_ld, (int)h->n, h->A0.dia_nr};
+    const DiaDev<T> a = dia_view<T>(h->A0);
     k_cur_max_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, h->d_ctl, h->d_partials);
     k_cur_acc_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, h->d_ctl, want_curr ? (T*)h->AP : nullptr,
                                                      (T*)h->d_cum, (T*)h->d_max, accumulate, h->opts.log_transform, KT);
@@ -2445,6 +2487,16 @@ int cs_b200_level_info(cs_b200_handle* h, int level, int which, int64_t* nrows, 
   if (nnz) *nnz = m->nnz;
   if (omega) *omega = om;
   if (windowed) *windowed = m->dia ? 2 : (m->win_meta ? 1 : 0);   // 2 = stencil (DIA) form
+  return CS_B200_OK;
+}
+
+int cs_b200_level_stencil(cs_b200_handle* h, int level, int* slots) {
+  bool f32 = false;
+  double om = 0.0;
+  int64_t nc = 0;
+  const DevCsr* m = pick_level(h, level, 0, &f32, &om, &nc);
+  if (!m || !slots) return CS_B200_ERR_ARG;
+  *slots = !m->dia ? 0 : m->dia_half ? 5 : 9;
   return CS_B200_OK;
 }
 

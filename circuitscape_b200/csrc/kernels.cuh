@@ -947,11 +947,24 @@ k_spmm_win(const WinCsr<T> A, const T* __restrict__ X, T* __restrict__ Y, const 
 // the round-robin tile order keeps in flight at the same time (L2).  Same epilogues / same
 // deterministic reductions as k_spmm / k_spmm_win.
 // ---------------------------------------------------------------------------
+// Half form (half = 1): an operator whose lower slot s < 4 of every row i holds, bit for bit, the upper slot
+// 8 - s of row i + off(s), off(s) = (s / 3 - 1) nr + s % 3 - 1 (and +0 where that row lies outside [0, n)), is
+// stored as slots 4 ... 8 only (setup_device.hpp halve_dia): 5 values per row instead of 9.  The kernels take
+// a lower slot from the neighbour row's upper slot, which is the same number in the same slot of the sums.
 template <typename T> struct DiaDev {
-  const T* vals;   // 9 diagonals, ld apart
+  const T* vals;   // 9 diagonals (half: slots 4 ... 8), ld apart
   size_t ld;
   int n;
   int nr;          // stride between raster columns
+  int half;
+  // the stored run of slot s (s >= 4 when half)
+  __device__ __forceinline__ const T* run(int s) const { return vals + (size_t)(half ? s - 4 : s) * ld; }
+  // entry (row, row + off(s)); half: a lower slot from the neighbour row, 0 outside [0, n)
+  __device__ __forceinline__ T at(int s, int row) const {
+    if (!half || s >= 4) return __ldg(run(s) + row);
+    const long long j = (long long)row + (s / 3 - 1) * (long long)nr + (s % 3 - 1);
+    return j >= 0 && j < n ? __ldg(run(8 - s) + j) : T(0);
+  }
 };
 
 constexpr int ST_TC = 16;   // raster columns per tile
@@ -1213,6 +1226,8 @@ k_stencil_cg(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __r
 //   panel ring (S + 3 slots): rows [c nr + r0 - 1, c nr + r0 + RPP] of each gathered panel, one contiguous range:
 //     the +-1 neighbours of a row are rows of the same slot, the +-nr ones the same rows of the slots of c -+ 1
 //   own ring (S + 1 slots): the 9 diagonal runs of the RPP rows of column c and the own-row streams the step reads
+// HALF (a half-form operator): the panel slot also holds the 5 upper-slot runs of its RPP + 2 rows and the own slot no
+// diagonals; a lower slot s is upper slot 8 - s at the panel row the gather of slot s reads (st_half_val).
 // A slot is rewritten three (panel) or one (own) step after its last read, behind the step's barrier.  Rows
 // outside [0, n) are zero-filled by the copy (src-size 0): such a neighbour has a zero diagonal, and 0 x 0 adds
 // nothing to a sum, as 0 x (the clamped row) does in the register kernels.  Every thread takes part in every copy
@@ -1275,8 +1290,23 @@ __device__ __forceinline__ void cp_diag(T* dst, const DiaDev<T>& A, long long ro
     if (NCH % NT == 0 || q < NCH) {
       const long long g = row0 + q % RPP;
       const bool ok = g < A.n;
-      cp_async_zfill<(int)sizeof(T)>(dst + q, A.vals + (size_t)(q / RPP) * A.ld + (ok ? g : 0), ok);
+      cp_async_zfill<(int)sizeof(T)>(dst + q, A.run(q / RPP) + (ok ? g : 0), ok);
     }
+  }
+}
+
+// half form: the upper-slot runs 4 + [u0, u1) of the RPP + 2 rows [g0, g0 + RPP + 2) of a panel slot, slot-major
+// (RPP + 2 apart), zero outside [0, n) -- the +0 that halve_dia demands of a lower slot whose mirror row is missing
+template <typename T, int RPP>
+__device__ __forceinline__ void cp_diag_half(T* dst, const DiaDev<T>& A, long long g0, int u0, int u1) {
+  constexpr int RW = RPP + 2;
+  const int nch = (u1 - u0) * RW;
+#pragma unroll 1
+  for (int q = (int)threadIdx.x; q < nch; q += NT) {
+    const int u = u0 + q / RW, rr = q % RW;
+    const long long g = g0 + rr;
+    const bool ok = g >= 0 && g < A.n;
+    cp_async_zfill<(int)sizeof(T)>(dst + u * RW + rr, A.run(4 + u) + (ok ? g : 0), ok);
   }
 }
 
@@ -1294,7 +1324,21 @@ struct StStep {
   __device__ __forceinline__ void next(int nrc, int ncol, int rpp) {
     if (++c > ce) start(t + gridDim.x, nrc, ncol, rpp);
   }
+  // half form: the upper-slot runs 4 + [u0, u1) this step loads -- all 5 where column c is computed (cs <= c < ce),
+  // 6 ... 8 (the lower slots 0 ... 2 of column c + 1) where it is only the left neighbour of one (c = cs - 1)
+  __device__ __forceinline__ void half_runs(int& u0, int& u1) const {
+    u0 = c >= cs ? 0 : 2;
+    u1 = c < ce ? 5 : 2;
+  }
 };
+
+// half form: slot s9 of the row at panel row rl + 1 of column c, out of the upper-slot runs of the panel slots of
+// columns c - 1, c (ds[0], ds[1]; RPP + 2 apart): a lower slot is upper slot 8 - s9 of the row the panel gather
+// of slot s9 reads, at panel row rl + s9 % 3 of column c + s9 / 3 - 1
+template <typename T, int RPP>
+__device__ __forceinline__ T st_half_val(const T* const (&ds)[3], int s9, int rl) {
+  return s9 < 4 ? ds[s9 / 3][(4 - s9) * (RPP + 2) + rl + s9 % 3] : ds[1][(s9 - 4) * (RPP + 2) + rl + 1];
+}
 
 // issue(step, panel slot, own slot) fills the slots of a load step; compute(step, panel slot, own slot) runs on the
 // step that loaded column step.c, for column step.c - 1, reading panel slots (slot - 2, slot - 1, slot) mod S + 3
@@ -1333,26 +1377,29 @@ __device__ __forceinline__ void stencil_pipe(int n, int nr, Issue&& issue, Compu
   cp_async_wait<0>();
 }
 
-template <typename T, int KT, int MODE> struct StPipe {
+template <typename T, int KT, int MODE, bool HALF> struct StPipe {
   static constexpr int V16 = 16 / (int)sizeof(T);
   static constexpr int CPT = KT < V16 ? KT : V16;
   static constexpr int RPP = NT / (KT / CPT);
   static constexpr bool NEEDB = (MODE == SP_RESNORM || MODE == SP_RES || MODE == SP_JACOBI || MODE == SP_JACOBI_DOT);
   static constexpr bool NEEDD = (MODE == SP_JACOBI || MODE == SP_JACOBI_DOT);
-  // panel slot: X (B for SP_RES0) rows, then for SP_RES0 1/diag rows ; own slot: diagonals, B rows, 1/diag
+  // panel slot: X (B for SP_RES0) rows, then for SP_RES0 1/diag rows, then (HALF) the 5 upper-slot runs of the
+  // same rows ; own slot: (!HALF) the 9 diagonal runs, B rows, 1/diag
   static constexpr int PX = st_a16((RPP + 2) * KT * (int)sizeof(T));
-  static constexpr int PANEL = PX + (MODE == SP_RES0 ? st_a16((RPP + 2) * (int)sizeof(T)) : 0);
-  static constexpr int OD = st_a16(9 * RPP * (int)sizeof(T));
+  static constexpr int PDG = PX + (MODE == SP_RES0 ? st_a16((RPP + 2) * (int)sizeof(T)) : 0);
+  static constexpr int PANEL = PDG + (HALF ? st_a16(5 * (RPP + 2) * (int)sizeof(T)) : 0);
+  static constexpr int OD = HALF ? 0 : st_a16(9 * RPP * (int)sizeof(T));
   static constexpr int OB = NEEDB ? st_a16(RPP * KT * (int)sizeof(T)) : 0;
   static constexpr int OWN = OD + OB + (NEEDD ? st_a16(RPP * (int)sizeof(T)) : 0);
   using D = StDepth<PANEL, OWN, 3>;
 };
 
-// k_stencil, operands through the shared-memory pipeline.  Three CTAs per SM as k_stencil.
-template <typename T, int KT, int MODE>
+// k_stencil, operands through the shared-memory pipeline.  Three CTAs per SM as k_stencil.  HALF: A is in the
+// half form (A.half), its diagonals come with the panel rows.
+template <typename T, int KT, int MODE, bool HALF>
 __global__ void __launch_bounds__(NT, 3)
 k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, const SpmmEpi<T> ep) {
-  using SP = StPipe<T, KT, MODE>;
+  using SP = StPipe<T, KT, MODE, HALF>;
   constexpr int CPT = SP::CPT, RPP = SP::RPP, S = SP::D::S;
   constexpr int RP = S + 3;
   extern __shared__ __align__(128) unsigned char st_sm[];
@@ -1371,10 +1418,15 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
     const long long g0 = (long long)s.c * nr + s.r0 - 1;
     cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), G, g0, n);
     if (MODE == SP_RES0) cp_rows<T, 1, RPP + 2>(reinterpret_cast<T*>(ps + SP::PX), ep.dinv, g0, n);
+    if (HALF) {
+      int u0, u1;
+      s.half_runs(u0, u1);
+      cp_diag_half<T, RPP>(reinterpret_cast<T*>(ps + SP::PDG), A, g0, u0, u1);
+    }
     if (s.c > s.cs) {
       unsigned char* os = oring + lo * SP::OWN;
       const long long row0 = (long long)(s.c - 1) * nr + s.r0;
-      cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
+      if (!HALF) cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
       if (SP::NEEDB) cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), ep.B, row0, n);
       if (SP::NEEDD) cp_rows<T, 1, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OB), ep.dinv, row0, n);
     }
@@ -1386,12 +1438,14 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
     const int row = (int)row_l;
     const T* xs[3];
     const T* ws[3];
+    const T* ds[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       const int k = sp + d + RP - 2;
       const unsigned char* p = pring + (k >= RP ? k - RP : k) * SP::PANEL;
       xs[d] = reinterpret_cast<const T*>(p);
       ws[d] = reinterpret_cast<const T*>(p + SP::PX);
+      ds[d] = reinterpret_cast<const T*>(p + SP::PDG);
     }
     const unsigned char* os = oring + so * SP::OWN;
     const T* dg = reinterpret_cast<const T*>(os);
@@ -1406,7 +1460,8 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
 #pragma unroll
         for (int i = 0; i < CPT; ++i) xo[i] = xv[i];
       }
-      const T vs = MODE == SP_RES0 ? dg[s9 * RPP + rl] * (ep.omega * ws[s9 / 3][rl + s9 % 3]) : dg[s9 * RPP + rl];
+      const T a9 = HALF ? st_half_val<T, RPP>(ds, s9, rl) : dg[s9 * RPP + rl];
+      const T vs = MODE == SP_RES0 ? a9 * (ep.omega * ws[s9 / 3][rl + s9 % 3]) : a9;
 #pragma unroll
       for (int i = 0; i < CPT; ++i) acc[i] += vs * xv[i];
     }
@@ -1479,23 +1534,24 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
 // CGP_MINB CTAs per SM.
 constexpr int CGP_MINB = 3;
 
-template <typename T, int KT, typename TV> struct StPipeCg {
+template <typename T, int KT, typename TV, bool HALF> struct StPipeCg {
   static constexpr int V16 = 16 / (int)sizeof(T);
   static constexpr int CPT = KT < V16 ? KT : V16;
   static constexpr int RPP = NT / (KT / CPT);
   static constexpr int PP = st_a16((RPP + 2) * KT * (int)sizeof(T));
-  static constexpr int PANEL = PP + st_a16((RPP + 2) * KT * (int)sizeof(TV));
-  static constexpr int OD = st_a16(9 * RPP * (int)sizeof(T));
+  static constexpr int PDG = PP + st_a16((RPP + 2) * KT * (int)sizeof(TV));
+  static constexpr int PANEL = PDG + (HALF ? st_a16(5 * (RPP + 2) * (int)sizeof(T)) : 0);
+  static constexpr int OD = HALF ? 0 : st_a16(9 * RPP * (int)sizeof(T));
   static constexpr int OX = st_a16(RPP * KT * (int)sizeof(T));
   static constexpr int OWN = OD + 2 * OX;
   using D = StDepth<PANEL, OWN, CGP_MINB>;
 };
 
-template <typename T, int KT, typename TV>
+template <typename T, int KT, typename TV, bool HALF>
 __global__ void __launch_bounds__(NT, CGP_MINB)
 k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __restrict__ X, T* __restrict__ Y,
                   PanelCtl* ctl, double* partials) {
-  using SP = StPipeCg<T, KT, TV>;
+  using SP = StPipeCg<T, KT, TV, HALF>;
   constexpr int CPT = SP::CPT, RPP = SP::RPP, S = SP::D::S;
   constexpr int RP = S + 3;
   extern __shared__ __align__(128) unsigned char st_sm[];
@@ -1524,10 +1580,15 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
     const long long g0 = (long long)s.c * nr + s.r0 - 1;
     cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), Pold, g0, n);
     cp_rows<TV, KT, RPP + 2>(reinterpret_cast<TV*>(ps + SP::PP), Z, g0, n);
+    if (HALF) {
+      int u0, u1;
+      s.half_runs(u0, u1);
+      cp_diag_half<T, RPP>(reinterpret_cast<T*>(ps + SP::PDG), A, g0, u0, u1);
+    }
     if (s.c > s.cs) {
       unsigned char* os = oring + lo * SP::OWN;
       const long long row0 = (long long)(s.c - 1) * nr + s.r0;
-      cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
+      if (!HALF) cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
       if (pair) {
         cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), X, row0, n);
         cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OX), Pd, row0, n);
@@ -1541,12 +1602,14 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
     const int row = (int)row_l;
     const T* ps[3];
     const TV* zs[3];
+    const T* ds[3];
 #pragma unroll
     for (int d = 0; d < 3; ++d) {
       const int k = sp + d + RP - 2;
       const unsigned char* p = pring + (k >= RP ? k - RP : k) * SP::PANEL;
       ps[d] = reinterpret_cast<const T*>(p);
       zs[d] = reinterpret_cast<const TV*>(p + SP::PP);
+      ds[d] = reinterpret_cast<const T*>(p + SP::PDG);
     }
     const unsigned char* os = oring + so * SP::OWN;
     const T* dg = reinterpret_cast<const T*>(os);
@@ -1569,7 +1632,7 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
 #pragma unroll
         for (int i = 0; i < CPT; ++i) pc[i] = pv[i];
       }
-      const T vs = dg[s9 * RPP + rl];
+      const T vs = HALF ? st_half_val<T, RPP>(ds, s9, rl) : dg[s9 * RPP + rl];
 #pragma unroll
       for (int i = 0; i < CPT; ++i) acc[i] += vs * pv[i];
     }
@@ -1647,7 +1710,9 @@ template <typename T, int KT> struct PjShape {
   // fp32: the 9 diagonal values of a row wait for the Jacobi step in shared memory (fp64: in registers)
   static constexpr bool VSMEM = sizeof(T) == 4;
   // the x1 ring, per thread the b vector and omega / diag of its row, and (VSMEM) per strip row its 9
-  // diagonal values, the last two double-buffered by column parity
+  // diagonal values, the last two double-buffered by column parity.  A half-form operator keeps 5 upper-slot
+  // values per strip row in three buffers by column (rel % 3): the lower slots of column c - 1 are read from
+  // column c - 2's buffer, which the step of column c + 1 must not refill yet; 15 RH <= 18 RH.
   static constexpr int SMEM = (PJ_RING * RH * KT + 2 * NT * CPT + 2 * NT + (VSMEM ? 2 * 9 * RH : 0)) * (int)sizeof(T);
 };
 
@@ -1721,15 +1786,26 @@ k_stencil_prolong_jacobi(const DiaDev<T> A, const CsrP<T> P, const T* __restrict
       T v[9];
       if constexpr (S::VSMEM) {
         // straight to shared memory (cp.async), one copy per row by its column group 0
-        if (zdo && g == 0) {
+        if (A.half) {
+          // the upper-slot runs of column c - 1, every strip row (the halo rows too, for the lower slots of the
+          // rows next to them): all 5 where it is computed (c > cb), 6 ... 8 (the lower slots 0 ... 2 of column c)
+          // where it is only the left neighbour of one (c = cb); zero for rows outside the raster, as halve_dia
+          // demands
+          if (g == 0) {
+            const int u0 = c > cb ? 0 : 2, u1 = c >= cb ? 5 : 2;
+            for (int u = u0; u < u1; ++u)
+              cp_async_zfill<(int)sizeof(T)>(vsm + ((rel % 3) * 5 + u) * RH + rr, A.run(4 + u) + rowp, okp);
+          }
+        } else if (zdo && g == 0) {
 #pragma unroll
           for (int s = 0; s < 9; ++s)
             asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(smem_u32(vsm + ((rel & 1) * 9 + s) * RH + rr)),
-                         "l"(A.vals + (size_t)s * A.ld + rowp), "n"((int)sizeof(T)) : "memory");
+                         "l"(A.run(s) + rowp), "n"((int)sizeof(T)) : "memory");
         }
       } else {
 #pragma unroll
-        for (int s = 0; s < 9; ++s) v[s] = zdo ? __ldcs(A.vals + (size_t)s * A.ld + rowp) : T(0);   // streamed once
+        for (int s = 0; s < 9; ++s)   // streamed once; half: the lower slots straight from the neighbour rows
+          v[s] = zdo ? (A.half && s < 4 ? A.at(s, rowp) : __ldcs(A.run(s) + rowp)) : T(0);
       }
       int rown;
       const bool okn = row_of(c + 1, rown);
@@ -1796,7 +1872,11 @@ k_stencil_prolong_jacobi(const DiaDev<T> A, const CsrP<T> P, const T* __restrict
         for (int i = 0; i < CPT; ++i) acc[i] = T(0);
 #pragma unroll
         for (int s = 0; s < 9; ++s) {
-          const T vs = S::VSMEM ? vsm[((rel & 1) * 9 + s) * RH + rr] : v[s];
+          // half: a lower slot is upper slot 8 - s of row rr + s % 3 - 1 of column c - 1 + s / 3 - 1
+          const T vs = !S::VSMEM ? v[s]
+                       : !A.half ? vsm[((rel & 1) * 9 + s) * RH + rr]
+                       : s >= 4  ? vsm[((rel % 3) * 5 + s - 4) * RH + rr]
+                                 : vsm[(((rel + (s / 3 == 1 ? 0 : 2)) % 3) * 5 + 4 - s) * RH + rr + s % 3 - 1];
           T xv[CPT];
           ldvec<T, CPT>(xs + ((size_t)((rel + s / 3 - 2) % PJ_RING) * RH + (rr + s % 3 - 1)) * KT + c0, xv);
 #pragma unroll
@@ -2367,7 +2447,7 @@ k_cur_max_dia(const DiaDev<T> A, const T* __restrict__ V, PanelCtl* ctl, double*
 #pragma unroll
     for (int q = 0; q < 4; ++q) {                       // the four slots with column > row: +1, nr-1, nr, nr+1
       const int s = 5 + q;
-      a[q] = __ldg(A.vals + (size_t)s * A.ld + row);
+      a[q] = __ldg(A.run(s) + row);
       const int j = min(n - 1, row + (s / 3 - 1) * nr + (s % 3 - 1));
       vj[q] = V[(size_t)j * KT + c];
     }
@@ -2405,7 +2485,7 @@ k_cur_acc_dia(const DiaDev<T> A, const T* __restrict__ V, const PanelCtl* ctl, T
       T a[9], vj[9];
 #pragma unroll
       for (int s = 0; s < 9; ++s) {
-        a[s] = __ldg(A.vals + (size_t)s * A.ld + row);
+        a[s] = A.at(s, row);
         const int j = max(0, min(n - 1, row + (s / 3 - 1) * nr + (s % 3 - 1)));
         vj[s] = V[(size_t)j * KT + c];
       }

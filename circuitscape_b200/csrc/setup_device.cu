@@ -1112,7 +1112,60 @@ __global__ void k_dia_fill(int n, int nr, size_t ld, const int* __restrict__ ptr
   }
 }
 
+template <typename T> struct Bits;
+template <> struct Bits<float> { using U = unsigned int; };
+template <> struct Bits<double> { using U = unsigned long long; };
+
+// bad = 1 unless every lower slot s < 4 of row i has the bit pattern of upper slot 8 - s of row i + off(s),
+// or +0 where that row lies outside [0, n)
+template <typename T>
+__global__ void k_dia_sym_check(int n, int nr, size_t ld, const T* __restrict__ dia, int* __restrict__ bad) {
+  using U = typename Bits<T>::U;
+  const U* d = reinterpret_cast<const U*>(dia);
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    int miss = 0;
+#pragma unroll
+    for (int s = 0; s < 4; ++s) {
+      const long long j = (long long)i + (s / 3 - 1) * (long long)nr + (s % 3 - 1);
+      const U lo = d[(size_t)s * ld + i];
+      miss |= (j >= 0 && j < n) ? lo != d[(size_t)(8 - s) * ld + j] : lo != U(0);
+    }
+    if (miss) atomicOr(bad, 1);
+  }
+}
+
 }  // namespace
+
+template <typename T>
+int halve_dia(cudaStream_t s, T** d_dia, int64_t n, int nr, size_t ld, int* half, std::string& err) {
+  *half = 0;
+  Scratch<int> bad;
+  CKD(bad.alloc(1, s));
+  CKD(cudaMemsetAsync(bad.p, 0, sizeof(int), s));
+  k_dia_sym_check<T><<<grid_for(n), TPB, 0, s>>>((int)n, nr, ld, *d_dia, bad.p);
+  int hb = 1;
+  cudaError_t e = cudaGetLastError();
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&hb, bad.p, sizeof(int), cudaMemcpyDeviceToHost, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) {
+    err = std::string("CUDA error ") + cudaGetErrorString(e) + " checking the stencil's symmetry";
+    return -2;
+  }
+  if (hb) return 0;
+  T* up = nullptr;
+  CKD(cudaMalloc(&up, 5 * ld * sizeof(T)));
+  e = cudaMemcpyAsync(up, *d_dia + 4 * ld, 5 * ld * sizeof(T), cudaMemcpyDeviceToDevice, s);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(s);
+  if (e != cudaSuccess) {
+    cudaFree(up);
+    err = std::string("CUDA error ") + cudaGetErrorString(e) + " compacting the stencil";
+    return -2;
+  }
+  cudaFree(*d_dia);
+  *d_dia = up;
+  *half = 1;
+  return 0;
+}
 
 template <typename T>
 int build_dia(cudaStream_t s, const int* d_rowptr, const int* d_colidx, const T* d_vals, int64_t n, T** d_dia, int* nr,
@@ -1381,6 +1434,8 @@ template int build_ell4<double>(cudaStream_t, const int*, const int*, const doub
 
 template int build_dia<float>(cudaStream_t, const int*, const int*, const float*, int64_t, float**, int*, size_t*, std::string&);
 template int build_dia<double>(cudaStream_t, const int*, const int*, const double*, int64_t, double**, int*, size_t*, std::string&);
+template int halve_dia<float>(cudaStream_t, float**, int64_t, int, size_t, int*, std::string&);
+template int halve_dia<double>(cudaStream_t, double**, int64_t, int, size_t, int*, std::string&);
 
 template int build_windowed<float>(cudaStream_t, const int*, const int*, const float*, int64_t, int64_t, int, const float*,
                                    DWin&, std::string&);

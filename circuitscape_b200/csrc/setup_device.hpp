@@ -112,6 +112,13 @@ template <typename T>
 int build_dia(cudaStream_t stream, const int* d_rowptr, const int* d_colidx, const T* d_vals, int64_t n, T** d_dia,
               int* nr, size_t* ld, std::string& err);
 
+// Half form of a stencil from build_dia: if every lower slot s < 4 of row i holds the bit pattern of the upper
+// slot 8 - s of row i + off(s) (off(s) = (s / 3 - 1) nr + s % 3 - 1), or +0 where that row lies outside [0, n),
+// *d_dia is replaced by a cudaMalloc'ed copy of slots 4 ... 8 (same ld) and *half set to 1; otherwise both
+// are left as they are (*half = 0).  Bit patterns, not values: -0 and NaN do not pass for +0 or each other.
+template <typename T>
+int halve_dia(cudaStream_t stream, T** d_dia, int64_t n, int nr, size_t ld, int* half, std::string& err);
+
 // Raster -> Laplacian WITH short-circuit polygons on the device (src/raster/pairwise.jl:271-367 +
 // src/core.jl:608-624): every cell of a polygon (NODATA cells too) takes the node of the polygon's first
 // valid cell, labels are compacted in order, parallel cell adjacencies of merged nodes add up, adjacencies

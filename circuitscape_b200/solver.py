@@ -191,7 +191,8 @@ class B200Factor:
 
     def levels(self):
         """The multigrid hierarchy as SciPy matrices (downloaded; parity / debugging hook):
-        list of dicts with A, P, R (None on the coarsest level), omega, windowed flags."""
+        list of dicts with A, P, R (None on the coarsest level), omega, windowed flags, and A_stencil_slots:
+        the diagonals the stencil form of A stores (0: none, 9, or 5 for a bitwise symmetric operator)."""
         out = []
         l = 0
         while True:
@@ -215,6 +216,9 @@ class B200Factor:
                 lev[name + "_stencil"] = win.value == 2
             if lev["A"] is None:
                 break
+            slots = C.c_int()
+            _lib.check(self._lib, self._h, self._lib.cs_b200_level_stencil(self._h, l, C.byref(slots)))
+            lev["A_stencil_slots"] = slots.value                # 0, 9, or 5: symmetric, upper diagonals only
             out.append(lev)
             l += 1
         return out

@@ -165,6 +165,9 @@ int cs_b200_level_info(cs_b200_handle* h, int level, int which, int64_t* nrows, 
                        int64_t* nnz, double* omega, int* windowed);
 int cs_b200_level_csr(cs_b200_handle* h, int level, int which, int32_t* rowptr, int32_t* colidx,
                       double* vals);
+/* Diagonals stored for the stencil form of operator A_l: 0 (no stencil form), 9, or 5 when the operator is
+ * bitwise symmetric and kept as its upper diagonals only (CS_B200_FULL_STENCIL in the environment keeps 9). */
+int cs_b200_level_stencil(cs_b200_handle* h, int level, int* slots);
 
 /* n and nnz of the handle's operator. */
 int cs_b200_get_dims(const cs_b200_handle* h, int64_t* n, int64_t* nnz);

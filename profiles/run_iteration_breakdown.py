@@ -53,6 +53,9 @@ def level_dims(f):
             lev[name] = (nr.value, nc.value, nnz.value, win.value) if rc == 0 else None
         if lev["A"] is None:
             break
+        slots = C.c_int()
+        f._lib.cs_b200_level_stencil(f._h, l, C.byref(slots))
+        lev["A_stencil_slots"] = slots.value
         out.append(lev)
     return out
 
@@ -75,7 +78,11 @@ def short(name):
 
 def finest_bytes(levels, prolong_form):
     """Bytes moved per launch by the finest-level kernels of one mixed-cycle iteration, k = 8.
-    Panels: n x 8 of fp64 (64 B per row) or fp32 (32 B per row).  Diagonals: 9 per row (stencil form).
+    Panels: n x 8 of fp64 (64 B per row) or fp32 (32 B per row).  Diagonals: 9 per row (stencil form), or with
+    the half form (level 0 reports 5 slots) 5 per row (3 more for the column left of each tile) plus the 2-row halo
+    of each panel slot (RPP + 2 rows for RPP, RPP = 64 in fp64, 128 in fp32) or prolongation strip.  Level 0 reports the fp32 copy the V-cycle runs on; the
+    fp64 operator of the CG step is the same matrix before rounding, so it takes the form the fp32 copy takes
+    (rounding keeps bit-equal entries bit-equal; the reverse is not guaranteed).
     Restriction records: nnz(R) (4 B value + 2 B local column) + 2 B row offsets per coarse row,
     reading the fp32 residual panel and writing the coarse right-hand side."""
     n = levels[0]["A"][0]
@@ -83,30 +90,40 @@ def finest_bytes(levels, prolong_form):
     nnz_r = levels[0]["R"][2] if levels[0]["R"] else 0
     d64, d32 = 8 * KT, 4 * KT
     rps = 256 // 2 - 2                                   # fp32, k = 8: 128-row strips less the 2 halo rows
+    half = levels[0].get("A_stencil_slots") == 5
+    # diagonals per row streamed by the pipelined kernels; half: 5 runs per computed column and 3 for the column
+    # left of each 16-column tile
+    dg64 = (5 + 3 / 16) * 66 / 64 if half else 9
+    dg32 = (5 + 3 / 16) * 130 / 128 if half else 9
     if prolong_form == "tile":
         halo = (130 * 10) / (128 * 8)                     # phase-1 streams of a 128 x 8 tile with its 1-cell halo
         # phase 1 (halo-inflated): b, 1/diag, ELL-4 (4 x (4 + 4) B), y gathers; phase 2: 9 diagonals, b, 1/diag, z
         prol = n * (halo * (d32 + 4 + 32 + d32) + 9 * 4 + d32 + 4 + d32)
     else:
         halo = (rps + 2) / rps
-        prol = n * (halo * (d32 + 4 + 32 + d32) + 9 * 4 + d32)
+        prol = n * (halo * (d32 + 4 + 32 + d32) + (5 * halo if half else 9) * 4 + d32)
     # the stencil kernels under either name: k_stencil[_cg]_pipe (shared-memory pipeline) or the register-gather
     # form (CS_B200_NO_STENCIL_PIPE)
-    cg_step = n * (9 * 8 + d32 + 3 * d64 + 1.5 * d64)
-    res0 = n * (9 * 4 + d32 + 4 + d32)
+    # (the pipelined ones carry a last template argument: the half form or not)
+    cg_step = n * (dg64 * 8 + d32 + 3 * d64 + 1.5 * d64)
+    res0 = n * (dg32 * 4 + d32 + 4 + d32)
     return {
         "k_stencil<double,8,1>": n * (9 * 8 + d64 + d64),               # CG SpMM: diagonals, P, AP
-        "k_stencil_pipe<double,8,1>": n * (9 * 8 + d64 + d64),
+        "k_stencil_pipe<double,8,1,*>": n * (dg64 * 8 + d64 + d64),
+        # residual gate: diagonals, X, B in, residual out
+        "k_stencil<double,8,2>": n * (9 * 8 + 3 * d64),
+        "k_stencil_pipe<double,8,2,*>": n * (dg64 * 8 + 3 * d64),
         # fused CG step: diagonals, Z32, p_{it-1} in, AP, p_it out; X in/out + p_{it-2} in every other step
         "k_stencil_cg<double,8,float>": cg_step,
-        "k_stencil_cg_pipe<double,8,float>": cg_step,
+        "k_stencil_cg_pipe<double,8,float,*>": cg_step,
         "k_cg_update_r0<double,8,float>": n * (d64 + 8 + 2 * d64 + d32),  # AP, 1/diag, R in/out, R32
-        "k_stencil<float,8,7>": res0,                                   # residual with implicit x0: diagonals, b, 1/diag, t
-        "k_stencil_pipe<float,8,7>": res0,
+        "k_stencil<float,8,7>#1": res0,                                 # residual with implicit x0: diagonals, b, 1/diag, t
+        "k_stencil_pipe<float,8,7,*>#1": res0,
         "k_spmm_win<float,8,0,*>#1": nnz_r * 6 + n1 * 2 + n * d32 + n1 * d32,
         "k_stencil_prolong_jacobi<float,8,5,*>": prol,
         "k_cg_update_xp2<double,8,float>": n * (d32 + 4 * d64),         # Z32, X in/out, P in/out
-    }, {"n": n, "n1": n1, "nnz_R0": nnz_r, "prolong_halo_factor": halo}
+    }, {"n": n, "n1": n1, "nnz_R0": nnz_r, "prolong_halo_factor": halo,
+        "level0_stencil_slots": levels[0].get("A_stencil_slots")}
 
 
 def match_bytes(key, table):
@@ -148,7 +165,7 @@ def main():
     # one iteration starts with the fp64 CG SpMM (or the fused CG step); the bench call runs 3 warm-up iterations +
     # reps, plus set-up kernels
     starts = [i for i, e in enumerate(evs) if short(e.name).startswith(("k_stencil<double,8,1>", "k_stencil_cg<double,8,",
-                                                                        "k_stencil_pipe<double,8,1>",
+                                                                        "k_stencil_pipe<double,8,1,",
                                                                         "k_stencil_cg_pipe<double,8,",
                                                                         "k_spmm_win<double,8,1,"))]
     iters = [evs[starts[j]:starts[j + 1]] for j in range(len(starts) - 1)]
