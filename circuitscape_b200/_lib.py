@@ -88,6 +88,9 @@ _PROTOS = {
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
                                          C.c_void_p]),
+    "cs_b200_solve_advanced": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                         C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "cs_b200_solve_sources": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                         C.c_void_p, C.c_double, C.c_int64, C.c_int64, C.c_void_p,
                                         C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,

@@ -14,6 +14,7 @@ flags ask for) come back.
 """
 from __future__ import annotations
 
+import time
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -448,6 +449,10 @@ class AdvancedOutput:
     curmap: np.ndarray | None = None
     node_currents: np.ndarray | None = None
     branch: tuple | None = None
+    result: np.ndarray | None = None      # raster_advanced: what the reference's raster_advanced returns
+    num_solves: int = 0                   # raster_advanced: components solved
+    iterations: int = 0                   # raster_advanced: PCG iterations over the columns
+    stats: dict = field(default_factory=dict)   # raster_advanced: setup_s / solve_s (host clock), columns
 
 
 def multiple_solver(cfg, solver, a, sources, grounds, finitegrounds, resident=None):
@@ -704,12 +709,14 @@ def sources_and_grounds_from_maps(source_map, ground_map, nodemap, n, policy):
 
 @dataclass
 class RasterData:
-    """The fields of src/io.jl:34-43 the one-to-all driver reads."""
+    """The fields of src/io.jl:34-43 the raster front ends read."""
     cellmap: np.ndarray
     polymap: np.ndarray | None
     points_rc: tuple                 # (rows, cols, ids) 1-based, sorted by id
     strengths: np.ndarray | None = None       # (P, 2) id, strength
     included_pairs: object | None = None      # .mode, .point_ids, .mat
+    source_map: np.ndarray | None = None      # advanced mode: source currents per cell (unit currents applied)
+    ground_map: np.ndarray | None = None      # advanced mode: ground conductances per cell, Inf = direct ground
 
 
 @dataclass
@@ -1447,4 +1454,94 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
         _onetoall_output(plan, device, gmap, o, out, res)
     out.resistances = np.column_stack([uniq, res])
     out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
+    return out
+
+
+# ---------------------------------------------------------------------------
+# raster advanced mode on one whole-raster operator  (src/raster/advanced.jl:17-80, 151-305)
+# ---------------------------------------------------------------------------
+def raster_advanced(data: RasterData, flags: Flags, cfg, solver=None, four_neighbors=False,
+                    avg_res=False) -> AdvancedOutput:
+    """src/raster/advanced.jl raster_advanced / compute_advanced_data / advanced_kernel: every connected
+    component with sum(sources) != 0 and sum(grounds) != 0 is one column of cs_b200_solve_advanced on ONE
+    whole-raster handle, its Inf grounds a Dirichlet set at 0 V, the finite grounds on the operator's
+    diagonal (set_grounds, once).  Each column meets its own stop rule, residual gate and 1e-8 current cut,
+    as the reference's per-component solve does.  `data.source_map` / `data.ground_map` are the maps as
+    io.jl delivers them (ground conductances, Inf for direct grounds, unit currents applied); the policy is
+    cfg's remove_src_or_gnd.  Returns AdvancedOutput: voltmap (the column voltages scattered by the node
+    map), curmap (the node currents summed over the columns, no log transform or nodata), voltages per node,
+    and result: the voltage raster, or the 1 x 1 [-1] when no component was solved (advanced.jl:246-249)."""
+    from scipy.sparse import csgraph
+    from . import graph
+    solver = solver or get_solver(cfg)
+    cellmap, polymap = data.cellmap, data.polymap
+    nodemap = graph.construct_node_map(cellmap, polymap)
+    adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
+    n = adj.shape[0]
+    adj.eliminate_zeros()
+    ncomp, comp_of = csgraph.connected_components(adj, directed=False)
+    s, g, f = sources_and_grounds_from_maps(np.asarray(data.source_map, dtype=np.float64),
+                                            np.asarray(data.ground_map, dtype=np.float64), nodemap, n,
+                                            cfg.get("remove_src_or_gnd", "keepall"))
+    order = np.argsort(comp_of, kind="stable")
+    comps = np.split(order, np.cumsum(np.bincount(comp_of, minlength=ncomp))[:-1]) if n else []
+    # one column per solved component: (its rows, Inf-ground rows, source rows, values, local node map or
+    # None when construct_local_node_map numbers the component like the node map, utils.jl:10-30)
+    columns, solved = [], 0
+    for ci, rows in enumerate(comps):
+        if s[rows].sum() == 0 or g[rows].sum() == 0:                  # advanced.jl:194-196
+            continue
+        solved += 1
+        inf = g[rows] == np.inf
+        src = rows[(s[rows] != 0) & ~inf]                             # sources on Inf grounds are deleted
+        if not len(src):
+            continue                                                  # b = 0: the component stays at 0 V
+        lm = None
+        if polymap is not None and not _local_map_is_global(nodemap, comp_of, ci, polymap):
+            lm = construct_local_node_map(nodemap, rows + 1, polymap)
+        columns.append((rows, rows[inf], src, s[src], lm))
+    out = AdvancedOutput(np.zeros(n), np.zeros(nodemap.shape), np.zeros(nodemap.shape), num_solves=solved)
+    out.stats = dict(setup_s=0.0, solve_s=0.0, columns=len(columns))
+    if columns:
+        t0 = time.perf_counter()
+        factor, dev_nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                                        avg_res=avg_res, log_transform=False)
+        with factor:
+            if not np.array_equal(np.asarray(dev_nodemap), nodemap):
+                raise RuntimeError("device node map differs from the host's")
+            if f[0] != NODATA:
+                factor.set_grounds(finite=f)
+            t1 = time.perf_counter()
+            factor.reset_currents()
+            bs = max(1, int(solver.bs))
+            # columns whose local node map is the node map accumulate on the device; the others bring their
+            # currents back to be scattered by their own map
+            for own_map in (False, True):
+                cols = [c for c in columns if (c[4] is not None) == own_map]
+                for st in range(0, len(cols), bs):
+                    chunk = cols[st:st + bs]
+                    sets, gset = [], []
+                    for c in chunk:                                   # -1: finite grounds only
+                        gset.append(len(sets) if len(c[1]) else -1)
+                        if len(c[1]):
+                            sets.append(c[1])
+                    res = factor.solve_advanced(sets, gset, [(c[2], c[3]) for c in chunk], want_volt=True,
+                                                want_curr=own_map, accumulate=not own_map)
+                    out.iterations += int(res["iters"].sum())
+                    for j, (rows, _, _, _, lm) in enumerate(chunk):
+                        v = np.asarray(res["volt"][rows, j], dtype=np.float64)
+                        out.voltages[rows] = v
+                        if lm is not None:
+                            out.voltmap += _scatter(v, lm)
+                            out.curmap += _scatter(np.asarray(res["curr"][rows, j], dtype=np.float64), lm)
+            cum, _ = factor.read_currents(want_max=False)
+            t2 = time.perf_counter()
+        out.stats.update(setup_s=t1 - t0, solve_s=t2 - t1)
+        glob = np.zeros(n, dtype=bool)
+        for rows, _, _, _, lm in columns:
+            glob[rows] = lm is None
+        vg = np.where(glob, out.voltages, 0.0)
+        out.voltmap += _scatter(vg, nodemap)
+        out.curmap += _scatter(np.where(glob, np.asarray(cum, dtype=np.float64), 0.0), nodemap)
+    out.result = out.voltmap.copy() if solved else np.array([[-1.0]])
     return out

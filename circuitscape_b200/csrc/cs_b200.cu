@@ -88,6 +88,7 @@ struct cs_b200_handle {
   void* d_vals = nullptr;
   bool owns_matrix = true;
   void* d_vals0 = nullptr;           // pristine values while grounds are applied (cs_b200_set_grounds)
+  void* d_fg = nullptr;              // the finite grounds of the last cs_b200_set_grounds, or null
   void* d_dinv = nullptr;
   int* d_bstart = nullptr;
   int nblocks = 0;
@@ -1517,20 +1518,23 @@ struct ColumnDriver {
 };
 
 // node currents of the panel in X (src/out.jl:178-290): branch-current maxima, then max(inflow, outflow)
-// per node with the 1e-8 zeroing, accumulated into the cumulative / max vectors (src/out.jl:100-107)
+// per node with the 1e-8 zeroing, accumulated into the cumulative / max vectors (src/out.jl:100-107).
+// fg: the finite-ground currents of each node join the sums (cs_b200_solve_advanced), or null.
 template <typename T, int KT>
-void launch_currents(cs_b200_handle* h, bool want_curr, int accumulate) {
+void launch_currents(cs_b200_handle* h, bool want_curr, int accumulate, const void* fg = nullptr) {
   const int grid = (int)std::min<int64_t>(h->grid_spmm, (h->n + (NT / KT) - 1) / (NT / KT));
   if (h->A0.dia) {
     const DiaDev<T> a = dia_view<T>(h->A0);
     k_cur_max_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, h->d_ctl, h->d_partials);
-    k_cur_acc_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, h->d_ctl, want_curr ? (T*)h->AP : nullptr,
+    k_cur_acc_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, (const T*)fg, h->d_ctl,
+                                                     want_curr ? (T*)h->AP : nullptr,
                                                      (T*)h->d_cum, (T*)h->d_max, accumulate, h->opts.log_transform, KT);
   } else {
     k_cur_max<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
                                                  (const T*)h->X, h->d_ctl, h->d_partials);
     k_cur_acc<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
-                                                 (const T*)h->X, h->d_ctl, want_curr ? (T*)h->AP : nullptr,
+                                                 (const T*)h->X, (const T*)fg, h->d_ctl,
+                                                 want_curr ? (T*)h->AP : nullptr,
                                                  (T*)h->d_cum, (T*)h->d_max, accumulate, h->opts.log_transform, KT);
   }
   h->stats.kernel_launches += 2;
@@ -1592,7 +1596,7 @@ int upload_sparse_rhs(cs_b200_handle* h, int kt, const int64_t* ptr, const int64
 }
 
 // d_rg_*: the panel's Dirichlet sets as the 2*kt row segments of k_seg_set -- segment 2c the rows of set
-// set_a[c], segment 2c+1 those of set_b[c] (empty without set_b).  Growing the buffers drops the region
+// set_a[c], segment 2c+1 those of set_b[c] (empty without set_b, or where the set index is -1).  Growing the buffers drops the region
 // graphs, which captured their addresses; the capacity is recorded once both buffers are allocated.
 int upload_set_segments(cs_b200_handle* h, int kt, const int64_t* set_ptr, const int64_t* set_rows,
                         const int64_t* set_a, const int64_t* set_b) {
@@ -1601,7 +1605,7 @@ int upload_set_segments(cs_b200_handle* h, int kt, const int64_t* set_ptr, const
   seg[0] = 0;
   for (int s = 0; s < 2 * kt; ++s) {
     const int64_t* sets = (s & 1) ? set_b : set_a;
-    if (sets)
+    if (sets && sets[s / 2] >= 0)
       for (int64_t e = set_ptr[sets[s / 2]]; e < set_ptr[sets[s / 2] + 1]; ++e) rows.push_back((int)set_rows[e]);
     seg[s + 1] = (int)rows.size();
   }
@@ -1663,8 +1667,9 @@ int download_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int volt_s
 
 // the node currents of launch_currents (into AP for curr, into the maps when accumulating), then download_outputs
 template <typename T, int KT>
-int currents_and_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int accumulate, int volt_shift) {
-  if (accumulate || curr) launch_currents<T, KT>(h, curr != nullptr, accumulate);
+int currents_and_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int accumulate, int volt_shift,
+                         const void* fg = nullptr) {
+  if (accumulate || curr) launch_currents<T, KT>(h, curr != nullptr, accumulate, fg);
   return download_outputs<T, KT>(h, c0, curr, volt, volt_shift);
 }
 
@@ -1885,15 +1890,16 @@ int region_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const in
   return CS_B200_OK;
 }
 
-// ---- direct-ground columns (cs_b200_solve_grounded) -----------------------------------------
-// Column c: the rows of its ground set are Dirichlet rows at 0 V (segment 2c of the region-panel table;
-// segment 2c+1, the region panels' set_b, is empty), b = its sparse sources, masked; A_c v = b.  No flux
-// or scaling step, and no set fix-up of the currents: every ground row is a node of its own.
+// ---- direct-ground columns (cs_b200_solve_grounded, cs_b200_solve_advanced) -------------------
+// Column c: the rows of its ground set are Dirichlet rows at 0 V (segment 2c of the region-panel table,
+// empty for gset[c] = -1; segment 2c+1, the region panels' set_b, is empty), b = its sparse sources,
+// masked; A_c v = b.  No flux or scaling step, and no set fix-up of the currents: every ground row is a
+// node of its own.  fg: the handle's finite grounds when their currents join the node currents, or null.
 template <typename T, int KT>
 int grounded_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const int64_t* set_rows,
                    const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
                    const double* weight, double rtol, int64_t itmax, T* src_volt, T* volt, T* curr,
-                   int accumulate, int64_t* iters, double* relres, ColumnDriver& cols) {
+                   int accumulate, int64_t* iters, double* relres, ColumnDriver& cols, const void* fg) {
   // k_pair_extract probes the first source row
   if (int rc = upload_ctl(h, KT, [&](int c) {
         return ColCtl{-1, src_rows[src_ptr[c0 + c]], col_weight(weight, c0 + c)};
@@ -1909,7 +1915,7 @@ int grounded_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const 
   if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres, true)) return rc;
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
   h->stats.kernel_launches++;
-  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 0)) return rc;
+  if (int rc = currents_and_outputs<T, KT>(h, c0, curr, volt, accumulate, 0, fg)) return rc;
   if (int rc = read_ctl(h)) return rc;
   if (src_volt)
     for (int c = 0; c < KT; ++c) src_volt[c0 + c] = (T)h->h_ctl->xdst[c];
@@ -2159,7 +2165,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1006; }
+int cs_b200_version(void) { return 1007; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2534,6 +2540,8 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   const size_t es = h->esize();
   const size_t vb = std::max<size_t>(1, (size_t)h->nnz) * es;
   cudaEventRecord(h->ev0, h->stream);
+  cudaFree(h->d_fg);                 // the previous call's finite grounds; this call's replace them
+  h->d_fg = nullptr;
   if (!h->d_vals0) {
     CK(h, cudaMalloc(&h->d_vals0, vb));
     CK(h, cudaMemcpyAsync(h->d_vals0, h->d_vals, vb, cudaMemcpyDeviceToDevice, h->stream));
@@ -2564,6 +2572,10 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   }
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e == cudaSuccess) {            // kept for the ground currents of cs_b200_solve_advanced
+    h->d_fg = d_g;
+    d_g = nullptr;
+  }
   cleanup();
   if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s applying the grounds", cudaGetErrorString(e));
   teardown_operators(h);
@@ -2592,6 +2604,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   teardown_operators(h);
   if (h->owns_matrix) { cudaFree(h->d_rowptr); cudaFree(h->d_colidx); cudaFree(h->d_vals); }
   cudaFree(h->d_vals0);
+  cudaFree(h->d_fg);
   void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->P, h->P2, h->AP, h->B, h->stage,
                   h->d_cum, h->d_max, h->d_ctl, h->d_partials, h->d_flush};
   for (void* b : bufs) if (b) cudaFree(b);
@@ -2961,20 +2974,21 @@ int cs_b200_solve_region_pairs(cs_b200_handle* h, int64_t nsets, const int64_t* 
   });
 }
 
-int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
-                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
-                           const double* src_vals, const double* weight, double rtol, int64_t itmax,
-                           void* src_volt, void* volt, void* curr, int accumulate, int64_t* iters,
-                           double* relres) {
-  // everything is checked before the handle, as in cs_b200_solve_region_pairs; row ranges need its n
-  if (k < 1 || nsets < 1 || !set_ptr || !set_rows || !gset || !src_ptr || !src_rows || !src_vals ||
-      !(rtol >= 0) || itmax < 0)
-    return set_err(h, CS_B200_ERR_ARG, "bad solve_grounded arguments");
+// the columns of cs_b200_solve_grounded / cs_b200_solve_advanced (`who`): everything is checked before
+// the handle, as in cs_b200_solve_region_pairs; row ranges need its n.  gset[c] = -1 (no direct grounds)
+// is accepted only when `floating_ok`.
+static int check_grounded_columns(cs_b200_handle* h, const char* who, int64_t nsets, const int64_t* set_ptr,
+                                  const int64_t* set_rows, int64_t k, const int64_t* gset, const int64_t* src_ptr,
+                                  const int64_t* src_rows, const double* src_vals, double rtol, int64_t itmax,
+                                  bool floating_ok) {
+  if (k < 1 || nsets < (floating_ok ? 0 : 1) || !set_ptr || (nsets > 0 && !set_rows) || !gset || !src_ptr ||
+      !src_rows || !src_vals || !(rtol >= 0) || itmax < 0)
+    return set_err(h, CS_B200_ERR_ARG, "bad %s arguments", who);
   if (int rc = check_sets(h, nsets, set_ptr, set_rows)) return rc;
   if (src_ptr[0] != 0) return set_err(h, CS_B200_ERR_ARG, "src_ptr[0] must be 0");
   for (int64_t c = 0; c < k; ++c) {
     const int64_t s = gset[c];
-    if (s < 0 || s >= nsets)
+    if (s < (floating_ok ? -1 : 0) || s >= nsets)
       return set_err(h, CS_B200_ERR_ARG, "column %lld: set index %lld out of range", (long long)c, (long long)s);
     if (src_ptr[c + 1] <= src_ptr[c])
       return set_err(h, CS_B200_ERR_ARG, "column %lld has no sources", (long long)c);
@@ -2984,16 +2998,49 @@ int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_
       const int64_t r = src_rows[e];
       if (r < 0 || (h && r >= h->n) || r > INT32_MAX)
         return set_err(h, CS_B200_ERR_ARG, "column %lld: source row %lld out of range", (long long)c, (long long)r);
-      if (std::binary_search(set_rows + set_ptr[s], set_rows + set_ptr[s + 1], r))
+      if (s >= 0 && std::binary_search(set_rows + set_ptr[s], set_rows + set_ptr[s + 1], r))
         return set_err(h, CS_B200_ERR_ARG, "column %lld: source row %lld is on its ground set %lld", (long long)c,
                        (long long)r, (long long)s);
     }
   }
+  return CS_B200_OK;
+}
+
+int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
+                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
+                           const double* src_vals, const double* weight, double rtol, int64_t itmax,
+                           void* src_volt, void* volt, void* curr, int accumulate, int64_t* iters,
+                           double* relres) {
+  if (int rc = check_grounded_columns(h, "solve_grounded", nsets, set_ptr, set_rows, k, gset, src_ptr, src_rows,
+                                      src_vals, rtol, itmax, false))
+    return rc;
   return solve_call(h, [&](auto t, ColumnDriver& cols) {
     using T = decltype(t);
     return cols.run(0, k, [&](auto kt, int64_t c0) {
       return grounded_panel<T, kt>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals, weight, rtol,
-                                   itmax, (T*)src_volt, (T*)volt, (T*)curr, accumulate, iters, relres, cols);
+                                   itmax, (T*)src_volt, (T*)volt, (T*)curr, accumulate, iters, relres, cols,
+                                   nullptr);
+    });
+  });
+}
+
+int cs_b200_solve_advanced(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
+                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
+                           const double* src_vals, const double* weight, double rtol, int64_t itmax, void* volt,
+                           void* curr, int accumulate, int64_t* iters, double* relres) {
+  if (int rc = check_grounded_columns(h, "solve_advanced", nsets, set_ptr, set_rows, k, gset, src_ptr, src_rows,
+                                      src_vals, rtol, itmax, true))
+    return rc;
+  for (int64_t c = 0; c < k; ++c)
+    if (gset[c] < 0 && !(h && h->d_fg))
+      return set_err(h, CS_B200_ERR_ARG, "column %lld has no direct grounds and the handle no finite grounds "
+                     "(cs_b200_set_grounds)", (long long)c);
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      return grounded_panel<T, kt>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals, weight, rtol,
+                                   itmax, (T*)nullptr, (T*)volt, (T*)curr, accumulate, iters, relres, cols,
+                                   h->d_fg);
     });
   });
 }

@@ -2348,7 +2348,16 @@ __global__ void k_panel_to_cm(int n, size_t ld, const T* __restrict__ panel, T* 
 //   node current = inflow > outflow ? inflow : outflow
 // which is the row-wise restatement of  B = triu branch currents; B - B'; drop
 // negatives; column sums  done once with the `pos` and once with the `neg` signs.
+// With finite grounds fg (k_cur_acc[_dia], non-null only for cs_b200_solve_advanced), x_i = fg_i v_i
+// adds its ground current to one side before the max (out.jl:193-202): -x_i to inflow when x_i < 0,
+// x_i to outflow when x_i > 0.  The 1e-8 cut does not apply to it.
 // ---------------------------------------------------------------------------
+template <typename T>
+__device__ __forceinline__ void ground_current(T x, T& inflow, T& outflow) {
+  if (x < T(0)) inflow -= x;
+  if (x > T(0)) outflow += x;
+}
+
 template <typename T, int KT>
 __global__ void __launch_bounds__(NT)
 k_cur_max(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
@@ -2380,7 +2389,7 @@ k_cur_max(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
 template <typename T, int KT>
 __global__ void __launch_bounds__(NT)
 k_cur_acc(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
-          const T* __restrict__ vals, const T* __restrict__ V, const PanelCtl* ctl,
+          const T* __restrict__ vals, const T* __restrict__ V, const T* __restrict__ fg, const PanelCtl* ctl,
           T* __restrict__ cur_out /*panel or null*/, T* __restrict__ cum, T* __restrict__ mx,
           int accumulate, int log_transform, int ncols) {
   const int c = threadIdx.x % KT;
@@ -2401,6 +2410,7 @@ k_cur_acc(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
         if (!(fabs(d / maxneg) < T(1e-8)) && d > T(0)) outflow += d;
         if (!(fabs(d / maxpos) < T(1e-8)) && d < T(0)) inflow -= d;
       }
+      if (fg) ground_current(fg[row] * vi, inflow, outflow);
       cur = inflow > outflow ? inflow : outflow;
       if (cur_out) cur_out[(size_t)row * KT + c] = cur;
     }
@@ -2470,7 +2480,8 @@ k_cur_max_dia(const DiaDev<T> A, const T* __restrict__ V, PanelCtl* ctl, double*
 
 template <typename T, int KT>
 __global__ void __launch_bounds__(NT)
-k_cur_acc_dia(const DiaDev<T> A, const T* __restrict__ V, const PanelCtl* ctl, T* __restrict__ cur_out,
+k_cur_acc_dia(const DiaDev<T> A, const T* __restrict__ V, const T* __restrict__ fg, const PanelCtl* ctl,
+              T* __restrict__ cur_out,
               T* __restrict__ cum, T* __restrict__ mx, int accumulate, int log_transform, int ncols) {
   const int c = threadIdx.x % KT;
   constexpr int RPP = NT / KT;
@@ -2498,6 +2509,7 @@ k_cur_acc_dia(const DiaDev<T> A, const T* __restrict__ V, const PanelCtl* ctl, T
         if (!(fabs(d / maxneg) < T(1e-8)) && d > T(0)) outflow += d;
         if (!(fabs(d / maxpos) < T(1e-8)) && d < T(0)) inflow -= d;
       }
+      if (fg) ground_current(fg[row] * vi, inflow, outflow);
       cur = inflow > outflow ? inflow : outflow;
       if (cur_out) cur_out[(size_t)row * KT + c] = cur;
     }

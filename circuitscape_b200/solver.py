@@ -443,6 +443,28 @@ class B200Factor:
         self._raise(rc, raise_on_residual)
         return dict(src_volt=self._io(sv), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
 
+    def solve_advanced(self, sets, gset, sources, weight=None, want_volt=False, want_curr=False,
+                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
+        """Raster advanced-mode columns on this operator and the finite grounds of the last set_grounds
+        (cs_b200_solve_advanced): column c holds the rows of sets[gset[c]] at 0 V (gset[c] = -1: no direct
+        grounds, which needs finite grounds on the handle) and injects sources[c] = (rows, values) (0-based
+        rows, none on the column's ground set).  The node currents include the finite-ground currents.
+        Returns dict with volt, curr, iters, relres."""
+        ptr, rows = _csr(sets, np.int64)
+        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        k = len(gset)
+        assert len(sources) == k
+        sptr, srows = _csr([r for r, _ in sources], np.int64)
+        _, svals = _csr([v for _, v in sources], np.float64)
+        assert len(srows) == len(svals) == sptr[-1]
+        volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
+        rc = self._lib.cs_b200_solve_advanced(
+            self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(gset), _lib._ptr(sptr),
+            _lib._ptr(srows), _lib._ptr(svals), _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax),
+            _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
+        self._raise(rc, raise_on_residual)
+        return dict(volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
+
     def solve_sources(self, columns, ref, probe=None, weight=None, want_volt=False, want_curr=False,
                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
         """Batched solve with sparse right-hand sides, device-resident
@@ -538,9 +560,10 @@ def construct_cholesky_factor(matrix, solver: CUDASolver, **kw) -> B200Factor:
 
 def construct_raster_factor(cellmap, polymap, solver: CUDASolver, four_neighbors=False, avg_res=False,
                             log_transform=False):
-    """The whole-raster operator of a focal-region job and its node map (1-based, 0 = none):
-    B200Factor.from_raster_polygons.  Not one of the three hooks: the region-pair driver needs the
-    handle's cs_b200_solve_region_pairs, which the Solver interface has no method for."""
+    """The whole-raster operator of a focal-region, one-to-all or advanced-mode job and its node map
+    (1-based, 0 = none): B200Factor.from_raster_polygons.  Not one of the three hooks: those drivers need
+    the handle's column entries (cs_b200_solve_region_pairs / _grounded / _advanced), which the Solver
+    interface has no method for."""
     return B200Factor.from_raster_polygons(cellmap, polymap, solver, four_neighbors=four_neighbors,
                                            avg_res=avg_res, log_transform=log_transform)
 

@@ -153,7 +153,8 @@ int cs_b200_get_csr(cs_b200_handle* h, int32_t* rowptr, int32_t* colidx, void* v
  * resident CSR (no matrix crosses PCIe; ~0.1 s at 10^6 nodes).  Right-hand sides passed afterwards must
  * be zero at the Dirichlet rows (the reference drops those sources).  Calling it again starts from the
  * pristine values; NULL, NULL restores the original operator.  Needs the device-side setup and a
- * handle that owns its matrix.                                                                    */
+ * handle that owns its matrix.  The handle keeps finite_g until the next call or cs_b200_destroy: the
+ * node currents of cs_b200_solve_advanced add the finite-ground currents from it.                  */
 int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* dirichlet);
 
 /* Multigrid hierarchy inspection (parity / debugging hooks; levels exist only with the AMG
@@ -263,6 +264,20 @@ int cs_b200_solve_grounded(cs_b200_handle* h, int64_t nsets, const int64_t* set_
                            const double* src_vals, const double* weight, double rtol, int64_t itmax,
                            void* src_volt, void* volt, void* curr, int accumulate, int64_t* iters,
                            double* relres);
+
+/* Raster advanced mode on ONE resident operator (src/raster/advanced.jl:151-305): column c is one connected
+ * component's solve on the handle's current operator L0 + diag(finite grounds of cs_b200_set_grounds).  The
+ * rows of set gset[c] (the component's Inf grounds) are held at 0 V; gset[c] = -1 means the column has no
+ * direct grounds, which needs a handle that carries finite grounds.  Sources, sets, weight / volt / curr /
+ * accumulate / iters / relres and the argument checks as cs_b200_solve_grounded (nsets may be 0 when every
+ * gset[c] is -1); gset[c] = -1 without finite grounds on the handle is CS_B200_ERR_ARG before any device
+ * work.  The node currents add each node's finite-ground current x = fg_i v_i to the inflow (x < 0, as -x)
+ * or the outflow (x > 0) before max(inflow, outflow) (src/out.jl:186-207); the 1e-8 cut of the branch
+ * currents stays per column and does not apply to it.  The other entry points never add that term.        */
+int cs_b200_solve_advanced(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr, const int64_t* set_rows,
+                           int64_t k, const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows,
+                           const double* src_vals, const double* weight, double rtol, int64_t itmax, void* volt,
+                           void* curr, int accumulate, int64_t* iters, double* relres);
 
 /* Batched solve with SPARSE right-hand sides, device-resident -- the advanced-mode kernel
  * (src/raster/advanced.jl:274-305) for source/ground sets without finite grounds, and
