@@ -99,6 +99,15 @@ _PROTOS = {
                                                C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int64,
                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.POINTER(C.c_int64)]),
+    "cs_b200_solve_advanced_network": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                                 C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_void_p]),
+    "cs_b200_solve_pairs_branch": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
+                                             C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
+    "cs_b200_branch_index": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
+    "cs_b200_read_branch_currents": (C.c_int, [_H, C.c_void_p]),
     "cs_b200_read_currents": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "cs_b200_reset_currents": (C.c_int, [_H]),
     "cs_b200_currents_device_ptrs": (C.c_int, [_H, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),

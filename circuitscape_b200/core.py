@@ -205,6 +205,9 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
     G = sp.csr_matrix(prob.G)
     points = np.asarray(prob.points)
     ids = np.asarray(prob.user_points)
+    # network branch currents from the device (cs_b200_solve_pairs_branch); the superposed driver keeps the
+    # host path
+    device_branch = not raster and getattr(solver, "branch_on_device", False) and not getattr(solver, "superpose", False)
 
     for comp in prob.cc:
         comp = np.asarray(comp)
@@ -226,13 +229,17 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
         dst = np.array([local_of[d] for _, d, _ in solves])
         weight = np.array([len(f) for _, _, f in solves], dtype=np.float64)
         need_curr = not shortcut                       # postprocess always builds the current map
-        per_pair_volt = o.write_volt_maps or (not raster and not shortcut)   # network branch currents need v
+        # host network branch currents need v
+        per_pair_volt = o.write_volt_maps or (not raster and not shortcut and not device_branch)
         per_pair_curr = need_curr and ((o.write_cur_maps and not o.write_cum_cur_map_only) or not raster)
         local_nodemap = construct_local_node_map(prob.nodemap, comp, prob.polymap) if raster and not shortcut else None
         # only raster maps are log-transformed (src/out.jl:96 process_grid!); the network branch of
         # write_cur_maps accumulates raw node currents (src/out.jl:48-88)
         with S.construct_cholesky_factor(matrix, solver, log_transform=bool(o.log_transform_maps and raster)) as factor:
             bs = max(1, int(solver.bs))
+            if device_branch:
+                lo, hi = _branch_index(factor, matrix)
+                bpos = branch_pos.positions(comp[lo], comp[hi])
             if shortcut:
                 inside = np.nonzero(np.isin(points, comp) & (points != 0))[0]
                 focal_rows = np.unique(local_of[points[inside]])
@@ -258,7 +265,8 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                         yield sl, res
                         continue
                     yield sl, factor.solve_pairs(src[sl], dst[sl], weight[sl], want_volt=per_pair_volt,
-                                                 want_curr=per_pair_curr, accumulate=need_curr)
+                                                 want_curr=per_pair_curr, accumulate=need_curr,
+                                                 want_branch=device_branch)
 
             for sl, res in batches():
                 out.stats.append(factor.stats())
@@ -268,7 +276,10 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                     r = float(res["R"][col])
                     v = res["volt"][:, col].astype(np.float64) if res.get("volt") is not None else None
                     cur = res["curr"][:, col].astype(np.float64) if res.get("curr") is not None else None
-                    br = _branch_currents(matrix, v, comp) if not raster and not shortcut else None
+                    if device_branch:
+                        br = (comp[lo], comp[hi], np.asarray(res["branch"][:, col], dtype=np.float64))
+                    else:
+                        br = _branch_currents(matrix, v, comp) if not raster and not shortcut else None
                     for ci, cj in fan:
                         R[ci, cj] = R[cj, ci] = r
                         key = (int(ids[ci]), int(ids[cj]))
@@ -294,8 +305,10 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                                     out.curmaps[key] = cm
                         else:
                             # every id combination is post-processed on its own (src/core.jl:235-249):
-                            # its branch currents go into the cumulative vector once each
-                            branch_pos.add(out.cum_branch, br)
+                            # its branch currents go into the cumulative vector once each (on the device:
+                            # weight[col] = len(fan) times)
+                            if not device_branch:
+                                branch_pos.add(out.cum_branch, br)
                             if sink is not None:
                                 sink.network(key, comp, v if o.write_volt_maps else None, cur, br)
                             else:
@@ -323,6 +336,8 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                         out.max_curmap = np.maximum(out.max_curmap, mmap)
                 else:
                     out.cum_node[rows] += cum
+                    if device_branch:
+                        np.add.at(out.cum_branch, bpos, np.asarray(factor.read_branch_currents(), dtype=np.float64))
         if shortcut:
             anchor = int(np.nonzero(points == csub[0])[0][0])
             _update_shortcut_resistances(anchor, voltmatrix, shortcut_res, R, points, comp)
@@ -379,8 +394,8 @@ class _BranchIndex:
         ok[ok] = self.keys[pos[ok]] == key[ok]
         return np.where(ok, self.order[np.minimum(pos, len(self.keys) - 1)], -1)
 
-    def add(self, cum, branch):
-        gr, gc, val = branch
+    def positions(self, gr, gc):
+        """Position in `coords` of every branch (gr, gc), or of (gc, gr) when only the reversed edge is there."""
         gr = np.asarray(gr, dtype=np.int64)
         gc = np.asarray(gc, dtype=np.int64)
         k = self._find(gr, gc)
@@ -390,7 +405,22 @@ class _BranchIndex:
         if (k < 0).any():
             i = int(np.nonzero(k < 0)[0][0])
             raise KeyError(f"branch ({int(gr[i])}, {int(gc[i])}) is not an edge of the graph")
-        np.add.at(cum, k, val)
+        return k
+
+    def add(self, cum, branch):
+        gr, gc, val = branch
+        np.add.at(cum, self.positions(gr, gc), val)
+
+
+def _branch_index(factor, matrix):
+    """The handle's branches (0-based lo, hi), checked against the order _branch_currents writes them in:
+    sp.triu(matrix, 1) sorted by column, then row."""
+    lo, hi = factor.branch_index()
+    coo = sp.triu(sp.csr_matrix(matrix), k=1).tocoo()
+    order = np.lexsort((coo.row, coo.col))
+    if not (np.array_equal(lo, coo.row[order]) and np.array_equal(hi, coo.col[order])):
+        raise RuntimeError("the device's branch order differs from the upper triangle's column-major order")
+    return lo, hi
 
 
 def _update_shortcut_resistances(anchor, voltmatrix, shortcut, resistances, points, comp):
@@ -536,6 +566,64 @@ def advanced_kernel(prob: AdvancedProblem, flags: Flags, cfg=None) -> AdvancedOu
         res.node_currents = node_currents_host(G, voltages, prob.finitegrounds)
         res.branch = _branch_currents(G, voltages, np.arange(1, n + 1))
     return res
+
+
+def network_advanced(prob: AdvancedProblem, flags: Flags, cfg=None) -> AdvancedOutput:
+    """advanced_kernel for networks (src/raster/advanced.jl:184-242) on ONE whole-graph handle: every connected
+    component with sum(sources) != 0, sum(grounds) != 0 and a source off its Inf grounds is one column of
+    cs_b200_solve_advanced_network, its Inf grounds a Dirichlet set at 0 V, the finite grounds on the
+    operator's diagonal (set_grounds, once).  The node and branch currents are taken of the summed voltages
+    under one 1e-8 cut over the whole graph, as the reference takes them, so every column goes into one
+    call (the device walks them in panels).  Returns AdvancedOutput with voltages, node_currents and branch
+    ((lo, hi) 1-based, values) as advanced_kernel's network output, num_solves, iterations and stats."""
+    G = sp.csr_matrix(prob.G)
+    n = G.shape[0]
+    s, g = np.asarray(prob.sources, dtype=np.float64), np.asarray(prob.grounds, dtype=np.float64)
+    f = np.asarray(prob.finitegrounds, dtype=np.float64)
+    columns, solved = [], 0
+    for c in prob.cc:
+        rows = np.asarray(c, dtype=np.int64) - 1
+        if s[rows].sum() == 0 or g[rows].sum() == 0:                      # advanced.jl:194-196
+            continue
+        solved += 1
+        inf = g[rows] == np.inf
+        src = rows[(s[rows] != 0) & ~inf]                                 # sources on Inf grounds are deleted
+        if len(src):                                                      # else b = 0: the component stays at 0 V
+            columns.append((rows, rows[inf], src, s[src]))
+    out = AdvancedOutput(np.zeros(n), num_solves=solved)
+    out.stats = dict(setup_s=0.0, solve_s=0.0, columns=len(columns))
+    if not columns:
+        out.node_currents = np.zeros(n)
+        out.branch = _branch_currents(G, out.voltages, np.arange(1, n + 1))
+        return out
+    # every diagonal entry stored, so that set_grounds can put a finite ground on a node without edges
+    coo = G.tocoo()
+    off = coo.row != coo.col
+    diag = np.arange(n)
+    A = sp.csr_matrix((np.r_[coo.data[off], G.diagonal()], (np.r_[coo.row[off], diag], np.r_[coo.col[off], diag])),
+                      shape=(n, n))
+    owner = np.full(n, -1, dtype=np.int64)
+    sets, gset = [], []
+    for j, (rows, gnd, _, _) in enumerate(columns):
+        owner[rows] = j
+        gset.append(len(sets) if len(gnd) else -1)                       # -1: finite grounds only
+        if len(gnd):
+            sets.append(gnd)
+    t0 = time.perf_counter()
+    with S.construct_cholesky_factor(A, prob.solver) as factor:
+        if f[0] != NODATA:
+            factor.set_grounds(finite=f)
+        lo, hi = _branch_index(factor, G)
+        t1 = time.perf_counter()
+        res = factor.solve_advanced_network(sets, gset, [(c[2], c[3]) for c in columns], owner, want_volt=True,
+                                            want_curr=True, want_branch=True)
+        t2 = time.perf_counter()
+    out.voltages = np.asarray(res["volt"], dtype=np.float64)
+    out.node_currents = np.asarray(res["curr"], dtype=np.float64)
+    out.branch = (lo + 1, hi + 1, np.asarray(res["branch"], dtype=np.float64))
+    out.iterations = int(res["iters"].sum())
+    out.stats.update(setup_s=t1 - t0, solve_s=t2 - t1)
+    return out
 
 
 def all_to_one_batched(factor, focal, rtol=None, shard=None, device_resident=False, accumulate=False):

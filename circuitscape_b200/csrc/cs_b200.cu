@@ -4,6 +4,7 @@
 #include "../../include/cs_b200.h"
 
 #include <cuda_runtime.h>
+#include <cub/device/device_scan.cuh>
 
 #include <algorithm>
 #include <chrono>
@@ -107,6 +108,13 @@ struct cs_b200_handle {
   std::vector<DevLevel> lv32;
   void *R32 = nullptr, *X32 = nullptr, *T32 = nullptr, *Z32 = nullptr;
   void *d_cum = nullptr, *d_max = nullptr;
+  // branch currents (kernels.cuh k_branch_cur), all built on first use: d_bptr[n+1] the exclusive scan of the
+  // strictly-lower entry count per row (nb = d_bptr[n] branches), d_cum_branch the cumulative branch vector
+  // (nb), d_branch_stage the nb x ktmax download panel
+  int* d_bptr = nullptr;
+  int64_t nb = 0;
+  void* d_cum_branch = nullptr;
+  void* d_branch_stage = nullptr;
   PanelCtl* d_ctl = nullptr;
   PanelCtl* h_ctl = nullptr;  // pinned
   double* d_partials = nullptr;
@@ -1517,27 +1525,43 @@ struct ColumnDriver {
   }
 };
 
+// the grid of the node-current kernels
+template <int KT>
+int cur_grid(cs_b200_handle* h) {
+  return (int)std::min<int64_t>(h->grid_spmm, (h->n + (NT / KT) - 1) / (NT / KT));
+}
+
+// the branch-current maxima of the panel in X (ctl->maxpos / maxneg), the first pass of launch_currents
+template <typename T, int KT>
+void launch_cur_max(cs_b200_handle* h) {
+  const int grid = cur_grid<KT>(h);
+  if (h->A0.dia)
+    k_cur_max_dia<T, KT><<<grid, NT, 0, h->stream>>>(dia_view<T>(h->A0), (const T*)h->X, h->d_ctl, h->d_partials);
+  else
+    k_cur_max<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
+                                                 (const T*)h->X, h->d_ctl, h->d_partials);
+  h->stats.kernel_launches++;
+}
+
 // node currents of the panel in X (src/out.jl:178-290): branch-current maxima, then max(inflow, outflow)
 // per node with the 1e-8 zeroing, accumulated into the cumulative / max vectors (src/out.jl:100-107).
 // fg: the finite-ground currents of each node join the sums (cs_b200_solve_advanced), or null.
 template <typename T, int KT>
 void launch_currents(cs_b200_handle* h, bool want_curr, int accumulate, const void* fg = nullptr) {
-  const int grid = (int)std::min<int64_t>(h->grid_spmm, (h->n + (NT / KT) - 1) / (NT / KT));
+  const int grid = cur_grid<KT>(h);
+  launch_cur_max<T, KT>(h);
   if (h->A0.dia) {
     const DiaDev<T> a = dia_view<T>(h->A0);
-    k_cur_max_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, h->d_ctl, h->d_partials);
     k_cur_acc_dia<T, KT><<<grid, NT, 0, h->stream>>>(a, (const T*)h->X, (const T*)fg, h->d_ctl,
                                                      want_curr ? (T*)h->AP : nullptr,
                                                      (T*)h->d_cum, (T*)h->d_max, accumulate, h->opts.log_transform, KT);
   } else {
-    k_cur_max<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
-                                                 (const T*)h->X, h->d_ctl, h->d_partials);
     k_cur_acc<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
                                                  (const T*)h->X, (const T*)fg, h->d_ctl,
                                                  want_curr ? (T*)h->AP : nullptr,
                                                  (T*)h->d_cum, (T*)h->d_max, accumulate, h->opts.log_transform, KT);
   }
-  h->stats.kernel_launches += 2;
+  h->stats.kernel_launches++;
 }
 
 // ---- panel staging and downloads shared by the column kinds ------------------------------------
@@ -1922,6 +1946,122 @@ int grounded_panel(cs_b200_handle* h, int64_t c0, const int64_t* set_ptr, const 
   return CS_B200_OK;
 }
 
+// ---- branch currents (cs_b200_branch_index, cs_b200_solve_pairs_branch, cs_b200_solve_advanced_network) --
+// device scratch of one call, freed on every return path
+struct DevScratch {
+  void* p = nullptr;
+  DevScratch() = default;
+  DevScratch(const DevScratch&) = delete;
+  DevScratch& operator=(const DevScratch&) = delete;
+  ~DevScratch() { cudaFree(p); }
+};
+
+// d_bptr and nb, on first use (the CSR's pattern never changes after create); a row whose columns do not
+// ascend is CS_B200_ERR_ARG
+int ensure_branch_index(cs_b200_handle* h) {
+  if (h->d_bptr) return CS_B200_OK;
+  const int n = (int)h->n;
+  const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
+  DevScratch bptr, cnt, bad, tmp;
+  CK(h, cudaMalloc(&bptr.p, ((size_t)n + 1) * sizeof(int)));
+  CK(h, cudaMalloc(&cnt.p, std::max(1, n) * sizeof(int)));
+  CK(h, cudaMalloc(&bad.p, sizeof(int)));
+  const int none = INT32_MAX;
+  CK(h, h2d(h, bad.p, &none, sizeof(int)));
+  k_branch_count<<<g, 256, 0, h->stream>>>(n, h->d_rowptr, h->d_colidx, (int*)cnt.p, (int*)bad.p);
+  size_t tb = 0;
+  CK(h, cub::DeviceScan::InclusiveSum(nullptr, tb, (const int*)cnt.p, (int*)bptr.p + 1, n, h->stream));
+  CK(h, cudaMalloc(&tmp.p, std::max<size_t>(tb, 1)));
+  CK(h, cub::DeviceScan::InclusiveSum(tmp.p, tb, (const int*)cnt.p, (int*)bptr.p + 1, n, h->stream));
+  CK(h, cudaMemsetAsync(bptr.p, 0, sizeof(int), h->stream));
+  CK(h, cudaGetLastError());
+  int bad_row = none, nb = 0;
+  CK(h, cudaMemcpyAsync(&bad_row, bad.p, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaMemcpyAsync(&nb, (int*)bptr.p + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  h->stats.kernel_launches += 3;
+  if (bad_row != none)
+    return set_err(h, CS_B200_ERR_ARG, "row %d: column indices do not ascend (branch currents need sorted rows)",
+                   bad_row);
+  h->d_bptr = (int*)bptr.p;
+  bptr.p = nullptr;
+  h->nb = nb;
+  return CS_B200_OK;
+}
+
+// d_cum_branch, zeroed, on first use
+int ensure_cum_branch(cs_b200_handle* h) {
+  if (h->d_cum_branch) return CS_B200_OK;
+  const size_t bytes = (size_t)std::max<int64_t>(h->nb, 1) * h->esize();
+  CK(h, cudaMalloc(&h->d_cum_branch, bytes));
+  CK(h, cudaMemsetAsync(h->d_cum_branch, 0, bytes, h->stream));
+  return CS_B200_OK;
+}
+
+// the branch pass of the panel in X, after k_cur_max left its maxima in ctl: the branch currents into
+// columns c0 .. c0+KT-1 of the caller's column-major nb x k `branch` (or null), and with `accumulate`
+// weighted by ctl->weight into d_cum_branch.  Needs ensure_branch_index.
+template <typename T, int KT>
+int branch_pass(cs_b200_handle* h, int64_t c0, T* branch, int accumulate, int ncols) {
+  if ((!branch && !accumulate) || h->nb == 0) return CS_B200_OK;
+  if (branch && !h->d_branch_stage) CK(h, cudaMalloc(&h->d_branch_stage, (size_t)h->nb * h->ktmax * sizeof(T)));
+  if (accumulate)
+    if (int rc = ensure_cum_branch(h)) return rc;
+  const int grid = (int)std::min<int64_t>((int64_t)h->num_sms * 16, (h->n + NT - 1) / NT);
+  k_branch_cur<T, KT><<<grid, NT, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (const T*)h->d_vals,
+                                                  h->d_bptr, (const T*)h->X, h->d_ctl,
+                                                  branch ? (T*)h->d_branch_stage : nullptr, (size_t)h->nb,
+                                                  accumulate ? (T*)h->d_cum_branch : nullptr, ncols);
+  h->stats.kernel_launches++;
+  CK(h, cudaGetLastError());
+  if (branch) {
+    CK(h, cudaMemcpyAsync(branch + (size_t)c0 * h->nb, h->d_branch_stage, (size_t)h->nb * KT * sizeof(T),
+                          cudaMemcpyDeviceToHost, h->stream));
+    h->stats.d2h_bytes += (double)h->nb * KT * sizeof(T);
+  }
+  CK(h, cudaStreamSynchronize(h->stream));
+  return CS_B200_OK;
+}
+
+// cs_b200_solve_advanced_network: every column on grounded_panel, each column's voltages added into vsum
+// on the rows it owns, then one node-current and branch pass over vsum as a KT = 1 panel
+template <typename T>
+int advanced_network_t(cs_b200_handle* h, const int64_t* set_ptr, const int64_t* set_rows, int64_t k,
+                       const int64_t* gset, const int64_t* src_ptr, const int64_t* src_rows, const double* src_vals,
+                       const int64_t* owner, double rtol, int64_t itmax, T* volt, T* curr, T* branch,
+                       int64_t* iters, double* relres, ColumnDriver& cols) {
+  if (branch)
+    if (int rc = ensure_branch_index(h)) return rc;
+  const size_t np = (size_t)h->n_pad;
+  DevScratch vsum, own;
+  CK(h, cudaMalloc(&vsum.p, np * sizeof(T)));
+  CK(h, cudaMalloc(&own.p, (size_t)h->n * sizeof(long long)));
+  CK(h, cudaMemsetAsync(vsum.p, 0, np * sizeof(T), h->stream));
+  CK(h, h2d(h, own.p, owner, (size_t)h->n * sizeof(long long)));
+  const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
+  const int rc = cols.run(0, k, [&](auto kt, int64_t c0) -> int {
+    if (int rc = grounded_panel<T, kt>(h, c0, set_ptr, set_rows, gset, src_ptr, src_rows, src_vals, nullptr, rtol,
+                                       itmax, (T*)nullptr, (T*)nullptr, (T*)nullptr, 0, iters, relres, cols, h->d_fg))
+      return rc;
+    k_owner_sum<T, kt><<<g, 256, 0, h->stream>>>((int)h->n, (const T*)h->X, (const long long*)own.p, c0,
+                                                 (T*)vsum.p);
+    h->stats.kernel_launches++;
+    return CS_B200_OK;
+  });
+  if (rc) return rc;
+  // the whole graph's voltages as one column: one 1e-8 cut over the graph for node and branch currents
+  CK(h, cudaMemcpyAsync(h->X, vsum.p, np * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
+  if (int rc = upload_ctl(h, 1, [](int) { return ColCtl{-1, -1, 1.0}; })) return rc;
+  if (curr)
+    launch_currents<T, 1>(h, true, 0, h->d_fg);
+  else if (branch)
+    launch_cur_max<T, 1>(h);
+  if (int rc = download_outputs<T, 1>(h, 0, curr, volt, 0)) return rc;
+  if (int rc = branch_pass<T, 1>(h, 0, branch, 0, 1)) return rc;
+  CK(h, cudaStreamSynchronize(h->stream));
+  return CS_B200_OK;
+}
+
 template <typename T>
 int solve_pairs_superposed_t(cs_b200_handle* h, int64_t np, const int64_t* nodes, int64_t k,
                              const int64_t* pi, const int64_t* pj, const double* weight, double rtol,
@@ -2165,7 +2305,7 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 
 extern "C" {
 
-int cs_b200_version(void) { return 1007; }
+int cs_b200_version(void) { return 1008; }
 
 const char* cs_b200_last_error(const cs_b200_handle* h) {
   return h ? h->err.c_str() : g_create_error.c_str();
@@ -2605,6 +2745,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   if (h->owns_matrix) { cudaFree(h->d_rowptr); cudaFree(h->d_colidx); cudaFree(h->d_vals); }
   cudaFree(h->d_vals0);
   cudaFree(h->d_fg);
+  cudaFree(h->d_bptr); cudaFree(h->d_cum_branch); cudaFree(h->d_branch_stage);
   void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->P, h->P2, h->AP, h->B, h->stage,
                   h->d_cum, h->d_max, h->d_ctl, h->d_partials, h->d_flush};
   for (void* b : bufs) if (b) cudaFree(b);
@@ -2637,6 +2778,8 @@ int cs_b200_reset_currents(cs_b200_handle* h) {
     k_fill<double><<<g, 256, 0, h->stream>>>((double*)h->d_max, (size_t)h->n_pad, -9999.0);
   else
     k_fill<float><<<g, 256, 0, h->stream>>>((float*)h->d_max, (size_t)h->n_pad, -9999.0f);
+  if (h->d_cum_branch)
+    CK(h, cudaMemsetAsync(h->d_cum_branch, 0, (size_t)std::max<int64_t>(h->nb, 1) * h->esize(), h->stream));
   CK(h, cudaGetLastError());
   CK(h, cudaStreamSynchronize(h->stream));
   return CS_B200_OK;
@@ -2647,6 +2790,38 @@ int cs_b200_read_currents(cs_b200_handle* h, void* cum, void* max) {
   cudaSetDevice(h->device);
   if (cum) CK(h, cudaMemcpyAsync(cum, h->d_cum, (size_t)h->n * h->esize(), cudaMemcpyDeviceToHost, h->stream));
   if (max) CK(h, cudaMemcpyAsync(max, h->d_max, (size_t)h->n * h->esize(), cudaMemcpyDeviceToHost, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  return CS_B200_OK;
+}
+
+int cs_b200_read_branch_currents(cs_b200_handle* h, void* cum_branch) {
+  if (!h || !cum_branch) return set_err(h, CS_B200_ERR_ARG, "bad read_branch_currents arguments");
+  cudaSetDevice(h->device);
+  if (int rc = ensure_branch_index(h)) return rc;
+  const size_t bytes = (size_t)h->nb * h->esize();
+  if (h->d_cum_branch)
+    CK(h, cudaMemcpyAsync(cum_branch, h->d_cum_branch, bytes, cudaMemcpyDeviceToHost, h->stream));
+  else
+    std::memset(cum_branch, 0, bytes);   // no call has accumulated branch currents yet
+  CK(h, cudaStreamSynchronize(h->stream));
+  return CS_B200_OK;
+}
+
+int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* hi) {
+  if (!h || !nb) return set_err(h, CS_B200_ERR_ARG, "bad branch_index arguments");
+  cudaSetDevice(h->device);
+  if (int rc = ensure_branch_index(h)) return rc;
+  *nb = h->nb;
+  if ((!lo && !hi) || h->nb == 0) return CS_B200_OK;
+  DevScratch ends;
+  CK(h, cudaMalloc(&ends.p, (size_t)h->nb * 2 * sizeof(long long)));
+  long long* d_lo = (long long*)ends.p;
+  long long* d_hi = d_lo + h->nb;
+  const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
+  k_branch_ends<<<g, 256, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, h->d_bptr, d_lo, d_hi);
+  CK(h, cudaGetLastError());
+  if (lo) CK(h, cudaMemcpyAsync(lo, d_lo, (size_t)h->nb * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
+  if (hi) CK(h, cudaMemcpyAsync(hi, d_hi, (size_t)h->nb * sizeof(int64_t), cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
   return CS_B200_OK;
 }
@@ -2857,20 +3032,44 @@ int cs_b200_solve_rhs(cs_b200_handle* h, int64_t k, const void* rhs, void* lhs, 
   });
 }
 
-int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
-                        const double* weight, double rtol, int64_t itmax, void* R, void* volt,
-                        void* curr, int accumulate, int64_t* iters, double* relres) {
+// the pairs of cs_b200_solve_pairs / cs_b200_solve_pairs_branch (`who`)
+static int check_pairs(cs_b200_handle* h, const char* who, int64_t k, const int64_t* src, const int64_t* dst,
+                       const void* R, double rtol, int64_t itmax) {
   if (!h || k < 1 || !src || !dst || !R || !(rtol >= 0) || itmax < 0)
-    return set_err(h, CS_B200_ERR_ARG, "bad solve_pairs arguments");
+    return set_err(h, CS_B200_ERR_ARG, "bad %s arguments", who);
   for (int64_t c = 0; c < k; ++c)
     if (src[c] < 0 || src[c] >= h->n || dst[c] < 0 || dst[c] >= h->n || src[c] == dst[c])
       return set_err(h, CS_B200_ERR_ARG, "pair %lld: src/dst out of range or equal (%lld, %lld)",
                      (long long)c, (long long)src[c], (long long)dst[c]);
+  return CS_B200_OK;
+}
+
+int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
+                        const double* weight, double rtol, int64_t itmax, void* R, void* volt,
+                        void* curr, int accumulate, int64_t* iters, double* relres) {
+  if (int rc = check_pairs(h, "solve_pairs", k, src, dst, R, rtol, itmax)) return rc;
   return solve_call(h, [&](auto t, ColumnDriver& cols) {
     using T = decltype(t);
     return cols.run(0, k, [&](auto kt, int64_t c0) {
       return pairs_panel<T, kt>(h, c0, src, dst, weight, rtol, itmax, (T*)R, (T*)volt, (T*)curr, accumulate,
                                 iters, relres, cols);
+    });
+  });
+}
+
+int cs_b200_solve_pairs_branch(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
+                               const double* weight, double rtol, int64_t itmax, void* R, void* volt,
+                               void* curr, int accumulate, int64_t* iters, double* relres, void* branch) {
+  if (int rc = check_pairs(h, "solve_pairs_branch", k, src, dst, R, rtol, itmax)) return rc;
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    if (int rc = ensure_branch_index(h)) return rc;
+    return cols.run(0, k, [&](auto kt, int64_t c0) {
+      if (int rc = pairs_panel<T, kt>(h, c0, src, dst, weight, rtol, itmax, (T*)R, (T*)volt, (T*)curr, accumulate,
+                                      iters, relres, cols))
+        return rc;
+      if (!accumulate && !curr) launch_cur_max<T, kt>(h);   // pairs_panel ran it only for the node currents
+      return branch_pass<T, kt>(h, c0, (T*)branch, accumulate, kt);
     });
   });
 }
@@ -3042,6 +3241,43 @@ int cs_b200_solve_advanced(cs_b200_handle* h, int64_t nsets, const int64_t* set_
                                    itmax, (T*)nullptr, (T*)volt, (T*)curr, accumulate, iters, relres, cols,
                                    h->d_fg);
     });
+  });
+}
+
+int cs_b200_solve_advanced_network(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
+                                   const int64_t* set_rows, int64_t k, const int64_t* gset, const int64_t* src_ptr,
+                                   const int64_t* src_rows, const double* src_vals, const int64_t* owner,
+                                   double rtol, int64_t itmax, void* volt, void* curr, void* branch,
+                                   int64_t* iters, double* relres) {
+  if (int rc = check_grounded_columns(h, "solve_advanced_network", nsets, set_ptr, set_rows, k, gset, src_ptr,
+                                      src_rows, src_vals, rtol, itmax, true))
+    return rc;
+  if (!owner) return set_err(h, CS_B200_ERR_ARG, "bad solve_advanced_network arguments (owner)");
+  for (int64_t c = 0; c < k; ++c)
+    if (gset[c] < 0 && !(h && h->d_fg))
+      return set_err(h, CS_B200_ERR_ARG, "column %lld has no direct grounds and the handle no finite grounds "
+                     "(cs_b200_set_grounds)", (long long)c);
+  if (h) {                           // owner has the handle's n rows
+    for (int64_t r = 0; r < h->n; ++r)
+      if (owner[r] < -1 || owner[r] >= k)
+        return set_err(h, CS_B200_ERR_ARG, "owner[%lld] = %lld is not a column or -1", (long long)r,
+                       (long long)owner[r]);
+    for (int64_t c = 0; c < k; ++c) {
+      for (int64_t e = src_ptr[c]; e < src_ptr[c + 1]; ++e)
+        if (owner[src_rows[e]] != c)
+          return set_err(h, CS_B200_ERR_ARG, "column %lld: source row %lld is owned by column %lld", (long long)c,
+                         (long long)src_rows[e], (long long)owner[src_rows[e]]);
+      if (gset[c] >= 0)
+        for (int64_t e = set_ptr[gset[c]]; e < set_ptr[gset[c] + 1]; ++e)
+          if (owner[set_rows[e]] != c)
+            return set_err(h, CS_B200_ERR_ARG, "column %lld: ground row %lld is owned by column %lld",
+                           (long long)c, (long long)set_rows[e], (long long)owner[set_rows[e]]);
+    }
+  }
+  return solve_call(h, [&](auto t, ColumnDriver& cols) {
+    using T = decltype(t);
+    return advanced_network_t<T>(h, set_ptr, set_rows, k, gset, src_ptr, src_rows, src_vals, owner, rtol, itmax,
+                                 (T*)volt, (T*)curr, (T*)branch, iters, relres, cols);
   });
 }
 

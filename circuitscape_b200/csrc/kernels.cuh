@@ -2538,6 +2538,85 @@ k_cur_acc_dia(const DiaDev<T> A, const T* __restrict__ V, const T* __restrict__ 
   }
 }
 
+// ---------------------------------------------------------------------------
+// branch currents (out.jl:150-158, 250-290).  The branches of an operator are its stored strictly-lower
+// CSR entries (hi, lo < hi), ordered by hi, then lo: the columns of a row ascend, so branch bptr[hi] + t
+// is entry rowptr[hi] + t for t < bptr[hi+1] - bptr[hi].  For a symmetric operator this is the order of
+// the reference's CSC walk of the upper triangle (_convert_to_3col).
+// ---------------------------------------------------------------------------
+// cnt[row] = the row's strictly-lower entry count; *bad_row = the smallest row whose columns do not ascend
+__global__ void k_branch_count(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
+                               int* __restrict__ cnt, int* bad_row) {
+  for (int row = blockIdx.x * blockDim.x + threadIdx.x; row < n; row += gridDim.x * blockDim.x) {
+    int low = 0;
+    for (int j = rowptr[row]; j < rowptr[row + 1]; ++j) {
+      const int col = colidx[j];
+      if (j > rowptr[row] && col <= colidx[j - 1]) atomicMin(bad_row, row);
+      low += col < row;
+    }
+    cnt[row] = low;
+  }
+}
+
+// the 0-based endpoints of every branch
+__global__ void k_branch_ends(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx,
+                              const int* __restrict__ bptr, long long* __restrict__ lo, long long* __restrict__ hi) {
+  for (int row = blockIdx.x * blockDim.x + threadIdx.x; row < n; row += gridDim.x * blockDim.x)
+    for (int e = bptr[row], j = rowptr[row]; e < bptr[row + 1]; ++e, ++j) {
+      lo[e] = colidx[j];
+      hi[e] = row;
+    }
+}
+
+// Branch currents of the panel V (n_pad x KT, row-major), with the maxima maxpos that k_cur_max left in
+// ctl for the same panel: b = |a_{hi,lo}| (v_lo - v_hi), zeroed when |b / maxpos| < 1e-8 -- the test is
+// written as in k_cur_acc, so a NaN keeps its value as in the reference -- and output as |b|.
+// out: column-major nb x KT (leading dimension ld), or null.  cum: cum[e] += sum_c w_c |b_c| in fp64 in
+// column order over the columns c < ncols with w_c != 0, or null; never log-transformed (out.jl:62-84).
+// One thread walks one row's branches for every column, so each branch's sum has a single owner.
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_branch_cur(int n, const int* __restrict__ rowptr, const int* __restrict__ colidx, const T* __restrict__ vals,
+             const int* __restrict__ bptr, const T* __restrict__ V, const PanelCtl* ctl, T* __restrict__ out,
+             size_t ld, T* __restrict__ cum, int ncols) {
+  T maxpos[KT];
+#pragma unroll
+  for (int c = 0; c < KT; ++c) maxpos[c] = (T)ctl->maxpos[c];
+  for (int row = blockIdx.x * NT + threadIdx.x; row < n; row += gridDim.x * NT) {
+    const int e0 = bptr[row], e1 = bptr[row + 1];
+    if (e0 == e1) continue;
+    T vhi[KT];
+#pragma unroll
+    for (int c = 0; c < KT; ++c) vhi[c] = V[(size_t)row * KT + c];
+    for (int e = e0, j = rowptr[row]; e < e1; ++e, ++j) {
+      const int lo = colidx[j];
+      const T a = fabs(vals[j]);
+      double s = 0.0;
+#pragma unroll
+      for (int c = 0; c < KT; ++c) {
+        const T d = a * (V[(size_t)lo * KT + c] - vhi[c]);
+        const T b = !(fabs(d / maxpos[c]) < T(1e-8)) ? fabs(d) : T(0);
+        if (out) out[(size_t)c * ld + e] = b;
+        if (cum) {
+          const double w = ctl->weight[c];
+          if (c < ncols && w != 0.0) s += w * (double)b;
+        }
+      }
+      if (cum) cum[e] = (T)((double)cum[e] + s);
+    }
+  }
+}
+
+// advanced mode on a network: vsum[row] += X[row, owner[row] - c0] for the rows the panel's columns own
+template <typename T, int KT>
+__global__ void k_owner_sum(int n, const T* __restrict__ X, const long long* __restrict__ owner, long long c0,
+                            T* __restrict__ vsum) {
+  for (int row = blockIdx.x * blockDim.x + threadIdx.x; row < n; row += gridDim.x * blockDim.x) {
+    const long long c = owner[row] - c0;
+    if (c >= 0 && c < KT) vsum[row] += X[(size_t)row * KT + c];
+  }
+}
+
 __global__ void k_set_ctl(PanelCtl* ctl, double rtol, double atol, int itmax, int stall_limit) {
   ctl->stall_limit = stall_limit;
   ctl->rtol = rtol;

@@ -51,6 +51,8 @@ class CUDASolver:
                                      # device (cs_b200_set_grounds) instead of a new handle per solve
     onetoall_raster: bool = False    # one-to-all / all-to-one iterations as columns on one whole-raster
                                      # handle (core.plan_onetoall); takes precedence over batch_*
+    branch_on_device: bool = False   # network pairwise: branch currents and their cumulative vector on the
+                                     # device (cs_b200_solve_pairs_branch) instead of from per-pair voltages
 
     @property
     def dtype(self):
@@ -365,20 +367,51 @@ class B200Factor:
         return (x[:, 0] if vec else x), iters, relres
 
     def solve_pairs(self, src, dst, weight=None, want_volt=False, want_curr=False,
-                    accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
+                    accumulate=False, rtol=None, itmax=None, raise_on_residual=True, want_branch=False):
         """Batched focal-pair solve (src/dst 0-based rows).  Returns dict with
-        R (k,), volt (n,k)|None, curr (n,k)|None, iters, relres."""
+        R (k,), volt (n,k)|None, curr (n,k)|None, iters, relres, branch (nb,k)|None.
+        want_branch: per-pair branch currents in the order of branch_index(), and with accumulate their
+        cumulative vector on the device (cs_b200_solve_pairs_branch, read_branch_currents)."""
         src = np.ascontiguousarray(src, dtype=np.int64)
         dst = np.ascontiguousarray(dst, dtype=np.int64)
         k = len(src)
         R = np.zeros(k, dtype=self.dtype)
         volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
-        rc = self._lib.cs_b200_solve_pairs(self._h, k, _lib._ptr(src), _lib._ptr(dst),
-                                           _lib._ptr(_opt(weight, np.float64)), *self._limits(rtol, itmax),
-                                           _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0,
-                                           _lib._ptr(iters), _lib._ptr(relres))
+        args = (self._h, k, _lib._ptr(src), _lib._ptr(dst), _lib._ptr(_opt(weight, np.float64)),
+                *self._limits(rtol, itmax), _lib._ptr(R), _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0,
+                _lib._ptr(iters), _lib._ptr(relres))
+        branch = None
+        if want_branch:
+            branch = np.empty((self._num_branches(), k), dtype=self.dtype, order="F")
+            rc = self._lib.cs_b200_solve_pairs_branch(*args, _lib._ptr(branch))
+        else:
+            rc = self._lib.cs_b200_solve_pairs(*args)
         self._raise(rc, raise_on_residual)
-        return dict(R=self._io(R), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
+        return dict(R=self._io(R), volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres,
+                    branch=self._io(branch))
+
+    def _num_branches(self):
+        """nb, the number of stored strictly-lower entries of the operator (cs_b200_branch_index)."""
+        nb = C.c_int64()
+        _lib.check(self._lib, self._h, self._lib.cs_b200_branch_index(self._h, C.byref(nb), None, None))
+        return nb.value
+
+    def branch_index(self):
+        """The operator's branches (cs_b200_branch_index): (lo, hi), 0-based int64 arrays with lo < hi, one per
+        stored strictly-lower entry, ordered by hi, then lo -- the order of every branch output."""
+        nb = self._num_branches()
+        lo = np.empty(nb, dtype=np.int64)
+        hi = np.empty(nb, dtype=np.int64)
+        n_ = C.c_int64()
+        _lib.check(self._lib, self._h,
+                   self._lib.cs_b200_branch_index(self._h, C.byref(n_), _lib._ptr(lo), _lib._ptr(hi)))
+        return lo, hi
+
+    def read_branch_currents(self):
+        """The cumulative branch vector (nb,) that solve_pairs(want_branch=True, accumulate=True) adds into."""
+        cum = np.empty(self._num_branches(), dtype=self.dtype)
+        _lib.check(self._lib, self._h, self._lib.cs_b200_read_branch_currents(self._h, _lib._ptr(cum)))
+        return cum
 
     def solve_pairs_superposed(self, nodes, pi, pj, weight=None, want_volt=False, want_curr=False,
                                accumulate=False, rtol=None, itmax=None, raise_on_residual=True):
@@ -464,6 +497,33 @@ class B200Factor:
             _lib._ptr(volt), _lib._ptr(curr), 1 if accumulate else 0, _lib._ptr(iters), _lib._ptr(relres))
         self._raise(rc, raise_on_residual)
         return dict(volt=self._io(volt), curr=self._io(curr), iters=iters, relres=relres)
+
+    def solve_advanced_network(self, sets, gset, sources, owner, want_volt=False, want_curr=False,
+                               want_branch=False, rtol=None, itmax=None, raise_on_residual=True):
+        """Network advanced mode on this whole-graph operator (cs_b200_solve_advanced_network): the columns of
+        solve_advanced (sets, gset with -1 for finite grounds only, sources), owner (n,) the column whose
+        component holds each row, or -1.  The columns' voltages are summed on the rows they own; returns dict
+        with volt (n,), curr (n,) (node currents with the finite-ground currents) and branch (nb,) of that one
+        vector under one 1e-8 cut over the graph (each None unless wanted), iters, relres."""
+        ptr, rows = _csr(sets, np.int64)
+        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        k = len(gset)
+        assert len(sources) == k
+        sptr, srows = _csr([r for r, _ in sources], np.int64)
+        _, svals = _csr([v for _, v in sources], np.float64)
+        assert len(srows) == len(svals) == sptr[-1]
+        owner = np.ascontiguousarray(owner, dtype=np.int64)
+        assert len(owner) == self.n
+        vec = lambda want, m: np.empty(m, dtype=self.dtype) if want else None
+        volt, curr = vec(want_volt, self.n), vec(want_curr, self.n)
+        branch = vec(want_branch, self._num_branches() if want_branch else 0)
+        iters, relres = np.zeros(k, dtype=np.int64), np.zeros(k, dtype=np.float64)
+        rc = self._lib.cs_b200_solve_advanced_network(
+            self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(gset), _lib._ptr(sptr),
+            _lib._ptr(srows), _lib._ptr(svals), _lib._ptr(owner), *self._limits(rtol, itmax), _lib._ptr(volt),
+            _lib._ptr(curr), _lib._ptr(branch), _lib._ptr(iters), _lib._ptr(relres))
+        self._raise(rc, raise_on_residual)
+        return dict(volt=self._io(volt), curr=self._io(curr), branch=self._io(branch), iters=iters, relres=relres)
 
     def solve_sources(self, columns, ref, probe=None, weight=None, want_volt=False, want_curr=False,
                       accumulate=False, rtol=None, itmax=None, raise_on_residual=True):

@@ -222,6 +222,23 @@ int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const 
                         void* volt, void* curr, int accumulate, int64_t* iters,
                         double* relres);
 
+/* Branches of the handle's operator (network mode): its stored strictly-lower CSR entries (hi, lo < hi),
+ * ordered by hi, then lo -- for a symmetric operator the order in which the reference writes branch
+ * currents (src/out.jl:128-148, 250-278).  Built on the device on first use and kept until cs_b200_destroy;
+ * a row whose column indices do not ascend is CS_B200_ERR_ARG (the row in cs_b200_last_error).  Returns nb
+ * and, for non-NULL lo / hi, the nb 0-based endpoints of every branch.                                   */
+int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* hi);
+
+/* cs_b200_solve_pairs with branch currents (network pairwise, src/out.jl:150-158, 250-290): arguments and
+ * outputs as cs_b200_solve_pairs, plus branch: NULL or host column-major nb x k of the per-pair branch
+ * currents |b|, b = |a_{hi,lo}| (v_lo - v_hi) zeroed where |b / max_e b| < 1e-8 (the maximum over the
+ * column's branches, as the node currents use it).  With accumulate, each column's branch currents are
+ * also added weight[c] times into the handle's cumulative branch vector (cs_b200_read_branch_currents;
+ * summed in fp64 in column order, no log transform).  The other entry points never touch that vector.   */
+int cs_b200_solve_pairs_branch(cs_b200_handle* h, int64_t k, const int64_t* src, const int64_t* dst,
+                               const double* weight, double rtol, int64_t itmax, void* R, void* volt,
+                               void* curr, int accumulate, int64_t* iters, double* relres, void* branch);
+
 /* Pairwise driver by SUPERPOSITION -- the reference's Shortcut (src/core.jl:685-739), extended
  * to voltage / current maps.  All pairs among `np` focal nodes of ONE connected component share
  * the operator and are linear in the right-hand side, so np-1 solves
@@ -279,6 +296,21 @@ int cs_b200_solve_advanced(cs_b200_handle* h, int64_t nsets, const int64_t* set_
                            const double* src_vals, const double* weight, double rtol, int64_t itmax, void* volt,
                            void* curr, int accumulate, int64_t* iters, double* relres);
 
+/* Network advanced mode on ONE whole-graph operator (src/raster/advanced.jl:184-242 for networks): the columns
+ * are solved as in cs_b200_solve_advanced (sets, gset with -1 for finite grounds only, sources, rtol, itmax,
+ * iters, relres).  owner: n values, owner[row] = the column whose connected component contains row, or -1.
+ * Each column's voltages are added into one vector on the rows it owns; volt (n), curr (n) and branch (nb,
+ * order of cs_b200_branch_index) -- each may be NULL -- are that vector, its node currents with the
+ * finite-ground currents, and its branch currents, all under ONE 1e-8 cut over the whole graph, as the
+ * reference takes them of the summed voltages.  The cumulative vectors are not touched.  owner values
+ * outside [-1, k), a source or ground-set row of column c not owned by c, and the checks of
+ * cs_b200_solve_advanced are CS_B200_ERR_ARG before any device work.                                     */
+int cs_b200_solve_advanced_network(cs_b200_handle* h, int64_t nsets, const int64_t* set_ptr,
+                                   const int64_t* set_rows, int64_t k, const int64_t* gset, const int64_t* src_ptr,
+                                   const int64_t* src_rows, const double* src_vals, const int64_t* owner,
+                                   double rtol, int64_t itmax, void* volt, void* curr, void* branch,
+                                   int64_t* iters, double* relres);
+
 /* Batched solve with SPARSE right-hand sides, device-resident -- the advanced-mode kernel
  * (src/raster/advanced.jl:274-305) for source/ground sets without finite grounds, and
  * the all-to-one loop built on it (src/raster/onetoall.jl:110-118,146-151):
@@ -324,6 +356,9 @@ int cs_b200_solve_advanced_batch(int64_t nwin, int64_t nrows, int64_t ncols, con
  * NULL).  max is initialised to -9999 like src/utils.jl:124.                        */
 int cs_b200_read_currents(cs_b200_handle* h, void* cum, void* max);
 int cs_b200_reset_currents(cs_b200_handle* h);
+/* The cumulative branch vector of cs_b200_solve_pairs_branch (nb values of dtype; zeros before any
+ * accumulation).  cs_b200_reset_currents zeroes it with the node vectors.                           */
+int cs_b200_read_branch_currents(cs_b200_handle* h, void* cum_branch);
 /* Device pointers of the same vectors (for an NCCL reduce across ranks).            */
 int cs_b200_currents_device_ptrs(cs_b200_handle* h, void** d_cum, void** d_max);
 
