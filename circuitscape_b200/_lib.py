@@ -108,6 +108,7 @@ _PROTOS = {
                                              C.c_void_p, C.c_void_p]),
     "cs_b200_branch_index": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
     "cs_b200_read_branch_currents": (C.c_int, [_H, C.c_void_p]),
+    "cs_b200_components": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_void_p]),
     "cs_b200_read_currents": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "cs_b200_reset_currents": (C.c_int, [_H]),
     "cs_b200_currents_device_ptrs": (C.c_int, [_H, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),

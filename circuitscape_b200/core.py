@@ -822,7 +822,8 @@ class OneToAllOutput:
 # ---------------------------------------------------------------------------
 def raster_pairwise(data: RasterData, flags: Flags, cfg, solver=None, four_neighbors=False, avg_res=False,
                     sink=None) -> PairwiseOutput:
-    """src/raster/pairwise.jl:14-30.  Focal points with distinct ids: one graph, single_ground_all_pairs.
+    """src/raster/pairwise.jl:14-30.  Focal points with distinct ids: one graph, single_ground_all_pairs (with
+    CUDASolver(pairwise_raster=True): every component's pairs on one whole-raster handle, _raster_pairs_device).
     An id on several cells makes focal regions (_pt_file_polygons_path): every region pair is a Dirichlet
     problem on the raster's own Laplacian (region a at 0 V, region b at 1 V), so the pairs are columns of
     cs_b200_solve_region_pairs on ONE whole-raster handle; pairs that operator cannot express exactly take
@@ -836,6 +837,9 @@ def raster_pairwise(data: RasterData, flags: Flags, cfg, solver=None, four_neigh
     regions = len(points_rc[0]) != len(np.unique(points_rc[2]))
     if inc is not None:
         points_rc, exclude = graph.generate_exclude_pairs(points_rc, inc)
+    if not regions and getattr(solver, "pairwise_raster", False):
+        return _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res,
+                                    sink)
     if not regions:
         nodemap = graph.construct_node_map(cellmap, polymap)
         G = graph.laplacian(graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors))
@@ -844,6 +848,181 @@ def raster_pairwise(data: RasterData, flags: Flags, cfg, solver=None, four_neigh
                             cellmap, solver)
         return single_ground_all_pairs(prob, flags, cfg, sink=sink)
     return _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink)
+
+
+def _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink):
+    """`solve` for raster focal points with distinct ids (CUDASolver(pairwise_raster=True)) on ONE whole-raster
+    handle: node map and operator assembled on the device, connected components labelled there
+    (cs_b200_components), no host graph.  Each component's pairs come from component_pairs on its focal nodes;
+    the pairs of every component are columns of the same solve_pairs / solve_sources panels (the operator is
+    block-diagonal: a column's other components stay constant, so they carry no current).  Components whose
+    construct_local_node_map numbers cells unlike the node map (a NODATA cell of a merged polygon) bring their
+    currents back and are scattered by their own map on the host.  Returns what `solve` returns."""
+    o = flags.outputflags
+    want_maps = o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
+    shortcut = not want_maps and not exclude                                     # src/core.jl:356-364
+    need_curr = not shortcut
+    per_pair_curr = need_curr and o.write_cur_maps and not o.write_cum_cur_map_only
+    superpose = getattr(solver, "superpose", False) and not shortcut
+    ids = np.asarray(points_rc[2])
+    P = len(ids)
+    R = -np.ones((P, P))
+    voltmatrix = np.zeros((P, P))
+    shortcut_res = -np.ones((P, P))
+    out = PairwiseOutput(resistances=None)
+    out.cum_curmap = np.zeros(cellmap.shape)
+    out.max_curmap = np.full(cellmap.shape, NODATA) if o.write_max_cur_maps else None
+    factor, nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                                avg_res=avg_res, log_transform=o.log_transform_maps)
+    with factor:
+        nodemap = np.asarray(nodemap, dtype=np.int64)
+        _, comp_of = factor.components()
+        points = nodemap[points_rc[0] - 1, points_rc[1] - 1]
+        focal = np.nonzero(points != 0)[0]
+        # one entry per component holding focal points, in component order: (index, focal nodes 1-based)
+        fcomp = comp_of[points[focal] - 1]
+        comps = [(int(ci), np.unique(points[focal[fcomp == ci]])) for ci in np.unique(fcomp)]
+        columns, own, super_comps = [], {}, []      # columns: (component, src row, dst row, fan)
+        for ci, cnodes in comps:
+            _, solves, zero = component_pairs(points, ids, exclude, cnodes, shortcut)
+            for a, b in zero:
+                R[a, b] = R[b, a] = 0.0
+            if not solves:
+                continue
+            if need_curr and polymap is not None and not _local_map_is_global(nodemap, comp_of, ci, polymap):
+                rows = np.nonzero(comp_of == ci)[0]
+                own[ci] = (rows, construct_local_node_map(nodemap, rows + 1, polymap))
+            cols = [(ci, s - 1, d - 1, fan) for s, d, fan in solves]
+            if superpose and len(solves) > 1:
+                super_comps.append(cols)
+            else:
+                columns += cols
+        if need_curr:
+            factor.reset_currents()
+        focal_rows = np.unique(points[focal] - 1)
+        focal_col = {int(r): i for i, r in enumerate(focal_rows)}
+        bs = max(1, int(solver.bs))
+        host_cum = {ci: (np.zeros(len(rows)), np.full(len(rows), NODATA), 0.0) for ci, (rows, _) in own.items()}
+        masks = {}
+
+        def batches():
+            """(columns, result) per device call: the own-map columns apart, with accumulate=False"""
+            for acc in (True, False):
+                sel = [c for c in columns if (c[0] in own) != acc]
+                for st in range(0, len(sel), bs):
+                    chunk = sel[st:st + bs]
+                    src = np.array([c[1] for c in chunk], dtype=np.int64)
+                    dst = np.array([c[2] for c in chunk], dtype=np.int64)
+                    if shortcut:
+                        # only the voltages at the focal nodes are used (src/core.jl:685-703)
+                        res = factor.solve_sources([([s_, d_], [-1.0, 1.0]) for s_, d_ in zip(src, dst)], ref=src,
+                                                   probe=focal_rows)
+                        res["R"] = np.array([res["probe_volt"][c, focal_col[int(d_)]] for c, d_ in enumerate(dst)])
+                    else:
+                        res = factor.solve_pairs(src, dst, np.array([len(c[3]) for c in chunk], dtype=np.float64),
+                                                 want_volt=o.write_volt_maps, want_curr=per_pair_curr or not acc,
+                                                 accumulate=acc)
+                    yield chunk, res
+            for chunk in super_comps:
+                acc = chunk[0][0] not in own
+                src = np.array([c[1] for c in chunk], dtype=np.int64)
+                dst = np.array([c[2] for c in chunk], dtype=np.int64)
+                nodes, inv = np.unique(np.concatenate([src, dst]), return_inverse=True)
+                yield chunk, factor.solve_pairs_superposed(
+                    nodes, inv[:len(src)], inv[len(src):], np.array([len(c[3]) for c in chunk], dtype=np.float64),
+                    want_volt=o.write_volt_maps, want_curr=per_pair_curr or not acc, accumulate=acc)
+
+        def local(ci, x):
+            """column x (n,) restricted to component ci, as a cell map of that component's local node map"""
+            if ci in own:
+                rows, lm = own[ci]
+                return _scatter(np.asarray(x, dtype=np.float64)[rows], lm)
+            if ci not in masks:
+                masks[ci] = comp_of == ci
+            return _scatter(np.where(masks[ci], np.asarray(x, dtype=np.float64), 0.0), nodemap)
+
+        for chunk, res in batches():
+            out.stats.append(factor.stats())
+            out.num_solves += len(res["R"])
+            out.iterations += int(res["iters"].sum())
+            for col, (ci, s, d, fan) in enumerate(chunk):
+                r = float(res["R"][col])
+                cur = None if res.get("curr") is None else res["curr"][:, col]
+                if ci in own:                          # the accumulation of `solve`'s handle, on the host
+                    rows = own[ci][0]
+                    c = np.asarray(cur, dtype=np.float64)[rows]
+                    if o.log_transform_maps:
+                        c = np.where(c > 0, np.log10(np.where(c > 0, c, 1.0)), NODATA)
+                    cum, mx, w = host_cum[ci]
+                    host_cum[ci] = (cum + len(fan) * c, np.maximum(mx, c), w + len(fan))
+                for ci_, cj in fan:
+                    R[ci_, cj] = R[cj, ci_] = r
+                    key = (int(ids[ci_]), int(ids[cj]))
+                    if shortcut:                                                 # src/core.jl:685-703
+                        pv = res["probe_volt"][col]
+                        inside = focal[fcomp == ci]
+                        for i in inside[inside >= 1]:
+                            voltmatrix[i, cj] = 1.0 - float(pv[focal_col[int(points[i]) - 1]]) / r
+                        continue
+                    if o.write_volt_maps:
+                        vm = _process_grid(local(ci, res["volt"][:, col]), cellmap, False, o.set_null_voltages_to_nodata)
+                        if sink is not None:
+                            sink.voltmap(key, vm)
+                        else:
+                            out.voltmaps[key] = vm
+                    if per_pair_curr:
+                        cm = _process_grid(local(ci, cur), cellmap, o.log_transform_maps, o.set_null_currents_to_nodata)
+                        if sink is not None:
+                            sink.curmap(key, cm)
+                        else:
+                            out.curmaps[key] = cm
+        accumulated = [c for c in columns + [x for sc in super_comps for x in sc] if c[0] not in own]
+        if need_curr and accumulated:
+            # the device's cumulative / max vectors: a column adds f(0) (0, or -9999 under log) on every row of the
+            # other components, which is what `solve` adds there per component; cells that are no node get the same
+            npost = float(sum(len(c[3]) for c in accumulated))
+            cum, mx = factor.read_currents(want_max=True)
+            off = nodemap == 0
+            cmap = _scatter(cum.astype(np.float64), nodemap)
+            if o.log_transform_maps:
+                cmap = np.where(off, NODATA * npost, cmap)
+            if o.set_null_currents_to_nodata:
+                cmap = np.where(cellmap == 0, NODATA * npost, cmap)
+            out.cum_curmap += cmap
+            if out.max_curmap is not None:
+                mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, _scatter(mx.astype(np.float64), nodemap))
+                if o.set_null_currents_to_nodata:
+                    mmap = np.where(cellmap == 0, NODATA, mmap)
+                out.max_curmap = np.maximum(out.max_curmap, mmap)
+    for ci, (cum, mx, npost) in host_cum.items():                      # as `solve` scatters one component
+        lm = own[ci][1]
+        cmap = _scatter(cum, lm)
+        if o.log_transform_maps:
+            cmap = np.where(lm == 0, NODATA * npost, cmap)
+        if o.set_null_currents_to_nodata:
+            cmap = np.where(cellmap == 0, NODATA * npost, cmap)
+        out.cum_curmap += cmap
+        if out.max_curmap is not None:
+            mmap = np.where(lm == 0, NODATA if o.log_transform_maps else 0.0, _scatter(mx, lm))
+            if o.set_null_currents_to_nodata:
+                mmap = np.where(cellmap == 0, NODATA, mmap)
+            out.max_curmap = np.maximum(out.max_curmap, mmap)
+    if shortcut:
+        for ci, cnodes in comps:
+            csub = [int(points[k]) for k in focal[fcomp == ci]]
+            _update_shortcut_resistances(int(np.nonzero(points == csub[0])[0][0]), voltmatrix, shortcut_res, R,
+                                         points, cnodes)
+        R = shortcut_res
+    np.fill_diagonal(R, 0.0)
+    full = np.zeros((P + 1, P + 1))
+    full[0, 1:] = ids
+    full[1:, 0] = ids
+    full[1:, 1:] = R
+    out.resistances = full                                                      # src/core.jl:294-299
+    out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)   # src/utils.jl:114-120
+    if out.max_curmap is not None:
+        out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
+    return out
 
 
 @dataclass

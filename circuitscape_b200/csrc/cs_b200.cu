@@ -2826,6 +2826,54 @@ int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* h
   return CS_B200_OK;
 }
 
+int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
+  if (!h || !ncomp) return set_err(h, CS_B200_ERR_ARG, "bad components arguments");
+  cudaSetDevice(h->device);
+  h->err.clear();
+  const int n = (int)h->n;
+  *ncomp = 0;
+  if (n == 0) return CS_B200_OK;
+  // scratch from the stream-ordered pool, released before return: parent, root flags, their exclusive scan,
+  // each row's root, then its label (n each) and cub's temporary storage
+  size_t tb = 0;
+  CK(h, cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int*)nullptr, (int*)nullptr, n, h->stream));
+  const size_t ib = (size_t)n * sizeof(int), ia = (ib + 255) & ~(size_t)255;
+  const size_t off_root = ia, off_idx = 2 * ia, off_lab = 3 * ia, off_tmp = 4 * ia;
+  char* s = nullptr;
+  CK(h, cudaMallocAsync((void**)&s, off_tmp + std::max<size_t>(tb, 1), h->stream));
+  int* parent = (int*)s;
+  int* root = (int*)(s + off_root);
+  int* idx = (int*)(s + off_idx);
+  int* lab = (int*)(s + off_lab);
+  const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
+  constexpr int CHUNK = 16;
+  const int ge = (int)std::max<int64_t>(1, std::min<int64_t>((h->nnz / CHUNK + 255) / 256, (int64_t)h->num_sms * 32));
+  const void* vals = h->d_vals0 ? h->d_vals0 : h->d_vals;    // pristine values: grounds do not split
+  k_cc_init<<<g, 256, 0, h->stream>>>(n, parent);
+  if (h->dtype == CS_B200_F64)
+    k_cc_hook<double><<<ge, 256, 0, h->stream>>>(n, (int)h->nnz, h->d_rowptr, h->d_colidx, (const double*)vals,
+                                                 parent, CHUNK);
+  else
+    k_cc_hook<float><<<ge, 256, 0, h->stream>>>(n, (int)h->nnz, h->d_rowptr, h->d_colidx, (const float*)vals,
+                                                parent, CHUNK);
+  k_cc_compress<<<g, 256, 0, h->stream>>>(n, parent, lab, root);
+  cudaError_t e = cub::DeviceScan::ExclusiveSum(s + off_tmp, tb, root, idx, n, h->stream);
+  int total = 0, last_flag = 0;
+  if (e == cudaSuccess) {
+    if (comp_of) k_cc_label<<<g, 256, 0, h->stream>>>(n, lab, idx);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&total, idx + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(&last_flag, root + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess && comp_of) e = cudaMemcpyAsync(comp_of, lab, ib, cudaMemcpyDeviceToHost, h->stream);
+  cudaFreeAsync(s, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (components)", cudaGetErrorString(e));
+  h->stats.kernel_launches += comp_of ? 5 : 4;
+  *ncomp = (int64_t)total + last_flag;
+  return CS_B200_OK;
+}
+
 int cs_b200_currents_device_ptrs(cs_b200_handle* h, void** d_cum, void** d_max) {
   if (!h) return CS_B200_ERR_ARG;
   if (d_cum) *d_cum = h->d_cum;

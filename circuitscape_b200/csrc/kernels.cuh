@@ -2766,4 +2766,75 @@ k_cur_accum(int n, const T* __restrict__ C, const PanelCtl* __restrict__ ctl, T*
   }
 }
 
+
+// ---------------------------------------------------------------------------
+// connected components of an operator (cs_b200_components): union-find over the stored off-diagonal
+// entries whose value is != 0 (a NaN is an edge), with integer atomics only.  A union always hangs the
+// larger root under the smaller, so parent[v] <= v throughout and every root ends as its component's
+// smallest row: the labels do not depend on the order in which the hooks race.
+// ---------------------------------------------------------------------------
+// the root of v, halving the path on the way up (a racing write only ever stores another ancestor of v)
+__device__ __forceinline__ int cc_find(int* parent, int v) {
+  int p = __ldcg(parent + v);
+  while (p != v) {
+    const int gp = __ldcg(parent + p);
+    if (gp == p) return p;
+    parent[v] = gp;
+    v = gp;
+    p = __ldcg(parent + v);
+  }
+  return v;
+}
+
+__global__ void k_cc_init(int n, int* __restrict__ parent) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) parent[v] = v;
+}
+
+// edge-parallel hooking: thread t takes the entries [t * chunk, (t + 1) * chunk), finds the first one's row
+// by bisection of rowptr and walks on, so a row of thousands of entries (a merged polygon) is spread over
+// many threads
+template <typename T>
+__global__ void k_cc_hook(int n, int nnz, const int* __restrict__ rowptr, const int* __restrict__ colidx,
+                          const T* __restrict__ vals, int* parent, int chunk) {
+  for (int64_t j0 = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) * chunk; j0 < nnz;
+       j0 += (int64_t)gridDim.x * blockDim.x * chunk) {
+    int lo = 0, hi = n;                            // the last row with rowptr[row] <= j0
+    while (hi - lo > 1) {
+      const int mid = (lo + hi) >> 1;
+      if (rowptr[mid] <= j0) lo = mid; else hi = mid;
+    }
+    int row = lo;
+    const int j1 = (int)(j0 + chunk < nnz ? j0 + chunk : nnz);
+    for (int j = (int)j0; j < j1; ++j) {
+      while (rowptr[row + 1] <= j) ++row;
+      const int col = colidx[j];
+      if (col == row || !(vals[j] != T(0))) continue;
+      int a = cc_find(parent, row), b = cc_find(parent, col);
+      while (a != b) {
+        if (a > b) { const int t = a; a = b; b = t; }
+        const int was = atomicCAS(parent + b, b, a);   // hang the larger root under the smaller
+        if (was == b) break;
+        b = cc_find(parent, was);                      // b was hooked meanwhile: retry from its new root
+        a = cc_find(parent, a);
+      }
+    }
+  }
+}
+
+// rootof[v] = the root of v, flag[v] = 1 for the roots (what the label scan numbers).  The roots go to their own
+// array: a racing path-halving write may still store a non-root ancestor into parent[v] after v's own thread
+// has stored the root there
+__global__ void k_cc_compress(int n, int* parent, int* __restrict__ rootof, int* __restrict__ flag) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
+    const int r = cc_find(parent, v);
+    rootof[v] = r;
+    flag[v] = r == v;
+  }
+}
+
+// lab[v] = number of roots below v's root, in place over rootof (idx = the exclusive scan of the root flags)
+__global__ void k_cc_label(int n, int* __restrict__ lab, const int* __restrict__ idx) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) lab[v] = idx[lab[v]];
+}
+
 }  // namespace csb

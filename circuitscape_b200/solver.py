@@ -53,6 +53,9 @@ class CUDASolver:
                                      # handle (core.plan_onetoall); takes precedence over batch_*
     branch_on_device: bool = False   # network pairwise: branch currents and their cumulative vector on the
                                      # device (cs_b200_solve_pairs_branch) instead of from per-pair voltages
+    pairwise_raster: bool = False    # raster pairwise with distinct point ids: every component's pairs as columns
+                                     # on one whole-raster handle, components labelled on the device
+                                     # (core._raster_pairs_device) instead of a host graph and a handle per component
 
     @property
     def dtype(self):
@@ -407,6 +410,15 @@ class B200Factor:
                    self._lib.cs_b200_branch_index(self._h, C.byref(n_), _lib._ptr(lo), _lib._ptr(hi)))
         return lo, hi
 
+    def components(self):
+        """Connected components of the operator, labelled on the device (cs_b200_components): (ncomp, comp_of)
+        with comp_of (n,) int32 numbered in order of each component's smallest row -- SciPy's labels of the
+        pristine operator's nonzero off-diagonal pattern."""
+        nc = C.c_int64()
+        comp_of = np.empty(self.n, dtype=np.int32)
+        _lib.check(self._lib, self._h, self._lib.cs_b200_components(self._h, C.byref(nc), _lib._ptr(comp_of)))
+        return nc.value, comp_of
+
     def read_branch_currents(self):
         """The cumulative branch vector (nb,) that solve_pairs(want_branch=True, accumulate=True) adds into."""
         cum = np.empty(self._num_branches(), dtype=self.dtype)
@@ -620,7 +632,7 @@ def construct_cholesky_factor(matrix, solver: CUDASolver, **kw) -> B200Factor:
 
 def construct_raster_factor(cellmap, polymap, solver: CUDASolver, four_neighbors=False, avg_res=False,
                             log_transform=False):
-    """The whole-raster operator of a focal-region, one-to-all or advanced-mode job and its node map
+    """The whole-raster operator of a pairwise, focal-region, one-to-all or advanced-mode job and its node map
     (1-based, 0 = none): B200Factor.from_raster_polygons.  Not one of the three hooks: those drivers need
     the handle's column entries (cs_b200_solve_region_pairs / _grounded / _advanced), which the Solver
     interface has no method for."""

@@ -229,6 +229,15 @@ int cs_b200_solve_pairs(cs_b200_handle* h, int64_t k, const int64_t* src, const 
  * and, for non-NULL lo / hi, the nb 0-based endpoints of every branch.                                   */
 int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* hi);
 
+/* Connected components of the handle's operator, labelled on the device: an edge is a stored off-diagonal
+ * entry whose value is != 0 (a NaN counts, stored zeros and the diagonal do not) -- what
+ * eliminate_zeros() + csgraph.connected_components(directed=False) sees.  After cs_b200_set_grounds the
+ * pristine values are used, so identity rows do not split components.  Returns ncomp and, for non-NULL
+ * comp_of (n int32 on the host), each row's component, numbered in order of each component's smallest row
+ * (SciPy's labels exactly).  Union-find with integer atomics: the output does not depend on the order of the
+ * races.  Scratch comes from the stream-ordered pool and is released before return.                      */
+int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of);
+
 /* cs_b200_solve_pairs with branch currents (network pairwise, src/out.jl:150-158, 250-290): arguments and
  * outputs as cs_b200_solve_pairs, plus branch: NULL or host column-major nb x k of the per-pair branch
  * currents |b|, b = |a_{hi,lo}| (v_lo - v_hi) zeroed where |b / max_e b| < 1e-8 (the maximum over the
