@@ -173,6 +173,99 @@ def _process_grid(cmap, cellmap, log_transform, set_null_to_nodata):
     return cmap
 
 
+def _any_map(o):
+    """Whether the job writes any current or voltage map (src/core.jl:356-364: otherwise raster pairwise
+    takes the shortcut)."""
+    return o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
+
+
+def _panels(n, solver):
+    """Slices of at most solver.bs columns over n columns (cholmod_batch_size, src/core.jl:448-452)."""
+    bs = max(1, int(solver.bs))
+    for st in range(0, n, bs):
+        yield slice(st, min(st + bs, n))
+
+
+def _pair_maps(out, sink, key, grid, volt, cur, cellmap, o):
+    """One pair's voltage and current maps (src/out.jl:90-112): `grid` scatters a node vector to cells;
+    `volt` / `cur` are None when not written.  Handed to `sink`, or kept in out.voltmaps / out.curmaps."""
+    if volt is not None:
+        vm = _process_grid(grid(volt), cellmap, False, o.set_null_voltages_to_nodata)
+        if sink is not None:
+            sink.voltmap(key, vm)
+        else:
+            out.voltmaps[key] = vm
+    if cur is not None:
+        cm = _process_grid(grid(cur), cellmap, o.log_transform_maps, o.set_null_currents_to_nodata)
+        if sink is not None:
+            sink.curmap(key, cm)
+        else:
+            out.curmaps[key] = cm
+
+
+def _add_current_maps(out, cum, mx, nodemap, npost, cellmap, o):
+    """Add the per-node cumulative and max currents of `npost` pairs, scattered by `nodemap`, into
+    out.cum_curmap / out.max_curmap.  Each pair's map holds 0 on cells that are no node of `nodemap`, which
+    the log transform makes NODATA, and NODATA on NODATA cells under set_null_currents_to_nodata: so those
+    cells get NODATA * npost in the sum and NODATA in the max."""
+    cmap = _scatter(np.asarray(cum, dtype=np.float64), nodemap)
+    off = nodemap == 0
+    if o.log_transform_maps:
+        cmap = np.where(off, NODATA * npost, cmap)
+    if o.set_null_currents_to_nodata:
+        cmap = np.where(cellmap == 0, NODATA * npost, cmap)
+    out.cum_curmap += cmap
+    if out.max_curmap is not None:
+        mmap = _scatter(np.asarray(mx, dtype=np.float64), nodemap)
+        mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, mmap)
+        if o.set_null_currents_to_nodata:
+            mmap = np.where(cellmap == 0, NODATA, mmap)
+        out.max_curmap = np.maximum(out.max_curmap, mmap)
+
+
+def _finish_pairwise(out, R, ids):
+    """R = 0 on the diagonal, framed by the point ids (src/core.jl:294-299), and the NODATA clamp of the
+    cumulative and max maps (src/utils.jl:114-120)."""
+    P = len(ids)
+    np.fill_diagonal(R, 0.0)
+    full = np.zeros((P + 1, P + 1))
+    full[0, 1:] = ids
+    full[1:, 0] = ids
+    full[1:, 1:] = R
+    out.resistances = full
+    if out.cum_curmap is not None:
+        out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
+    if out.max_curmap is not None:
+        out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
+    return out
+
+
+def _probe_solve(factor, src, dst, focal_rows, focal_col):
+    """Shortcut mode: only the voltages at the focal nodes are used (update_voltmatrix!, src/core.jl:685-703),
+    so the pairs are solved with probe rows instead of bringing n x k voltages back; R read off the probe."""
+    res = factor.solve_sources([([s_, d_], [-1.0, 1.0]) for s_, d_ in zip(src, dst)], ref=src, probe=focal_rows)
+    res["R"] = np.array([res["probe_volt"][c, focal_col[int(d_)]] for c, d_ in enumerate(dst)])
+    return res
+
+
+def _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res, log_transform=False):
+    """The whole-raster handle (S.construct_raster_factor), checked to number its nodes as the host's `nodemap`."""
+    factor, dev_nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                                    avg_res=avg_res, log_transform=log_transform)
+    if not np.array_equal(np.asarray(dev_nodemap), nodemap):
+        factor.close()
+        raise RuntimeError("device node map differs from the host's")
+    return factor
+
+
+def _component_labels(adj):
+    """(ncomp, label per node) of a construct_graph adjacency, a stored zero being no edge; drops those zeros
+    from `adj`."""
+    from scipy.sparse import csgraph
+    adj.eliminate_zeros()
+    return csgraph.connected_components(adj, directed=False)
+
+
 # ---------------------------------------------------------------------------
 # pairwise driver
 # ---------------------------------------------------------------------------
@@ -189,8 +282,7 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
     o = flags.outputflags
     P = len(prob.points)
     R = -np.ones((P, P))
-    want_maps = o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
-    shortcut = flags.is_raster and not want_maps and not prob.exclude_pairs      # src/core.jl:356-364
+    shortcut = flags.is_raster and not _any_map(o) and not prob.exclude_pairs    # src/core.jl:356-364
     voltmatrix = np.zeros((P, P))
     shortcut_res = -np.ones((P, P))
     out = PairwiseOutput(resistances=None)
@@ -236,7 +328,6 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
         # only raster maps are log-transformed (src/out.jl:96 process_grid!); the network branch of
         # write_cur_maps accumulates raw node currents (src/out.jl:48-88)
         with S.construct_cholesky_factor(matrix, solver, log_transform=bool(o.log_transform_maps and raster)) as factor:
-            bs = max(1, int(solver.bs))
             if device_branch:
                 lo, hi = _branch_index(factor, matrix)
                 bpos = branch_pos.positions(comp[lo], comp[hi])
@@ -254,15 +345,9 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                         nodes, inv[:len(src)], inv[len(src):], weight, want_volt=per_pair_volt,
                         want_curr=per_pair_curr, accumulate=need_curr)
                     return
-                for st in range(0, len(solves), bs):                            # src/core.jl:448-452
-                    sl = slice(st, min(st + bs, len(solves)))
+                for sl in _panels(len(solves), solver):
                     if shortcut:
-                        # only the voltages at the focal nodes are used (update_voltmatrix!,
-                        # src/core.jl:685-703): probe rows instead of n x k voltages over PCIe
-                        res = factor.solve_sources([([s_, d_], [-1.0, 1.0]) for s_, d_ in zip(src[sl], dst[sl])],
-                                                   ref=src[sl], probe=focal_rows)
-                        res["R"] = np.array([res["probe_volt"][c, focal_col[d_]] for c, d_ in enumerate(dst[sl])])
-                        yield sl, res
+                        yield sl, _probe_solve(factor, src[sl], dst[sl], focal_rows, focal_col)
                         continue
                     yield sl, factor.solve_pairs(src[sl], dst[sl], weight[sl], want_volt=per_pair_volt,
                                                  want_curr=per_pair_curr, accumulate=need_curr,
@@ -289,20 +374,7 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
                                 voltmatrix[i, cj] = 1.0 - float(pv[focal_col[int(local_of[points[i]])]]) / r
                             continue
                         if raster:
-                            if o.write_volt_maps:
-                                vm = _process_grid(_scatter(v, local_nodemap), prob.cellmap,
-                                                   False, o.set_null_voltages_to_nodata)
-                                if sink is not None:
-                                    sink.voltmap(key, vm)
-                                else:
-                                    out.voltmaps[key] = vm
-                            if per_pair_curr:
-                                cm = _process_grid(_scatter(cur, local_nodemap), prob.cellmap,
-                                                   o.log_transform_maps, o.set_null_currents_to_nodata)
-                                if sink is not None:
-                                    sink.curmap(key, cm)
-                                else:
-                                    out.curmaps[key] = cm
+                            _pair_maps(out, sink, key, lambda x: _scatter(x, local_nodemap), v, cur, prob.cellmap, o)
                         else:
                             # every id combination is post-processed on its own (src/core.jl:235-249):
                             # its branch currents go into the cumulative vector once each (on the device:
@@ -319,21 +391,7 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
             if need_curr:
                 cum, mx = factor.read_currents(want_max=True)
                 if raster:
-                    npost = float(weight.sum())
-                    cmap = _scatter(cum.astype(np.float64), local_nodemap)
-                    if o.log_transform_maps:
-                        # cells outside the component hold 0 -> log-transformed to NODATA per pair
-                        cmap = np.where(local_nodemap == 0, NODATA * npost, cmap)
-                    if o.set_null_currents_to_nodata:
-                        cmap = np.where(prob.cellmap == 0, NODATA * npost, cmap)
-                    out.cum_curmap += cmap
-                    if out.max_curmap is not None:
-                        mmap = _scatter(mx.astype(np.float64), local_nodemap)
-                        off = local_nodemap == 0
-                        mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, mmap)
-                        if o.set_null_currents_to_nodata:
-                            mmap = np.where(prob.cellmap == 0, NODATA, mmap)
-                        out.max_curmap = np.maximum(out.max_curmap, mmap)
+                    _add_current_maps(out, cum, mx, local_nodemap, float(weight.sum()), prob.cellmap, o)
                 else:
                     out.cum_node[rows] += cum
                     if device_branch:
@@ -341,29 +399,22 @@ def solve(prob: GraphProblem, solver: S.CUDASolver, flags: Flags, cfg=None, log=
         if shortcut:
             anchor = int(np.nonzero(points == csub[0])[0][0])
             _update_shortcut_resistances(anchor, voltmatrix, shortcut_res, R, points, comp)
-    if shortcut:
-        R = shortcut_res
-    np.fill_diagonal(R, 0.0)
-    full = np.zeros((P + 1, P + 1))
-    full[0, 1:] = ids
-    full[1:, 0] = ids
-    full[1:, 1:] = R
-    out.resistances = full                                                      # src/core.jl:294-299
-    if raster:
-        out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)   # src/utils.jl:114-120
-        if out.max_curmap is not None:
-            out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
-    return out
+    return _finish_pairwise(out, shortcut_res if shortcut else R, ids)
+
+
+def _upper_branches(matrix):
+    """(row, col, value) of the stored upper triangle of `matrix` in the order `_convert_to_3col` walks the CSC
+    branch matrix (column-major: sorted by column, then row), so written files match the reference's."""
+    coo = sp.triu(sp.csr_matrix(matrix), k=1).tocoo()
+    order = np.lexsort((coo.row, coo.col))
+    return coo.row[order], coo.col[order], coo.data[order]
 
 
 def _branch_currents(matrix, v, comp):
     """Network mode branch currents |G_ij| |v_i - v_j| over the stored upper triangle
     with the 1e-8 relative zeroing (src/out.jl:154-158, 250-290); host side, network
-    graphs only.  Rows come in the order `_convert_to_3col` walks the CSC branch matrix
-    (column-major: sorted by column, then row), so written files match the reference's."""
-    coo = sp.triu(sp.csr_matrix(matrix), k=1).tocoo()
-    order = np.lexsort((coo.row, coo.col))
-    row, col, data = coo.row[order], coo.col[order], coo.data[order]
+    graphs only, in the order of _upper_branches."""
+    row, col, data = _upper_branches(matrix)
     b = np.abs(data) * (v[row] - v[col])
     if len(b):
         mx = b.max()
@@ -413,12 +464,11 @@ class _BranchIndex:
 
 
 def _branch_index(factor, matrix):
-    """The handle's branches (0-based lo, hi), checked against the order _branch_currents writes them in:
-    sp.triu(matrix, 1) sorted by column, then row."""
+    """The handle's branches (0-based lo, hi), checked against the order _branch_currents writes them in
+    (_upper_branches)."""
     lo, hi = factor.branch_index()
-    coo = sp.triu(sp.csr_matrix(matrix), k=1).tocoo()
-    order = np.lexsort((coo.row, coo.col))
-    if not (np.array_equal(lo, coo.row[order]) and np.array_equal(hi, coo.col[order])):
+    row, col, _ = _upper_branches(matrix)
+    if not (np.array_equal(lo, row) and np.array_equal(hi, col)):
         raise RuntimeError("the device's branch order differs from the upper triangle's column-major order")
     return lo, hi
 
@@ -859,8 +909,7 @@ def _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, fo
     construct_local_node_map numbers cells unlike the node map (a NODATA cell of a merged polygon) bring their
     currents back and are scattered by their own map on the host.  Returns what `solve` returns."""
     o = flags.outputflags
-    want_maps = o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
-    shortcut = not want_maps and not exclude                                     # src/core.jl:356-364
+    shortcut = not _any_map(o) and not exclude                                   # src/core.jl:356-364
     need_curr = not shortcut
     per_pair_curr = need_curr and o.write_cur_maps and not o.write_cum_cur_map_only
     superpose = getattr(solver, "superpose", False) and not shortcut
@@ -901,7 +950,6 @@ def _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, fo
             factor.reset_currents()
         focal_rows = np.unique(points[focal] - 1)
         focal_col = {int(r): i for i, r in enumerate(focal_rows)}
-        bs = max(1, int(solver.bs))
         host_cum = {ci: (np.zeros(len(rows)), np.full(len(rows), NODATA), 0.0) for ci, (rows, _) in own.items()}
         masks = {}
 
@@ -909,15 +957,12 @@ def _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, fo
             """(columns, result) per device call: the own-map columns apart, with accumulate=False"""
             for acc in (True, False):
                 sel = [c for c in columns if (c[0] in own) != acc]
-                for st in range(0, len(sel), bs):
-                    chunk = sel[st:st + bs]
+                for sl in _panels(len(sel), solver):
+                    chunk = sel[sl]
                     src = np.array([c[1] for c in chunk], dtype=np.int64)
                     dst = np.array([c[2] for c in chunk], dtype=np.int64)
                     if shortcut:
-                        # only the voltages at the focal nodes are used (src/core.jl:685-703)
-                        res = factor.solve_sources([([s_, d_], [-1.0, 1.0]) for s_, d_ in zip(src, dst)], ref=src,
-                                                   probe=focal_rows)
-                        res["R"] = np.array([res["probe_volt"][c, focal_col[int(d_)]] for c, d_ in enumerate(dst)])
+                        res = _probe_solve(factor, src, dst, focal_rows, focal_col)
                     else:
                         res = factor.solve_pairs(src, dst, np.array([len(c[3]) for c in chunk], dtype=np.float64),
                                                  want_volt=o.write_volt_maps, want_curr=per_pair_curr or not acc,
@@ -964,65 +1009,24 @@ def _raster_pairs_device(cellmap, polymap, points_rc, exclude, flags, solver, fo
                         for i in inside[inside >= 1]:
                             voltmatrix[i, cj] = 1.0 - float(pv[focal_col[int(points[i]) - 1]]) / r
                         continue
-                    if o.write_volt_maps:
-                        vm = _process_grid(local(ci, res["volt"][:, col]), cellmap, False, o.set_null_voltages_to_nodata)
-                        if sink is not None:
-                            sink.voltmap(key, vm)
-                        else:
-                            out.voltmaps[key] = vm
-                    if per_pair_curr:
-                        cm = _process_grid(local(ci, cur), cellmap, o.log_transform_maps, o.set_null_currents_to_nodata)
-                        if sink is not None:
-                            sink.curmap(key, cm)
-                        else:
-                            out.curmaps[key] = cm
+                    _pair_maps(out, sink, key, lambda x: local(ci, x),
+                               res["volt"][:, col] if o.write_volt_maps else None,
+                               cur if per_pair_curr else None, cellmap, o)
         accumulated = [c for c in columns + [x for sc in super_comps for x in sc] if c[0] not in own]
         if need_curr and accumulated:
             # the device's cumulative / max vectors: a column adds f(0) (0, or -9999 under log) on every row of the
             # other components, which is what `solve` adds there per component; cells that are no node get the same
-            npost = float(sum(len(c[3]) for c in accumulated))
             cum, mx = factor.read_currents(want_max=True)
-            off = nodemap == 0
-            cmap = _scatter(cum.astype(np.float64), nodemap)
-            if o.log_transform_maps:
-                cmap = np.where(off, NODATA * npost, cmap)
-            if o.set_null_currents_to_nodata:
-                cmap = np.where(cellmap == 0, NODATA * npost, cmap)
-            out.cum_curmap += cmap
-            if out.max_curmap is not None:
-                mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, _scatter(mx.astype(np.float64), nodemap))
-                if o.set_null_currents_to_nodata:
-                    mmap = np.where(cellmap == 0, NODATA, mmap)
-                out.max_curmap = np.maximum(out.max_curmap, mmap)
+            _add_current_maps(out, cum, mx, nodemap, float(sum(len(c[3]) for c in accumulated)), cellmap, o)
     for ci, (cum, mx, npost) in host_cum.items():                      # as `solve` scatters one component
-        lm = own[ci][1]
-        cmap = _scatter(cum, lm)
-        if o.log_transform_maps:
-            cmap = np.where(lm == 0, NODATA * npost, cmap)
-        if o.set_null_currents_to_nodata:
-            cmap = np.where(cellmap == 0, NODATA * npost, cmap)
-        out.cum_curmap += cmap
-        if out.max_curmap is not None:
-            mmap = np.where(lm == 0, NODATA if o.log_transform_maps else 0.0, _scatter(mx, lm))
-            if o.set_null_currents_to_nodata:
-                mmap = np.where(cellmap == 0, NODATA, mmap)
-            out.max_curmap = np.maximum(out.max_curmap, mmap)
+        _add_current_maps(out, cum, mx, own[ci][1], npost, cellmap, o)
     if shortcut:
         for ci, cnodes in comps:
             csub = [int(points[k]) for k in focal[fcomp == ci]]
             _update_shortcut_resistances(int(np.nonzero(points == csub[0])[0][0]), voltmatrix, shortcut_res, R,
                                          points, cnodes)
         R = shortcut_res
-    np.fill_diagonal(R, 0.0)
-    full = np.zeros((P + 1, P + 1))
-    full[0, 1:] = ids
-    full[1:, 0] = ids
-    full[1:, 1:] = R
-    out.resistances = full                                                      # src/core.jl:294-299
-    out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)   # src/utils.jl:114-120
-    if out.max_curmap is not None:
-        out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
-    return out
+    return _finish_pairwise(out, R, ids)
 
 
 @dataclass
@@ -1111,14 +1115,11 @@ def plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of):
 def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink):
     """src/raster/pairwise.jl:72-135 on one whole-raster operator (see raster_pairwise)."""
     from . import graph
-    from scipy.sparse import csgraph
     o = flags.outputflags
-    want_maps = o.write_volt_maps or o.write_cur_maps or o.write_cum_cur_map_only or o.write_max_cur_maps
+    want_maps = _any_map(o)
     per_pair_curr = o.write_cur_maps and not o.write_cum_cur_map_only
     nodemap = graph.construct_node_map(cellmap, polymap)
-    adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
-    adj.eliminate_zeros()
-    _, comp_of = csgraph.connected_components(adj, directed=False)
+    _, comp_of = _component_labels(graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors))
     plan = plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of)
     pts = plan.ids
     P = len(pts)
@@ -1126,33 +1127,15 @@ def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, fou
     out = PairwiseOutput(resistances=None)
     out.cum_curmap = np.zeros(cellmap.shape)
     out.max_curmap = np.full(cellmap.shape, NODATA) if o.write_max_cur_maps else None
-
-    def emit(key, vm, cm):
-        if vm is not None:
-            if sink is not None:
-                sink.voltmap(key, vm)
-            else:
-                out.voltmaps[key] = vm
-        if cm is not None:
-            if sink is not None:
-                sink.curmap(key, cm)
-            else:
-                out.curmaps[key] = cm
-
     if plan.batched:
-        factor, dev_nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
-                                                        avg_res=avg_res, log_transform=o.log_transform_maps)
-        with factor:
-            if not np.array_equal(np.asarray(dev_nodemap), nodemap):
-                raise RuntimeError("device node map differs from the host's")
+        with _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res, o.log_transform_maps) as factor:
             used = sorted({pts[i] for i, _ in plan.batched} | {pts[j] for _, j in plan.batched})
             slot = {p: s for s, p in enumerate(used)}
             sets = [plan.sets[p] for p in used]
             if want_maps:
                 factor.reset_currents()
-            bs = max(1, int(solver.bs))
-            for st in range(0, len(plan.batched), bs):
-                chunk = plan.batched[st:st + bs]
+            for sl in _panels(len(plan.batched), solver):
+                chunk = plan.batched[sl]
                 res = factor.solve_region_pairs(sets, [slot[pts[i]] for i, _ in chunk],
                                                 [slot[pts[j]] for _, j in chunk], want_volt=o.write_volt_maps,
                                                 want_curr=per_pair_curr, accumulate=want_maps)
@@ -1161,31 +1144,13 @@ def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, fou
                 out.iterations += int(res["iters"].sum())
                 for col, (i, j) in enumerate(chunk):
                     R[i, j] = R[j, i] = float(res["R"][col])
-                    vm = cm = None
-                    if o.write_volt_maps:
-                        vm = _process_grid(_scatter(res["volt"][:, col].astype(np.float64), nodemap), cellmap,
-                                           False, o.set_null_voltages_to_nodata)
-                    if per_pair_curr:
-                        cm = _process_grid(_scatter(res["curr"][:, col].astype(np.float64), nodemap), cellmap,
-                                           o.log_transform_maps, o.set_null_currents_to_nodata)
-                    emit((pts[i], pts[j]), vm, cm)
+                    _pair_maps(out, sink, (pts[i], pts[j]), lambda x: _scatter(x.astype(np.float64), nodemap),
+                               res["volt"][:, col] if o.write_volt_maps else None,
+                               res["curr"][:, col] if per_pair_curr else None, cellmap, o)
             if want_maps:
-                # the per-node accumulation of every batched pair, as core.solve scatters it (cells that are
-                # no node hold 0 in each pair's map: NODATA once log-transformed)
-                npost = float(len(plan.batched))
+                # the per-node accumulation of every batched pair, as core.solve scatters it
                 cum, mx = factor.read_currents(want_max=True)
-                cmap = _scatter(cum.astype(np.float64), nodemap)
-                off = nodemap == 0
-                if o.log_transform_maps:
-                    cmap = np.where(off, NODATA * npost, cmap)
-                if o.set_null_currents_to_nodata:
-                    cmap = np.where(cellmap == 0, NODATA * npost, cmap)
-                out.cum_curmap += cmap
-                if out.max_curmap is not None:
-                    mmap = np.where(off, NODATA if o.log_transform_maps else 0.0, _scatter(mx.astype(np.float64), nodemap))
-                    if o.set_null_currents_to_nodata:
-                        mmap = np.where(cellmap == 0, NODATA, mmap)
-                    out.max_curmap = np.maximum(out.max_curmap, mmap)
+                _add_current_maps(out, cum, mx, nodemap, float(len(plan.batched)), cellmap, o)
     rr, cc_, ids = points_rc
     for i, j in plan.per_pair:                                   # the reference's own algorithm
         p1, p2 = pts[i], pts[j]
@@ -1205,19 +1170,10 @@ def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, fou
         out.cum_curmap += r.cum_curmap
         if out.max_curmap is not None:
             out.max_curmap = np.maximum(out.max_curmap, r.max_curmap)
-    np.fill_diagonal(R, 0.0)
-    full = np.zeros((P + 1, P + 1))
-    full[0, 1:] = pts
-    full[1:, 0] = pts
-    full[1:, 1:] = R
-    out.resistances = full
     # every pair's map goes into one shared cumulative map, clamped once when it is written
-    # (write_cum_maps -> postprocess_cum_curmap!, src/out.jl:467-479, src/utils.jl:114-120): a cell that
-    # is NODATA in every pair's map stays NODATA instead of adding up to -9999 * pairs
-    out.cum_curmap = np.where(out.cum_curmap < NODATA, NODATA, out.cum_curmap)
-    if out.max_curmap is not None:
-        out.max_curmap = np.where(out.max_curmap < NODATA, NODATA, out.max_curmap)
-    return out
+    # (write_cum_maps -> postprocess_cum_curmap!, src/out.jl:467-479): a cell that is NODATA in every pair's
+    # map stays NODATA instead of adding up to -9999 * pairs
+    return _finish_pairwise(out, R, pts)
 
 
 def _one_to_all_batched_raster(G, comps, nodemap, newpoly, point_map, unique_point_map, uniq, rr, cc_,
@@ -1484,19 +1440,14 @@ def _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solv
     want_v = o.write_volt_maps
     want_c = o.write_cur_maps or o.write_cum_cur_map_only
     served = {}
-    factor, dev_nodemap = S.construct_raster_factor(gmap, newpoly, solver, four_neighbors=four_neighbors,
-                                                    avg_res=avg_res, log_transform=False)
     iters = 0
-    with factor:
-        if not np.array_equal(np.asarray(dev_nodemap), nodemap):
-            raise RuntimeError("device node map differs from the host's")
+    with _raster_factor(gmap, newpoly, nodemap, solver, four_neighbors, avg_res) as factor:
         factor.reset_currents()
         singular = lambda c: (not one_to_all) and len(c.ground) == 1
-        bs = max(1, int(solver.bs))
         for kind in (False, True):
             cols = [c for c in plan.columns if singular(c) == kind]
-            for st in range(0, len(cols), bs):
-                chunk = cols[st:st + bs]
+            for sl in _panels(len(cols), solver):
+                chunk = cols[sl]
                 if kind:
                     res = factor.solve_sources(
                         [(np.r_[c.rows, c.ground], np.r_[c.vals, -c.vals.sum()]) for c in chunk],
@@ -1595,10 +1546,7 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
     adj = graph.construct_graph(gmap, nodemap, avg_res, four_neighbors)
     device, plan = {}, None
     if getattr(solver, "onetoall_raster", False):       # precedence over batch_one_to_all / batch_all_to_one
-        from scipy.sparse import csgraph
-        a = adj.copy()
-        a.eliminate_zeros()
-        comp_of = csgraph.connected_components(a, directed=False)[1]
+        comp_of = _component_labels(adj.copy())[1]
         plan = plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths, inc)
         if plan.columns:
             device = dict(zip(("served", "cum", "max", "iters"),
@@ -1626,6 +1574,17 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
         batched1 = _one_to_all_batched_raster(G, comps, nodemap, newpoly, point_map, unique_point_map, uniq,
                                               rr, cc_, strengths, solver)
     resident_factors = {}          # CUDASolver(resident_grounds=True): one device factor per component
+
+    def record(n, outvolt, outcurr):
+        """iteration n's voltage and current rasters into the output maps"""
+        if o.write_volt_maps:
+            out.voltmaps[n] = outvolt
+        if o.write_cur_maps or o.write_cum_cur_map_only:
+            out.curmaps[n] = outcurr
+        out.cum_curmap += outcurr
+        if out.max_curmap is not None:
+            out.max_curmap = np.maximum(out.max_curmap, outcurr)
+
     for i, n in enumerate(uniq):
         if plan is not None and i not in plan.reasons:              # served by the plan (_onetoall_output)
             continue
@@ -1647,25 +1606,13 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
             outvolt, outcurr, val = batched1[i]
             out.num_solves += 1
             res[i] = -1 if np.isclose(val, 0) else val               # advanced.jl:252-263
-            if o.write_volt_maps:
-                out.voltmaps[n] = outvolt
-            if o.write_cur_maps or o.write_cum_cur_map_only:
-                out.curmaps[n] = outcurr
-            out.cum_curmap += outcurr
-            if out.max_curmap is not None:
-                out.max_curmap = np.maximum(out.max_curmap, outcurr)
+            record(n, outvolt, outcurr)
             continue
         if i in batched:                                            # solved as a column of the batch
             outvolt, outcurr = batched[i]
             out.num_solves += 1
             res[i] = 0
-            if o.write_volt_maps:
-                out.voltmaps[n] = outvolt
-            if o.write_cur_maps or o.write_cum_cur_map_only:
-                out.curmaps[n] = outcurr
-            out.cum_curmap += outcurr
-            if out.max_curmap is not None:
-                out.max_curmap = np.maximum(out.max_curmap, outcurr)
+            record(n, outvolt, outcurr)
             continue
         if one_to_all:
             strv = strengths[i, 1] if strengths is not None else 1.0
@@ -1708,13 +1655,7 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
             res[i] = -1 if np.isclose(val[0], 0) else val[0]         # advanced.jl:252-263
         else:
             res[i] = 0
-        if o.write_volt_maps:
-            out.voltmaps[n] = outvolt
-        if o.write_cur_maps or o.write_cum_cur_map_only:
-            out.curmaps[n] = outcurr
-        out.cum_curmap += outcurr
-        if out.max_curmap is not None:
-            out.max_curmap = np.maximum(out.max_curmap, outcurr)
+        record(n, outvolt, outcurr)
     for f in resident_factors.values():
         f.close()
     if plan is not None:
@@ -1738,15 +1679,13 @@ def raster_advanced(data: RasterData, flags: Flags, cfg, solver=None, four_neigh
     cfg's remove_src_or_gnd.  Returns AdvancedOutput: voltmap (the column voltages scattered by the node
     map), curmap (the node currents summed over the columns, no log transform or nodata), voltages per node,
     and result: the voltage raster, or the 1 x 1 [-1] when no component was solved (advanced.jl:246-249)."""
-    from scipy.sparse import csgraph
     from . import graph
     solver = solver or get_solver(cfg)
     cellmap, polymap = data.cellmap, data.polymap
     nodemap = graph.construct_node_map(cellmap, polymap)
     adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
     n = adj.shape[0]
-    adj.eliminate_zeros()
-    ncomp, comp_of = csgraph.connected_components(adj, directed=False)
+    ncomp, comp_of = _component_labels(adj)
     s, g, f = sources_and_grounds_from_maps(np.asarray(data.source_map, dtype=np.float64),
                                             np.asarray(data.ground_map, dtype=np.float64), nodemap, n,
                                             cfg.get("remove_src_or_gnd", "keepall"))
@@ -1771,22 +1710,17 @@ def raster_advanced(data: RasterData, flags: Flags, cfg, solver=None, four_neigh
     out.stats = dict(setup_s=0.0, solve_s=0.0, columns=len(columns))
     if columns:
         t0 = time.perf_counter()
-        factor, dev_nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
-                                                        avg_res=avg_res, log_transform=False)
-        with factor:
-            if not np.array_equal(np.asarray(dev_nodemap), nodemap):
-                raise RuntimeError("device node map differs from the host's")
+        with _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res) as factor:
             if f[0] != NODATA:
                 factor.set_grounds(finite=f)
             t1 = time.perf_counter()
             factor.reset_currents()
-            bs = max(1, int(solver.bs))
             # columns whose local node map is the node map accumulate on the device; the others bring their
             # currents back to be scattered by their own map
             for own_map in (False, True):
                 cols = [c for c in columns if (c[4] is not None) == own_map]
-                for st in range(0, len(cols), bs):
-                    chunk = cols[st:st + bs]
+                for sl in _panels(len(cols), solver):
+                    chunk = cols[sl]
                     sets, gset = [], []
                     for c in chunk:                                   # -1: finite grounds only
                         gset.append(len(sets) if len(c[1]) else -1)

@@ -88,6 +88,18 @@ def _csr(ragged, dtype):
     return ptr, np.ascontiguousarray(vals, dtype=dtype)
 
 
+def _grounded_columns(sets, gset, sources):
+    """Columns with Dirichlet sets and sparse sources as the C entries take them: sets as CSR (ptr, rows),
+    gset (k,) int64, sources[c] = (rows, values) as CSR (sptr, srows, svals)."""
+    ptr, rows = _csr(sets, np.int64)
+    gset = np.ascontiguousarray(gset, dtype=np.int64)
+    assert len(sources) == len(gset)
+    sptr, srows = _csr([r for r, _ in sources], np.int64)
+    _, svals = _csr([v for _, v in sources], np.float64)
+    assert len(srows) == len(svals) == sptr[-1]
+    return ptr, rows, gset, sptr, srows, svals
+
+
 class SolverResidualError(RuntimeError):
     """The reference's `error("... residual $r exceeds tolerance 1e-4 ...")`
     (src/core.jl:641,650)."""
@@ -97,15 +109,11 @@ class B200Factor:
     """Opaque factor: CSR + preconditioner resident on one GPU (cs_b200_create)."""
 
     def __init__(self, matrix, solver: CUDASolver, log_transform=False):
-        lib = _lib.load()
-        self._lib = lib
-        self._h = C.c_void_p()
+        self._bind(solver)
+        lib = self._lib
         m = sp.csr_matrix(matrix)
         m.sort_indices()
         self.n = m.shape[0]
-        self.io_dtype = np.dtype(solver.dtype)
-        self.dtype = np.dtype(solver.device_dtype)
-        self.solver = solver
         vals = np.ascontiguousarray(m.data, dtype=self.dtype)
         rowptr = np.ascontiguousarray(m.indptr)
         colidx = np.ascontiguousarray(m.indices)
@@ -117,6 +125,15 @@ class B200Factor:
                                 bits, 0, _lib.dtype_code(self.dtype), solver.device,
                                 C.byref(opts), C.byref(self._h))
         _lib.check(lib, None, rc)
+
+    def _bind(self, solver):
+        """The attributes every factor carries before its handle is created: the library, an empty handle, the
+        caller's (io_dtype) and the device's (dtype) element types, the solver."""
+        self._lib = _lib.load()
+        self._h = C.c_void_p()
+        self.io_dtype = np.dtype(solver.dtype)
+        self.dtype = np.dtype(solver.device_dtype)
+        self.solver = solver
 
     @staticmethod
     def _opts(solver, log_transform=False):
@@ -139,13 +156,9 @@ class B200Factor:
         (cs_b200_create_from_raster_poly: construct_node_map with a polygon map, construct_graph with
         summed parallel adjacencies, laplacian!).  Returns (factor, nodemap) -- nodemap as the reference's
         (1-based node id per cell, 0 = none).  NODATA cells may be given as 0 or negative values."""
-        lib = _lib.load()
         f = cls.__new__(cls)
-        f._lib = lib
-        f._h = C.c_void_p()
-        f.io_dtype = np.dtype(solver.dtype)
-        f.dtype = np.dtype(solver.device_dtype)
-        f.solver = solver
+        f._bind(solver)
+        lib = f._lib
         g = np.asfortranarray(conductance, dtype=f.dtype)
         pm = None if polymap is None else np.asfortranarray(polymap, dtype=np.int32)
         nodemap = np.zeros(g.shape, dtype=np.int32, order="F")
@@ -167,13 +180,9 @@ class B200Factor:
         laplacian! (src/raster/pairwise.jl:271-367, src/core.jl:608-624).  `conductance`:
         2-D array, cells <= 0 / NODATA are not nodes; rows of the factor are the reference's
         node numbers minus one (column-major over the valid cells)."""
-        lib = _lib.load()
         f = cls.__new__(cls)
-        f._lib = lib
-        f._h = C.c_void_p()
-        f.io_dtype = np.dtype(solver.dtype)
-        f.dtype = np.dtype(solver.device_dtype)
-        f.solver = solver
+        f._bind(solver)
+        lib = f._lib
         g = np.asfortranarray(conductance, dtype=f.dtype)       # Julia's memory order
         n, nnz = C.c_int64(), C.c_int64()
         opts = cls._opts(solver, log_transform)
@@ -471,13 +480,8 @@ class B200Factor:
         on the column's ground set).  sets: list of 0-based row arrays (sorted, unique, non-empty).
         Returns dict with src_volt (v at each column's first source row), volt, curr (every ground row is
         a node of its own), iters, relres."""
-        ptr, rows = _csr(sets, np.int64)
-        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        ptr, rows, gset, sptr, srows, svals = _grounded_columns(sets, gset, sources)
         k = len(gset)
-        assert len(sources) == k
-        sptr, srows = _csr([r for r, _ in sources], np.int64)
-        _, svals = _csr([v for _, v in sources], np.float64)
-        assert len(srows) == len(svals) == sptr[-1]
         sv = np.zeros(k, dtype=self.dtype)
         volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
         rc = self._lib.cs_b200_solve_grounded(
@@ -495,13 +499,8 @@ class B200Factor:
         grounds, which needs finite grounds on the handle) and injects sources[c] = (rows, values) (0-based
         rows, none on the column's ground set).  The node currents include the finite-ground currents.
         Returns dict with volt, curr, iters, relres."""
-        ptr, rows = _csr(sets, np.int64)
-        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        ptr, rows, gset, sptr, srows, svals = _grounded_columns(sets, gset, sources)
         k = len(gset)
-        assert len(sources) == k
-        sptr, srows = _csr([r for r, _ in sources], np.int64)
-        _, svals = _csr([v for _, v in sources], np.float64)
-        assert len(srows) == len(svals) == sptr[-1]
         volt, curr, iters, relres = self._columns(k, want_volt, want_curr)
         rc = self._lib.cs_b200_solve_advanced(
             self._h, len(sets), _lib._ptr(ptr), _lib._ptr(rows), k, _lib._ptr(gset), _lib._ptr(sptr),
@@ -517,13 +516,8 @@ class B200Factor:
         component holds each row, or -1.  The columns' voltages are summed on the rows they own; returns dict
         with volt (n,), curr (n,) (node currents with the finite-ground currents) and branch (nb,) of that one
         vector under one 1e-8 cut over the graph (each None unless wanted), iters, relres."""
-        ptr, rows = _csr(sets, np.int64)
-        gset = np.ascontiguousarray(gset, dtype=np.int64)
+        ptr, rows, gset, sptr, srows, svals = _grounded_columns(sets, gset, sources)
         k = len(gset)
-        assert len(sources) == k
-        sptr, srows = _csr([r for r, _ in sources], np.int64)
-        _, svals = _csr([v for _, v in sources], np.float64)
-        assert len(srows) == len(svals) == sptr[-1]
         owner = np.ascontiguousarray(owner, dtype=np.int64)
         assert len(owner) == self.n
         vec = lambda want, m: np.empty(m, dtype=self.dtype) if want else None
