@@ -116,6 +116,7 @@ _PROTOS = {
     "cs_b200_stream": (C.c_int, [_H, C.POINTER(C.c_void_p)]),
     "cs_b200_profile_spmm": (C.c_int, [_H, C.c_int, C.POINTER(C.c_double), C.POINTER(C.c_int64)]),
     "cs_b200_profile_classes": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cs_b200_profile_classes_n": (C.c_int, [_H, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_b200_profile_bytes": (C.c_int, [_H, C.POINTER(C.c_double)]),
     "cs_b200_comm_unique_id": (C.c_int, [C.c_void_p]),
     "cs_b200_comm_init": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_void_p, C.POINTER(_H)]),

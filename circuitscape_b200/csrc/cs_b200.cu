@@ -30,8 +30,9 @@ namespace {
 
 thread_local std::string g_create_error;
 
-constexpr int PROF_CLASSES = 18;   // cs_b200_profile_classes: 9 kernel classes x (fp64, fp32)
+constexpr int PROF_CLASSES = 20;   // cs_b200_profile_classes_n: 10 kernel classes x (fp64, fp32)
 constexpr int PROF_CGF = 8;        // class of the fused CG step (after the 8 SpMM epilogues)
+constexpr int PROF_RSW = 9;        // class of the fused residual update + level-0 residual sweep
 
 struct GraphSlot {
   cudaGraphExec_t exec = nullptr;
@@ -97,6 +98,7 @@ struct cs_b200_handle {
   void *X = nullptr, *R = nullptr, *P = nullptr, *AP = nullptr, *B = nullptr, *stage = nullptr;
   void* Z = nullptr;                 // AMG: z = M^-1 r
   void* P2 = nullptr;                // fused CG step (k_stencil_cg): p of even iterations; P holds the odd ones
+  void* R2 = nullptr;                // fused residual sweep (k_stencil_res_update): r of odd iterations; R the even ones
   DevCsr A0;                         // view of the finest operator (aliases d_rowptr/...)
   std::vector<DevLevel> lv;          // lv[0] = finest (A aliases A0), lv.back() = coarsest
   double* d_pinv = nullptr;          // dense pseudo-inverse of the coarsest operator
@@ -159,7 +161,7 @@ struct cs_b200_handle {
   double prof_bytes = 0.0;   // algorithmic bytes of the timed launches (DESIGN.md §4 formula)
   int64_t prof_launches = 0;
   // the same per kernel class: slot = 2 * MODE + (fp32 ? 1 : 0), MODE 7 = fused prolongation + sweep,
-  // MODE 8 = fused CG step
+  // MODE 8 = fused CG step, MODE 9 = fused residual update + level-0 residual sweep
   std::vector<int> prof_slot;           // one entry per event pair in flight
   std::vector<double> prof_pair_bytes;
   double prof_slot_ms[PROF_CLASSES] = {}, prof_slot_bytes[PROF_CLASSES] = {};
@@ -541,6 +543,25 @@ inline bool full_stencil() {
   return on || !stencil_pipe();
 }
 
+// stencil-form levels keep the zero-guess Jacobi sweep implicit: x0 = omega D^-1 b is formed on the fly
+// by the residual kernel (SP_RES0) and by the fused upward kernel, never stored (CS_B200_NO_IMPLICIT_X0
+// switches back to the stored form for A/B runs)
+inline bool implicit_x0(const DevLevel& L) {
+  static const bool off = std::getenv("CS_B200_NO_IMPLICIT_X0") != nullptr || std::getenv("CS_B200_NO_FUSED_PROLONG") != nullptr;
+  return L.A.dia != nullptr && !off;
+}
+
+// The fused residual sweep (kernels.cuh k_stencil_res_update) forms r -= alpha A p, r32 and the level-0 residual
+// of the fp32 V-cycle in one pass, in place of k_cg_update_r0 and the level-0 SP_RES0 sweep.  It is written for
+// what the bench workload runs: an fp32 cycle (mixed) on a half-form stencil finest level, pipelined kernels,
+// implicit x0 (and, checked when R2 is allocated, fp32 level-0 diagonals that are the fp64 ones rounded).
+// CS_B200_NO_FUSED_RES keeps the two kernels for A/B runs.
+inline bool fused_res_form(const cs_b200_handle* h) {
+  static const bool off = std::getenv("CS_B200_NO_FUSED_RES") != nullptr;
+  return !off && h->mixed && stencil_pipe() && h->A0.dia && h->A0.dia_half && !h->lv32.empty() &&
+         h->lv32[0].A.dia_half && implicit_x0(h->lv32[0]);
+}
+
 // the kernels' view of a stencil-form operator
 template <typename T>
 DiaDev<T> dia_view(const DevCsr& m) {
@@ -805,6 +826,30 @@ int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::
       if (e == cudaSuccess) e = cudaMemsetAsync(h->P2, 0, pe, h->stream);
       if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (second p panel)", cudaGetErrorString(e));
     }
+    if (h->P2 && fused_res_form(h)) {
+      // the fused residual sweep rounds the fp64 diagonals to the fp32 level 0's on chip: it runs only where the
+      // stored fp32 runs are exactly those roundings.  R2: its second r panel
+      int* d_diff = nullptr;
+      int diff = 1;
+      cudaError_t e = cudaMalloc(&d_diff, sizeof(int));
+      if (e == cudaSuccess) e = cudaMemsetAsync(d_diff, 0, sizeof(int), h->stream);
+      if (e == cudaSuccess) {
+        k_dia_rounds<T, float><<<std::min<int64_t>((5 * h->n + 255) / 256, 4096), 256, 0, h->stream>>>(
+            dia_view<T>(h->A0), dia_view<float>(h->lv32[0].A), d_diff);
+        e = cudaMemcpyAsync(&diff, d_diff, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+      }
+      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+      cudaFree(d_diff);
+      if (e == cudaSuccess && diff == 0 && !h->R2) {
+        const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(T);
+        e = cudaMalloc(&h->R2, pe);
+        if (e == cudaSuccess) e = cudaMemsetAsync(h->R2, 0, pe, h->stream);
+      } else if (diff != 0) {
+        cudaFree(h->R2);
+        h->R2 = nullptr;
+      }
+      if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (second r panel)", cudaGetErrorString(e));
+    }
   } else {
     csb_dev::seed_discard(job);
   }
@@ -990,14 +1035,6 @@ int ew_grid_n(cs_b200_handle* h, int64_t n_pad) {
   return (int)std::max<size_t>(1, std::min<size_t>(h->grid_ew, (nelem + per - 1) / per));
 }
 
-// stencil-form levels keep the zero-guess Jacobi sweep implicit: x0 = omega D^-1 b is formed on the fly
-// by the residual kernel (SP_RES0) and by the fused upward kernel, never stored (CS_B200_NO_IMPLICIT_X0
-// switches back to the stored form for A/B runs)
-inline bool implicit_x0(const DevLevel& L) {
-  static const bool off = std::getenv("CS_B200_NO_IMPLICIT_X0") != nullptr || std::getenv("CS_B200_NO_FUSED_PROLONG") != nullptr;
-  return L.A.dia != nullptr && !off;
-}
-
 // T = B - A (omega D^-1 B) on a stencil-form level
 template <typename T, int KT>
 void launch_stencil_res0(cs_b200_handle* h, DevLevel& L, const T* B, T* Tout, bool timed) {
@@ -1078,10 +1115,13 @@ void launch_prolong_jacobi(cs_b200_handle* h, DevLevel& L, const T* Yc, const T*
 //   in : h->R (residual, read-only)      out: h->Z ; rho_new = r.z folded into the last kernel
 // Level buffers: b = right-hand side, x = running correction, t = residual scratch,
 // y = post-smoothed correction.  Finest level: b = R, x = stage, t = AP, y = Z.
+// level0_residual: t of the finest level is already formed (k_stencil_res_update); the cycle starts at the
+// restriction.
 struct VcBufs { void *b0, *x0, *t0, *y0; };   // finest-level panels of the cycle
 
 template <typename T, int KT>
-void launch_vcycle_on(cs_b200_handle* h, std::vector<DevLevel>& lv, const VcBufs& vb, bool level0_presmoothed) {
+void launch_vcycle_on(cs_b200_handle* h, std::vector<DevLevel>& lv, const VcBufs& vb, bool level0_presmoothed,
+                      bool level0_residual) {
   const int nl = (int)lv.size();
   auto B = [&](int l) { return l == 0 ? (T*)vb.b0 : (T*)lv[l].b; };
   auto X = [&](int l) { return l == 0 ? (T*)vb.x0 : (T*)lv[l].x; };
@@ -1091,7 +1131,7 @@ void launch_vcycle_on(cs_b200_handle* h, std::vector<DevLevel>& lv, const VcBufs
     DevLevel& L = lv[l];
     const size_t nelem = (size_t)L.n_pad * KT;
     if (implicit_x0(L)) {
-      launch_stencil_res0<T, KT>(h, L, B(l), Tm(l), l == 0);
+      if (!(l == 0 && level0_residual)) launch_stencil_res0<T, KT>(h, L, B(l), Tm(l), l == 0);
     } else {
       if (!(l == 0 && level0_presmoothed)) {
         k_jacobi0<T, KT><<<ew_grid_n<T, KT>(h, L.n_pad), NT, 0, h->stream>>>(
@@ -1137,13 +1177,13 @@ void launch_vcycle_on(cs_b200_handle* h, std::vector<DevLevel>& lv, const VcBufs
 
 // the cycle of this handle: fp32 copies when `mixed`, else the handle's own type
 template <typename T, int KT>
-void launch_vcycle(cs_b200_handle* h, bool level0_presmoothed) {
+void launch_vcycle(cs_b200_handle* h, bool level0_presmoothed, bool level0_residual = false) {
   if (h->mixed) {
     const VcBufs vb{h->R32, h->X32, h->T32, h->Z32};
-    launch_vcycle_on<float, KT>(h, h->lv32, vb, level0_presmoothed);
+    launch_vcycle_on<float, KT>(h, h->lv32, vb, level0_presmoothed, level0_residual);
   } else {
     const VcBufs vb{h->R, h->stage, h->AP, h->Z};
-    launch_vcycle_on<T, KT>(h, h->lv, vb, level0_presmoothed);
+    launch_vcycle_on<T, KT>(h, h->lv, vb, level0_presmoothed, level0_residual);
   }
 }
 
@@ -1181,19 +1221,29 @@ inline bool fused_cg(const cs_b200_handle* h) {
   return h->amg && h->A0.dia && h->P2 && !off;
 }
 
-template <typename T, int KT, typename TV, bool HALF>
+// the iteration runs the fused residual sweep; region panels mask AP between the CG step and the residual
+// update, so they keep k_cg_update_r0
+inline bool fused_res(const cs_b200_handle* h) {
+  return fused_cg(h) && h->R2 && !h->rg_on && fused_res_form(h);
+}
+
+template <typename T, int KT, typename TV, bool HALF, bool STORE_AP>
 void launch_stencil_cg_pipe(cs_b200_handle* h, const DiaDev<T>& a, const TV* Z, int sg) {
   constexpr int SMEM = StPipeCg<T, KT, TV, HALF>::D::BYTES;
   static bool once[64] = {};
   bool& set = once[h->device & 63];
-  if (!set) { cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
-  k_stencil_cg_pipe<T, KT, TV, HALF><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP,
-                                                                  h->d_ctl, h->d_partials);
+  if (!set) {
+    cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV, HALF, STORE_AP>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    set = true;
+  }
+  k_stencil_cg_pipe<T, KT, TV, HALF, STORE_AP><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X,
+                                                                            (T*)h->AP, h->d_ctl, h->d_partials);
 }
 
-// the z panel the CG update reads: the fp32 cycle's output on mixed handles
+// the z panel the CG update reads: the fp32 cycle's output on mixed handles.  !store_ap (fused_res): A p is not
+// stored, the residual sweep forms it again.
 template <typename T, int KT, typename TV>
-void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
+void launch_stencil_cg(cs_b200_handle* h, const TV* Z, bool store_ap) {
   const DevCsr& m = h->A0;
   const DiaDev<T> a = dia_view<T>(m);
   constexpr int V16 = 16 / (int)sizeof(T);
@@ -1208,17 +1258,20 @@ void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
       for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
     e0 = h->prof_ev[h->prof_used++];
     e1 = h->prof_ev[h->prof_used++];
-    // 9 diagonals, Z and p_{it-1} in, AP and p_it out; X in + out and p_{it-2} in on every other step
+    // 9 diagonals, Z and p_{it-1} in, AP (store_ap) and p_it out; X in + out and p_{it-2} in on every other step
     const double pe = (double)m.nrows * KT * sizeof(T);
-    const double fb = (double)m.nrows * 9 * sizeof(T) + (double)m.nrows * KT * sizeof(TV) + 3.0 * pe + 1.5 * pe;
+    const double fb = (double)m.nrows * 9 * sizeof(T) + (double)m.nrows * KT * sizeof(TV) + (store_ap ? 3.0 : 2.0) * pe +
+                      1.5 * pe;
     h->prof_bytes += fb;
     h->prof_slot.push_back(2 * PROF_CGF + (sizeof(T) == 4 ? 1 : 0));
     h->prof_pair_bytes.push_back(fb);
     cudaEventRecord(e0, h->stream);
   }
   if (stencil_pipe()) {
-    if (a.half) launch_stencil_cg_pipe<T, KT, TV, true>(h, a, Z, sg);
-    else launch_stencil_cg_pipe<T, KT, TV, false>(h, a, Z, sg);
+    if (!store_ap) {   // fused_res: fp64 with an fp32 cycle, half form
+      if constexpr (sizeof(T) == 8 && sizeof(TV) == 4) launch_stencil_cg_pipe<T, KT, TV, true, false>(h, a, Z, sg);
+    } else if (a.half) launch_stencil_cg_pipe<T, KT, TV, true, true>(h, a, Z, sg);
+    else launch_stencil_cg_pipe<T, KT, TV, false, true>(h, a, Z, sg);
   } else {
     if (a.half) refuse_half("k_stencil_cg");
     k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
@@ -1229,14 +1282,58 @@ void launch_stencil_cg(cs_b200_handle* h, const TV* Z) {
   h->stats.spmm_launches++;
 }
 
+// r -= alpha A p, r32 = (float) r and the level-0 residual T32 of the fp32 cycle (kernels.cuh
+// k_stencil_res_update), in place of k_cg_update_r0 and the cycle's level-0 SP_RES0 sweep
+template <typename T, int KT>
+void launch_res_update(cs_b200_handle* h) {
+  const DevCsr& m = h->A0;
+  DevLevel& L = h->lv32[0];
+  using SH = RuShape<T, float, KT>;
+  constexpr int SMEM = SH::D::BYTES;
+  static bool once[64] = {};
+  bool& set = once[h->device & 63];
+  if (!set) {
+    cudaFuncSetAttribute(k_stencil_res_update<T, float, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
+    set = true;
+  }
+  // one resident wave, as launch_prolong_jacobi: long runs keep the halo columns rebuilt at their ends rare
+  int occ = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_stencil_res_update<T, float, KT>, NT, SMEM);
+  occ = std::max(1, occ);
+  const long long nsteps = (long long)((m.dia_nr + SH::RPS - 1) / SH::RPS) *
+                           (((long long)m.nrows + m.dia_nr - 1) / m.dia_nr);
+  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min(h->grid_spmm, h->num_sms * occ), nsteps));
+  cudaEvent_t e0 = nullptr, e1 = nullptr;
+  if (h->profile) {
+    if (h->prof_used + 2 > h->prof_ev.size())
+      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
+    e0 = h->prof_ev[h->prof_used++];
+    e1 = h->prof_ev[h->prof_used++];
+    // p, r in and r out (T), R32 and T32 out (float), the 5 upper diagonals (T), the float 1/diag
+    const double nr = (double)m.nrows;
+    const double fb = nr * KT * (3.0 * sizeof(T) + 2.0 * sizeof(float)) + nr * 5 * sizeof(T) + nr * sizeof(float);
+    h->prof_bytes += fb;
+    h->prof_slot.push_back(2 * PROF_RSW + (sizeof(T) == 4 ? 1 : 0));
+    h->prof_pair_bytes.push_back(fb);
+    cudaEventRecord(e0, h->stream);
+  }
+  k_stencil_res_update<T, float, KT><<<grid, NT, SMEM, h->stream>>>(
+      dia_view<T>(m), (const float*)L.dinv, (float)L.omega, (const T*)h->P2, (const T*)h->P,
+      (T*)h->R, (T*)h->R2, (float*)h->R32, (float*)h->T32, h->d_ctl);
+  if (h->profile) cudaEventRecord(e1, h->stream);
+  h->stats.kernel_launches++;
+  h->stats.spmm_launches++;
+}
+
 template <typename T, int KT>
 void launch_iteration(cs_b200_handle* h) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int g = ew_grid<T, KT>(h);
   const bool fused = fused_cg(h);
+  const bool fres = sizeof(T) == 8 && fused_res(h);   // mixed handles are fp64 ones
   if (fused) {
-    if (h->mixed) launch_stencil_cg<T, KT, float>(h, (const float*)h->Z32);
-    else launch_stencil_cg<T, KT, T>(h, (const T*)h->Z);
+    if (h->mixed) launch_stencil_cg<T, KT, float>(h, (const float*)h->Z32, !fres);
+    else launch_stencil_cg<T, KT, T>(h, (const T*)h->Z, true);
   } else {
     launch_spmm<T, KT, SP_CG>(h, (const T*)h->P, (T*)h->AP, nullptr);
   }
@@ -1253,11 +1350,16 @@ void launch_iteration(cs_b200_handle* h) {
     // x += alpha p together with p = z + beta p  (9 instead of 11 panel passes), which the fused
     // CG step of the next iteration does instead
     if (h->mixed) {
-      k_cg_update_r0<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
-                                                            (T)h->lv[0].omega, (T*)h->R,
-                                                            implicit_x0(h->lv32[0]) ? nullptr : (float*)h->X32,
-                                                            (float*)h->R32, h->d_ctl);
-      launch_vcycle<T, KT>(h, true);
+      if (fres) {
+        if constexpr (sizeof(T) == 8) launch_res_update<T, KT>(h);
+      } else {
+        k_cg_update_r0<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
+                                                              (T)h->lv[0].omega, (T*)h->R,
+                                                              implicit_x0(h->lv32[0]) ? nullptr : (float*)h->X32,
+                                                              (float*)h->R32, h->d_ctl);
+        h->stats.kernel_launches++;
+      }
+      launch_vcycle<T, KT>(h, true, fres);
       mask_z<T, KT>(h);
       if (!fused)
         k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
@@ -1267,12 +1369,13 @@ void launch_iteration(cs_b200_handle* h) {
                                                         (T)h->lv[0].omega, (T*)h->R,
                                                         implicit_x0(h->lv[0]) ? nullptr : (T*)h->stage, nullptr,
                                                         h->d_ctl);
+      h->stats.kernel_launches++;
       launch_vcycle<T, KT>(h, true);
       mask_z<T, KT>(h);
       if (!fused)
         k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
-    h->stats.kernel_launches += fused ? 1 : 2;
+    if (!fused) h->stats.kernel_launches++;
   }
 }
 
@@ -2746,7 +2849,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   cudaFree(h->d_vals0);
   cudaFree(h->d_fg);
   cudaFree(h->d_bptr); cudaFree(h->d_cum_branch); cudaFree(h->d_branch_stage);
-  void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->P, h->P2, h->AP, h->B, h->stage,
+  void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->R2, h->P, h->P2, h->AP, h->B, h->stage,
                   h->d_cum, h->d_max, h->d_ctl, h->d_partials, h->d_flush};
   for (void* b : bufs) if (b) cudaFree(b);
   if (h->h_ctl) cudaFreeHost(h->h_ctl);
@@ -2905,11 +3008,15 @@ int cs_b200_profile_spmm(cs_b200_handle* h, int enable, double* total_ms, int64_
 }
 
 int cs_b200_profile_classes(cs_b200_handle* h, double* ms18, double* bytes18, int64_t* launches18) {
-  if (!h) return CS_B200_ERR_ARG;
-  for (int i = 0; i < PROF_CLASSES; ++i) {
-    if (ms18) ms18[i] = h->prof_slot_ms[i];
-    if (bytes18) bytes18[i] = h->prof_slot_bytes[i];
-    if (launches18) launches18[i] = h->prof_slot_launches[i];
+  return cs_b200_profile_classes_n(h, 18, ms18, bytes18, launches18);
+}
+
+int cs_b200_profile_classes_n(cs_b200_handle* h, int nslots, double* ms, double* bytes, int64_t* launches) {
+  if (!h || nslots < 0) return CS_B200_ERR_ARG;
+  for (int i = 0; i < std::min(nslots, PROF_CLASSES); ++i) {
+    if (ms) ms[i] = h->prof_slot_ms[i];
+    if (bytes) bytes[i] = h->prof_slot_bytes[i];
+    if (launches) launches[i] = h->prof_slot_launches[i];
   }
   return CS_B200_OK;
 }

@@ -1240,11 +1240,12 @@ k_stencil_cg(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __r
 constexpr int ST_SMAX = 4;
 constexpr int st_a16(int b) { return (b + 15) & ~15; }
 
-template <int PANEL, int OWN, int MINB> struct StDepth {
-  static constexpr int BUDGET = 228 * 1024 / MINB - 1024 - 3 * 1024;   // less the per-CTA reserve, static buffers
+// EXTRA: dynamic shared memory the kernel keeps beside the two rings
+template <int PANEL, int OWN, int MINB, int EXTRA = 0> struct StDepth {
+  static constexpr int BUDGET = 228 * 1024 / MINB - 1024 - 3 * 1024 - EXTRA;   // less the per-CTA reserve, static buffers
   static constexpr int FIT = (BUDGET - 3 * PANEL - OWN) / (PANEL + OWN);
   static constexpr int S = FIT < 1 ? 1 : (FIT > ST_SMAX ? ST_SMAX : FIT);
-  static constexpr int BYTES = (S + 3) * PANEL + (S + 1) * OWN;
+  static constexpr int BYTES = (S + 3) * PANEL + (S + 1) * OWN + EXTRA;
 };
 
 template <int B>
@@ -1338,6 +1339,22 @@ struct StStep {
 template <typename T, int RPP>
 __device__ __forceinline__ T st_half_val(const T* const (&ds)[3], int s9, int rl) {
   return s9 < 4 ? ds[s9 / 3][(4 - s9) * (RPP + 2) + rl + s9 % 3] : ds[1][(s9 - 4) * (RPP + 2) + rl + 1];
+}
+
+// acc = the sum over the 9 slots, in slot order, of coef(s9) * val(s9): one row of a stencil product, the
+// accumulation every pipelined stencil kernel shares so that they form the same row bit for bit
+template <typename T, int CPT, class Val, class Coef>
+__device__ __forceinline__ void stencil_row(T (&acc)[CPT], Val&& val, Coef&& coef) {
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) acc[i] = T(0);
+#pragma unroll
+  for (int s9 = 0; s9 < 9; ++s9) {
+    T v[CPT];
+    val(s9, v);
+    const T a = coef(s9);
+#pragma unroll
+    for (int i = 0; i < CPT; ++i) acc[i] += a * v[i];
+  }
 }
 
 // issue(step, panel slot, own slot) fills the slots of a load step; compute(step, panel slot, own slot) runs on the
@@ -1531,7 +1548,7 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
 
 // k_stencil_cg, operands through the shared-memory pipeline: panel slot p_{it-1} and Z rows, own slot the diagonals
 // and, on odd iterations, the X and Pd (p_{it-2}) rows.  Without the register arrays of the gathers it runs at
-// CGP_MINB CTAs per SM.
+// CGP_MINB CTAs per SM.  !STORE_AP: Y is not written (k_stencil_res_update forms A p again from the stored p).
 constexpr int CGP_MINB = 3;
 
 template <typename T, int KT, typename TV, bool HALF> struct StPipeCg {
@@ -1547,7 +1564,7 @@ template <typename T, int KT, typename TV, bool HALF> struct StPipeCg {
   using D = StDepth<PANEL, OWN, CGP_MINB>;
 };
 
-template <typename T, int KT, typename TV, bool HALF>
+template <typename T, int KT, typename TV, bool HALF, bool STORE_AP>
 __global__ void __launch_bounds__(NT, CGP_MINB)
 k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T* __restrict__ X, T* __restrict__ Y,
                   PanelCtl* ctl, double* partials) {
@@ -1614,32 +1631,28 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
     const unsigned char* os = oring + so * SP::OWN;
     const T* dg = reinterpret_cast<const T*>(os);
     T acc[CPT], po[CPT], pc[CPT];
+    stencil_row<T, CPT>(
+        acc,
+        [&](int s9, T (&pv)[CPT]) {
+          TV zv[CPT];
+          ldvec<T, CPT>(ps[s9 / 3] + (rl + s9 % 3) * KT + c0, pv);
+          ldvec<TV, CPT>(zs[s9 / 3] + (rl + s9 % 3) * KT + c0, zv);
+          if (s9 == 4) {
 #pragma unroll
-    for (int i = 0; i < CPT; ++i) acc[i] = T(0);
+            for (int i = 0; i < CPT; ++i) po[i] = pv[i];
+          }
 #pragma unroll
-    for (int s9 = 0; s9 < 9; ++s9) {
-      T pv[CPT];
-      TV zv[CPT];
-      ldvec<T, CPT>(ps[s9 / 3] + (rl + s9 % 3) * KT + c0, pv);
-      ldvec<TV, CPT>(zs[s9 / 3] + (rl + s9 % 3) * KT + c0, zv);
-      if (s9 == 4) {
+          for (int i = 0; i < CPT; ++i) pv[i] = (T)zv[i] + be[i] * pv[i];
+          if (s9 == 4) {
 #pragma unroll
-        for (int i = 0; i < CPT; ++i) po[i] = pv[i];
-      }
-#pragma unroll
-      for (int i = 0; i < CPT; ++i) pv[i] = (T)zv[i] + be[i] * pv[i];
-      if (s9 == 4) {
-#pragma unroll
-        for (int i = 0; i < CPT; ++i) pc[i] = pv[i];
-      }
-      const T vs = HALF ? st_half_val<T, RPP>(ds, s9, rl) : dg[s9 * RPP + rl];
-#pragma unroll
-      for (int i = 0; i < CPT; ++i) acc[i] += vs * pv[i];
-    }
+            for (int i = 0; i < CPT; ++i) pc[i] = pv[i];
+          }
+        },
+        [&](int s9) { return HALF ? st_half_val<T, RPP>(ds, s9, rl) : dg[s9 * RPP + rl]; });
 #pragma unroll
     for (int i = 0; i < CPT; ++i) dot0[i] += (double)acc[i] * (double)pc[i];
     const size_t o = (size_t)row * KT + c0;
-    stvec<T, CPT>(Y + o, acc);
+    if (STORE_AP) stvec<T, CPT>(Y + o, acc);
     stvec<T, CPT>(Pd + o, pc);
     if (pair) {
       T xo[CPT], pd[CPT];
@@ -1667,6 +1680,225 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
       ctl->alpha[tid] = al;
       ctl->alpha_ring[it % 3][tid] = al;
     }
+  }
+}
+
+// ---------------------------------------------------------------------------
+// Residual update and finest-level residual sweep of the AMG-PCG iteration, fused, on a half-form stencil finest
+// level with an fp32 (TV) V-cycle, iteration it = ctl->iter, right after k_stencil_cg_pipe<..., false> (no A p):
+//   Ap  = A p_it                            (p_it: the panel the CG step wrote, Pb0 / Pb1 by it as there)
+//   r'  = r - alpha_it Ap ; r32 = (TV) r'   (k_cg_update_r0's expressions)
+//   T32 = r32 - A32 (omega D32^-1 r32)      (k_stencil_pipe<SP_RES0>'s expressions on the fp32 level 0)
+// A p is formed by stencil_row as the CG step forms it, so it is the same number, and neither A p nor r32 goes
+// through global memory.  r of even iterations lives in Rb0, of odd ones in Rb1: a strip reads the halo rows of r
+// that neighbouring strips rewrite, so the update cannot be in place.
+// Work split as k_stencil_prolong_jacobi: strips of RPS = RH - 2 rows, (strip, raster column) steps strip-major,
+// one contiguous run per CTA; thread (rr, g) takes row rr - 1 of the strip (rr = 0, RH - 1: the halo rows) and
+// column group g.  A run's segment [cb, ce) of one strip takes the load steps x = cb - 2 ... ce + 2 through the
+// cp.async rings of stencil_pipe (one barrier per step):
+//   panel slot (S + 3): p rows -2 ... RPS + 1 of column x and their 5 upper-slot runs (x <= ce + 1); the fp32
+//                       1/diag of rows -1 ... RPS of column x - 2 (x - 2 in [cb - 1, ce])
+//   own slot (S + 1):   r rows -1 ... RPS of column x - 1
+// and, once the slots of step x are in, computes A p, r', r32 of the RH rows of column x - 1 (x - 1 in [cb - 1, ce];
+// r32 and the fp32 rounding of the row's 5 upper-slot values into rings of 4 columns) and T32 of the strip rows of
+// column x - 3 (in [cb, ce)) out of the ring columns x - 4 ... x - 2, which the previous steps wrote.  The fp32
+// level-0 operator is the fp64 one rounded, so its diagonals are not read: launch_res_update runs the kernel only
+// where the stored fp32 runs equal the rounded fp64 ones bit for bit (k_dia_rounds).  Halo rows and columns are recomputed bit for bit by the
+// owner; only the owner stores r', R32 and T32.
+// ---------------------------------------------------------------------------
+constexpr int RU_MINB = 3;
+constexpr int RU_RING = 4;   // r32 columns: x - 4 ... x - 2 read, x - 1 written
+
+template <typename T, typename TV, int KT> struct RuShape {
+  static constexpr int V16 = 16 / (int)sizeof(T);
+  static constexpr int CPT = KT < V16 ? KT : V16;
+  static constexpr int CG = KT / CPT;
+  static constexpr int RH = NT / CG;
+  static constexpr int RPS = RH - 2;
+  static constexpr int PDG = st_a16((RH + 2) * KT * (int)sizeof(T));
+  static constexpr int PW32 = PDG + st_a16(5 * (RH + 2) * (int)sizeof(T));
+  static constexpr int PANEL = PW32 + st_a16(RH * (int)sizeof(TV));
+  static constexpr int OWN = st_a16(RH * KT * (int)sizeof(T));
+  static constexpr int RING = RU_RING * RH * KT * (int)sizeof(TV);     // r32 columns
+  static constexpr int DRING = RU_RING * 5 * RH * (int)sizeof(TV);     // fp32 upper-slot runs, per column
+  using D = StDepth<PANEL, OWN, RU_MINB, RING + DRING>;
+};
+
+// one load step: column x of the segment [cb, ce) of strip `strip`; s0 = the segment's first (strip, column) step
+struct RuStep {
+  int s0, s_end, ncol, strip, cb, ce, x;
+  __device__ __forceinline__ void start(int s) {
+    s0 = s;
+    if (s >= s_end) return;
+    strip = s / ncol;
+    cb = s % ncol;
+    ce = min(ncol, cb + (s_end - s));
+    x = cb - 2;
+  }
+  __device__ __forceinline__ bool valid() const { return s0 < s_end; }
+  __device__ __forceinline__ void next() {
+    if (++x > ce + 2) start(s0 + (ce - cb));
+  }
+};
+
+template <typename T, typename TV, int KT>
+__global__ void __launch_bounds__(NT, RU_MINB)
+k_stencil_res_update(const DiaDev<T> A, const TV* __restrict__ dinv32, TV omega,
+                     const T* __restrict__ Pb0, const T* __restrict__ Pb1, T* Rb0, T* Rb1, TV* __restrict__ R32,
+                     TV* __restrict__ T32, const PanelCtl* __restrict__ ctl) {
+  using SH = RuShape<T, TV, KT>;
+  constexpr int CPT = SH::CPT, CG = SH::CG, RH = SH::RH, RPS = SH::RPS, S = SH::D::S;
+  constexpr int RP = S + 3, RO = S + 1;
+  extern __shared__ __align__(128) unsigned char st_sm[];
+  unsigned char* const pring = st_sm;
+  unsigned char* const oring = st_sm + RP * SH::PANEL;
+  TV* const xring = reinterpret_cast<TV*>(oring + RO * SH::OWN);   // [RU_RING][RH][KT]
+  TV* const dring = xring + RU_RING * RH * KT;                       // [RU_RING][5][RH]
+  const int it = ctl->iter;
+  const T* const Pk = (it & 1) ? Pb1 : Pb0;
+  const T* const Rin = (it & 1) ? Rb1 : Rb0;
+  T* const Rout = (it & 1) ? Rb0 : Rb1;
+  const int tid = threadIdx.x;
+  const int g = tid % CG, rr = tid / CG, c0 = g * CPT;
+  const bool inner = rr >= 1 && rr <= RPS;
+  const int n = A.n, nr = A.nr;
+  const int ncol = (n + nr - 1) / nr;
+  const int nstrip = (nr + RPS - 1) / RPS;
+  // nstep <= nr * ncol < n + nr: int for every operator launch_prolong_jacobi accepts (n + nr < 2^31)
+  const int nstep = nstrip * ncol;
+  const int per = (nstep + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int s_beg = (int)min((long long)nstep, (long long)blockIdx.x * per);
+  const int s_end = (int)min((long long)nstep, ((long long)blockIdx.x + 1) * per);
+  T al[CPT];
+#pragma unroll
+  for (int i = 0; i < CPT; ++i) al[i] = (T)ctl->alpha[c0 + i];
+
+  auto issue = [&](const RuStep& s, int lp, int lo) {
+    unsigned char* ps = pring + lp * SH::PANEL;
+    const long long r0 = (long long)s.strip * RPS;
+    if (s.x <= s.ce + 1) {
+      const long long g0 = (long long)s.x * nr + r0 - 2;
+      cp_rows<T, KT, RH + 2>(reinterpret_cast<T*>(ps), Pk, g0, n);
+      cp_diag_half<T, RH>(reinterpret_cast<T*>(ps + SH::PDG), A, g0, 0, 5);
+    }
+    if (s.x - 2 >= s.cb - 1)
+      cp_rows<TV, 1, RH>(reinterpret_cast<TV*>(ps + SH::PW32), dinv32, (long long)(s.x - 2) * nr + r0 - 1, n);
+    if (s.x - 1 >= s.cb - 1 && s.x - 1 <= s.ce)
+      cp_rows<T, KT, RH>(reinterpret_cast<T*>(oring + lo * SH::OWN), Rin, (long long)(s.x - 1) * nr + r0 - 1, n);
+  };
+  auto compute = [&](const RuStep& s, int sp, int so, int q) {
+    const unsigned char* pk[3];
+#pragma unroll
+    for (int d = 0; d < 3; ++d) {
+      const int k = sp + d + RP - 2;
+      pk[d] = pring + (k >= RP ? k - RP : k) * SH::PANEL;
+    }
+    const int r = s.strip * RPS + rr - 1;                  // this thread's row within a raster column
+    const int ca = s.x - 1;                                // A p, r', r32 of column ca
+    if (ca >= s.cb - 1 && ca <= s.ce) {
+      const T* ps[3];
+      const T* ds[3];
+#pragma unroll
+      for (int d = 0; d < 3; ++d) {
+        ps[d] = reinterpret_cast<const T*>(pk[d]);
+        ds[d] = reinterpret_cast<const T*>(pk[d] + SH::PDG);
+      }
+      T acc[CPT], rv[CPT];
+      TV r32[CPT];
+      stencil_row<T, CPT>(
+          acc, [&](int s9, T (&pv)[CPT]) { ldvec<T, CPT>(ps[s9 / 3] + (rr + s9 % 3) * KT + c0, pv); },
+          [&](int s9) { return st_half_val<T, RH>(ds, s9, rr); });
+      ldvec<T, CPT>(reinterpret_cast<const T*>(oring + so * SH::OWN) + rr * KT + c0, rv);
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) {
+        rv[i] -= al[i] * acc[i];
+        r32[i] = (TV)rv[i];
+      }
+      stvec<TV, CPT>(xring + (q * RH + rr) * KT + c0, r32);
+      if (g == 0) {
+#pragma unroll
+        for (int u = 0; u < 5; ++u) dring[(q * 5 + u) * RH + rr] = (TV)ds[1][u * (RH + 2) + rr + 1];
+      }
+      const long long row = (long long)ca * nr + r;
+      if (inner && r < nr && ca >= s.cb && ca < s.ce && row < n) {
+        stvec<T, CPT>(Rout + (size_t)row * KT + c0, rv);
+        stvec<TV, CPT>(R32 + (size_t)row * KT + c0, r32);
+      }
+    }
+    const int ct = s.x - 3;                                // T32 of column ct
+    const long long row = (long long)ct * nr + r;
+    if (ct >= s.cb && ct < s.ce && inner && r < nr && row < n) {
+      const TV* xs[3];
+      const TV* ws[3];
+      const TV* ds[3];
+#pragma unroll
+      for (int d = 0; d < 3; ++d) {
+        xs[d] = xring + ((q + 1 + d) & (RU_RING - 1)) * RH * KT;   // columns ct - 1, ct, ct + 1
+        ws[d] = reinterpret_cast<const TV*>(pk[d] + SH::PW32);
+        ds[d] = dring + ((q + 1 + d) & (RU_RING - 1)) * 5 * RH;
+      }
+      const int rl = rr - 1;
+      TV acc[CPT], xo[CPT], out[CPT];
+      stencil_row<TV, CPT>(
+          acc,
+          [&](int s9, TV (&xv)[CPT]) {
+            ldvec<TV, CPT>(xs[s9 / 3] + (rl + s9 % 3) * KT + c0, xv);
+            if (s9 == 4) {
+#pragma unroll
+              for (int i = 0; i < CPT; ++i) xo[i] = xv[i];
+            }
+          },
+          [&](int s9) { return st_half_val<TV, RPS>(ds, s9, rl) * (omega * ws[s9 / 3][rl + s9 % 3]); });
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) out[i] = xo[i] - acc[i];
+      stvec<TV, CPT>(T32 + (size_t)row * KT + c0, out);
+    }
+  };
+
+  RuStep ld, st;
+  ld.s_end = s_end;
+  ld.ncol = ncol;
+  ld.start(s_beg);
+  st = ld;
+  int lp = 0, lo = 0, sp = 0, so = 0, q = 0;
+#pragma unroll 1
+  for (int k = 0; k < S; ++k) {
+    if (ld.valid()) issue(ld, lp, lo);
+    cp_async_commit();
+    if (ld.valid()) ld.next();
+    lp = lp + 1 == RP ? 0 : lp + 1;
+    lo = lo + 1 == RO ? 0 : lo + 1;
+  }
+#pragma unroll 1
+  while (st.valid()) {
+    cp_async_wait<S - 1>();
+    __syncthreads();                 // this step's slots are in, the previous step's r32 column is written
+    if (ld.valid()) issue(ld, lp, lo);
+    cp_async_commit();
+    if (ld.valid()) ld.next();
+    lp = lp + 1 == RP ? 0 : lp + 1;
+    lo = lo + 1 == RO ? 0 : lo + 1;
+    compute(st, sp, so, q);
+    st.next();
+    sp = sp + 1 == RP ? 0 : sp + 1;
+    so = so + 1 == RO ? 0 : so + 1;
+    q = (q + 1) & (RU_RING - 1);
+  }
+  cp_async_wait<0>();
+}
+
+// differs = 1 unless the 5 upper-slot runs of A32 are those of A rounded to TV, bit for bit
+template <typename T, typename TV>
+__global__ void k_dia_rounds(const DiaDev<T> A, const DiaDev<TV> A32, int* differs) {
+  const long long tot = 5LL * A.n;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < tot; i += (long long)gridDim.x * blockDim.x) {
+    const int u = (int)(i / A.n), row = (int)(i % A.n);
+    const TV a = (TV)A.run(4 + u)[row], b = A32.run(4 + u)[row];
+    static_assert(sizeof(TV) == 4, "fp32 copies");
+    unsigned ua, ub;
+    memcpy(&ua, &a, 4);
+    memcpy(&ub, &b, 4);
+    if (ua != ub) *differs = 1;
   }
 }
 

@@ -305,11 +305,12 @@ class B200Factor:
     def profile_classes(self):
         """per kernel class of the timed finest-level launches: {name: (ms, algorithmic bytes, launches)}"""
         names = ["plain", "cg", "residual_gate", "residual", "jacobi", "jacobi_dot", "prolong_add", "prolong_jacobi_fused",
-                 "cg_step_fused"]
+                 "cg_step_fused", "residual_sweep_fused"]
         ms = np.zeros(2 * len(names))
         by = np.zeros(2 * len(names))
         ln = np.zeros(2 * len(names), dtype=np.int64)
-        _lib.check(self._lib, self._h, self._lib.cs_b200_profile_classes(self._h, _lib._ptr(ms), _lib._ptr(by), _lib._ptr(ln)))
+        _lib.check(self._lib, self._h, self._lib.cs_b200_profile_classes_n(self._h, len(ms), _lib._ptr(ms), _lib._ptr(by),
+                                                                           _lib._ptr(ln)))
         return {f"{names[i // 2]}_{'f32' if i % 2 else 'f64'}": (float(ms[i]), float(by[i]), int(ln[i]))
                 for i in range(2 * len(names)) if ln[i]}
 

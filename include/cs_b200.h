@@ -430,6 +430,10 @@ int cs_b200_comm_barrier(cs_b200_comm* c);
  * sweep + r.z, 6 prolong-add, 7 fused prolongation + sweep, 8 fused CG step (p = z + beta p, A p, p.Ap,
  * deferred x update; since ABI 1005, 16 slots before).                                             */
 int cs_b200_profile_classes(cs_b200_handle* h, double* ms18, double* bytes18, int64_t* launches18);
+/* The same for the first nslots slots (20 exist): slot 18 (19 unused) is the fused residual update + level-0
+ * residual sweep of the mixed cycle (r -= alpha A p, r32, the fp32 level-0 residual; kernels.cuh
+ * k_stencil_res_update), which the 18-slot call leaves out.                                       */
+int cs_b200_profile_classes_n(cs_b200_handle* h, int nslots, double* ms, double* bytes, int64_t* launches);
 
 /* Library/ABI version: major*1000 + minor.                                          */
 int cs_b200_version(void);

@@ -106,7 +106,11 @@ def finest_bytes(levels, prolong_form):
     # form (CS_B200_NO_STENCIL_PIPE)
     # (the pipelined ones carry a last template argument: the half form or not)
     cg_step = n * (dg64 * 8 + d32 + 3 * d64 + 1.5 * d64)
+    cg_step_no_ap = cg_step - n * d64
     res0 = n * (dg32 * 4 + d32 + 4 + d32)
+    # fused residual sweep (strips of 62 rows): p and the 5 fp64 upper runs on rows -2 ... 63, r and the fp32 1/diag
+    # on rows -1 ... 62 in; r, R32, T32 out (the fp32 diagonals are the fp64 ones rounded on chip)
+    ru = n * ((d64 + 5 * 8) * 66 / 62 + (d64 + 4) * 64 / 62 + d64 + d32 + d32)
     return {
         "k_stencil<double,8,1>": n * (9 * 8 + d64 + d64),               # CG SpMM: diagonals, P, AP
         "k_stencil_pipe<double,8,1,*>": n * (dg64 * 8 + d64 + d64),
@@ -115,7 +119,9 @@ def finest_bytes(levels, prolong_form):
         "k_stencil_pipe<double,8,2,*>": n * (dg64 * 8 + 3 * d64),
         # fused CG step: diagonals, Z32, p_{it-1} in, AP, p_it out; X in/out + p_{it-2} in every other step
         "k_stencil_cg<double,8,float>": cg_step,
-        "k_stencil_cg_pipe<double,8,float,*>": cg_step,
+        "k_stencil_cg_pipe<double,8,float,*,true>": cg_step,
+        "k_stencil_cg_pipe<double,8,float,*,false>": cg_step_no_ap,                # A p not stored
+        "k_stencil_res_update<double,float,8>": ru,
         "k_cg_update_r0<double,8,float>": n * (d64 + 8 + 2 * d64 + d32),  # AP, 1/diag, R in/out, R32
         "k_stencil<float,8,7>#1": res0,                                 # residual with implicit x0: diagonals, b, 1/diag, t
         "k_stencil_pipe<float,8,7,*>#1": res0,
@@ -187,6 +193,9 @@ def main():
             agg[key][1] += e.time_range.elapsed_us()
     niter = max(1, len(iters))
     table, shape = finest_bytes(levels, a.prolong_form)
+    if any(k.startswith("k_stencil_res_update<") for k in agg):
+        # the fused sweep forms the level-0 residual: the first SP_RES0 launch of the iteration is level 1's
+        table = {k: v for k, v in table.items() if not k.startswith(("k_stencil<float,8,7>", "k_stencil_pipe<float,8,7,"))}
     sum_us = sum(v[1] for v in agg.values()) / niter
     rows = {}
     for key, (cnt, us) in sorted(agg.items(), key=lambda kv: -kv[1][1]):
