@@ -242,16 +242,21 @@ int win_mask() {
   return e ? atoi(e) : 15;
 }
 
+// sizes, lanes per row of k_spmm and the row-block height of an operator with `nrows` rows: small operators
+// (coarse levels) get shorter blocks so that >= 4 CTAs per SM exist -- their kernels are latency-bound chains
+// of dependent gathers, not bandwidth-bound
+int size_csr(const cs_b200_handle* h, DevCsr& d, int64_t nrows, int64_t nnz) {
+  d.nrows = (int)nrows;
+  d.nnz = nnz;
+  d.lpr = (nrows > 0 && (double)nnz / (double)nrows >= 20.0) ? 4 : 1;
+  const int unit = d.lpr == 4 ? 8 : 32;          // rows per pass of k_spmm at KT = 8
+  const int max_rows = (int)((nrows + 4 * h->num_sms - 1) / (4 * h->num_sms));
+  return std::min(NT, std::max(unit, (max_rows + unit - 1) / unit * unit));
+}
+
 template <typename T>
 int upload_csr(cs_b200_handle* h, const csb_amg::Csr& m, DevCsr& d, bool windowed, const T* d_dinv = nullptr) {
-  d.nrows = (int)m.nrows;
-  d.nnz = m.nnz();
-  d.lpr = (m.nrows > 0 && (double)d.nnz / (double)m.nrows >= 20.0) ? 4 : 1;
-  // small operators (coarse levels): shrink the row blocks so that >= 4 CTAs per SM exist --
-  // their kernels are latency-bound chains of dependent gathers, not bandwidth-bound
-  const int unit = d.lpr == 4 ? 8 : 32;          // rows per pass of k_spmm at KT = 8
-  int max_rows = (int)((m.nrows + 4 * h->num_sms - 1) / (4 * h->num_sms));
-  max_rows = std::min(NT, std::max(unit, (max_rows + unit - 1) / unit * unit));
+  const int max_rows = size_csr(h, d, m.nrows, m.nnz());
   std::vector<int> bstart;
   build_row_blocks(m.ptr, m.nrows, bstart, max_rows);
   d.nblocks = (int)bstart.size() - 1;
@@ -324,37 +329,57 @@ int build_windowed(cs_b200_handle* h, DevCsr& d, const int* rowptr, const int* c
   return CS_B200_OK;
 }
 
+// cudaMalloc + zero fill on the handle's stream
+int alloc_zeroed(cs_b200_handle* h, void** p, size_t bytes) {
+  CK(h, cudaMalloc(p, bytes));
+  CK(h, cudaMemsetAsync(*p, 0, bytes, h->stream));
+  return CS_B200_OK;
+}
+
+// Level l of either builder's hierarchy: n rows, smoother weight omega.  Without `own0` level 0 aliases the
+// handle's operator and 1/diag, and false is returned: the builder has no A or 1/diag of its own to make.
+bool begin_level(cs_b200_handle* h, DevLevel& L, int l, bool own0, int64_t n, double omega) {
+  L.n = n;
+  L.n_pad = (n + 3) / 4 * 4;
+  L.omega = omega;
+  if (l > 0 || own0) return true;
+  L.A = h->A0;  // alias, not owned
+  L.dinv = h->d_dinv;
+  return false;
+}
+
+// the x / b / t / y panels of a coarse level
+template <typename TV>
+int level_panels(cs_b200_handle* h, DevLevel& L) {
+  const size_t pe = (size_t)L.n_pad * h->ktmax * sizeof(TV);
+  void** bufs[] = {&L.x, &L.b, &L.t, &L.y};
+  for (void** bp : bufs)
+    if (int rc = alloc_zeroed(h, bp, pe)) return rc;
+  return CS_B200_OK;
+}
+
+// windowed row-block forms are built for level l's operator (mask bit 0 finest, 1 coarse), P (bit 2), R (bit 3)
+bool level_windowed(const cs_b200_handle* h, int l, int64_t n) {
+  return h->opts.window > 0 || (n >= 20000 && (win_mask() & (l == 0 ? 1 : 2)));
+}
+
 // Upload a host hierarchy as device levels of type TV.  `own0`: the finest level gets its own
 // device CSR (float copy for the mixed-precision cycle); otherwise it aliases the handle's.
 template <typename TV>
-int upload_levels(cs_b200_handle* h, const csb_amg::Hierarchy& hier, std::vector<DevLevel>& lv, bool own0) {
+int make_levels(cs_b200_handle* h, const csb_amg::Hierarchy& hier, std::vector<DevLevel>& lv, bool own0) {
   const int nl = (int)hier.levels.size();
   lv.resize(nl);
   for (int l = 0; l < nl; ++l) {
     const csb_amg::HostLevel& hl = hier.levels[l];
     DevLevel& L = lv[l];
-    L.n = hl.A.nrows;
-    L.n_pad = (L.n + 3) / 4 * 4;
-    L.omega = hl.omega;
-    if (l == 0 && !own0) {
-      L.A = h->A0;  // alias, not owned
-      L.dinv = h->d_dinv;
-    } else {
+    if (begin_level(h, L, l, own0, hl.A.nrows, hl.omega)) {
       std::vector<TV> dv(L.n_pad, TV(0));
       for (int64_t i = 0; i < L.n; ++i) dv[i] = (TV)hl.dinv[i];
       CK(h, cudaMalloc(&L.dinv, (size_t)L.n_pad * sizeof(TV)));
       CK(h, h2d(h, L.dinv, dv.data(), (size_t)L.n_pad * sizeof(TV)));
-      const bool win = h->opts.window > 0 || (L.n >= 20000 && (win_mask() & (l == 0 ? 1 : 2)));
-      int rc = upload_csr<TV>(h, hl.A, L.A, win, (const TV*)L.dinv);
+      int rc = upload_csr<TV>(h, hl.A, L.A, level_windowed(h, l, L.n), (const TV*)L.dinv);
+      if (!rc && l > 0) rc = level_panels<TV>(h, L);
       if (rc) return rc;
-      if (l > 0) {
-        const size_t pe = (size_t)L.n_pad * h->ktmax * sizeof(TV);
-        void** bufs[] = {&L.x, &L.b, &L.t, &L.y};
-        for (void** bp : bufs) {
-          CK(h, cudaMalloc(bp, pe));
-          CK(h, cudaMemsetAsync(*bp, 0, pe, h->stream));
-        }
-      }
     }
     if (l + 1 < nl) {
       int rc = upload_csr<TV>(h, hl.P, L.P, L.n >= 20000 && (win_mask() & 4));
@@ -366,10 +391,53 @@ int upload_levels(cs_b200_handle* h, const csb_amg::Hierarchy& hier, std::vector
   return CS_B200_OK;
 }
 
+template <typename TV>
+int make_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLevel>& lv, bool own0);
+
+void wait_pinv(csb_amg::Hierarchy&) {}
+void wait_pinv(csb_dev::DHierarchy& hier) { csb_dev::coarse_pinv_wait(hier); }
+
+// What either builder's hierarchy leaves on the handle: its levels resident (make_levels), the fp32 or Z panels,
+// the coarse pseudo-inverse.  fp64 handles run the V-cycle in fp32 (opts.mixed: 0 auto = on, -1 off): the
+// preconditioner only has to be a good approximate inverse, CG's own vectors stay fp64.
+template <typename T, class Hier>
+int adopt_hierarchy(cs_b200_handle* h, Hier& hier) {
+  const int nl = (int)hier.levels.size();
+  h->mixed = nl > 1 && sizeof(T) == 8 && h->opts.mixed >= 0;
+  Tick tick;
+  if (h->mixed) {
+    int rc = make_levels<float>(h, hier, h->lv32, true);
+    if (rc) return rc;
+    // the fp64 side only needs level 0's omega / dinv (already on the handle)
+    h->lv.resize(nl);
+    for (int l = 0; l < nl; ++l) { h->lv[l].n = hier.levels[l].A.nrows; h->lv[l].omega = hier.levels[l].omega; }
+    h->lv[0].A = h->A0;
+    h->lv[0].dinv = h->d_dinv;
+    const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(float);
+    void** bufs[] = {&h->R32, &h->X32, &h->T32, &h->Z32};
+    for (void** bp : bufs)
+      if ((rc = alloc_zeroed(h, bp, pe))) return rc;
+  } else {
+    int rc = make_levels<T>(h, hier, h->lv, false);
+    if (!rc) rc = alloc_zeroed(h, &h->Z, (size_t)h->n_pad * h->ktmax * sizeof(T));
+    if (rc) return rc;
+  }
+  tick("levels");
+  wait_pinv(hier);
+  tick("coarse pseudo-inverse (wait)");
+  const size_t nc = (size_t)hier.levels.back().A.nrows;
+  if (hier.coarse_pinv.size() == nc * nc && nc > 0) {
+    CK(h, cudaMalloc(&h->d_pinv, nc * nc * sizeof(double)));
+    CK(h, h2d(h, h->d_pinv, hier.coarse_pinv.data(), nc * nc * sizeof(double)));
+  }
+  CK(h, cudaStreamSynchronize(h->stream));
+  h->amg = nl > 1;
+  return CS_B200_OK;
+}
+
 // Smoothed-aggregation hierarchy: built on the host (amg_host.hpp), resident on the device.
 template <typename T>
-int setup_amg(cs_b200_handle* h, const std::vector<int>& rp, const std::vector<int>& ci,
-              const T* vals_host) {
+int setup_amg(cs_b200_handle* h, const std::vector<int>& rp, const std::vector<int>& ci, const T* vals_host) {
   csb_amg::Csr a0;
   a0.nrows = a0.ncols = h->n;
   a0.ptr = rp;
@@ -379,40 +447,7 @@ int setup_amg(cs_b200_handle* h, const std::vector<int>& rp, const std::vector<i
   csb_amg::Hierarchy hier = csb_amg::build_hierarchy(std::move(a0));
   tick("host hierarchy");
   h->amg_opc = hier.operator_complexity();
-  const int nl = (int)hier.levels.size();
-  // fp64 handles run the V-cycle in fp32 (opts.mixed: 0 auto = on, -1 off): the preconditioner
-  // only has to be a good approximate inverse, CG's own vectors stay fp64
-  h->mixed = nl > 1 && sizeof(T) == 8 && h->opts.mixed >= 0;
-  int rc = h->mixed ? upload_levels<float>(h, hier, h->lv32, true) : CS_B200_OK;
-  if (rc) return rc;
-  tick("levels: windows + upload");
-  if (h->mixed) {
-    // the fp64 side only needs level 0's omega / dinv (already on the handle)
-    h->lv.resize(nl);
-    for (int l = 0; l < nl; ++l) { h->lv[l].n = hier.levels[l].A.nrows; h->lv[l].omega = hier.levels[l].omega; }
-    h->lv[0].A = h->A0;
-    h->lv[0].dinv = h->d_dinv;
-    const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(float);
-    void** bufs[] = {&h->R32, &h->X32, &h->T32, &h->Z32};
-    for (void** bp : bufs) {
-      CK(h, cudaMalloc(bp, pe));
-      CK(h, cudaMemsetAsync(*bp, 0, pe, h->stream));
-    }
-  } else {
-    rc = upload_levels<T>(h, hier, h->lv, false);
-    if (rc) return rc;
-    const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(T);
-    CK(h, cudaMalloc(&h->Z, pe));
-    CK(h, cudaMemsetAsync(h->Z, 0, pe, h->stream));
-  }
-  const size_t nc = (size_t)hier.levels.back().A.nrows;
-  if (hier.coarse_pinv.size() == nc * nc && nc > 0) {
-    CK(h, cudaMalloc(&h->d_pinv, nc * nc * sizeof(double)));
-    CK(h, h2d(h, h->d_pinv, hier.coarse_pinv.data(), nc * nc * sizeof(double)));
-  }
-  CK(h, cudaStreamSynchronize(h->stream));
-  h->amg = nl > 1;
-  return CS_B200_OK;
+  return adopt_hierarchy<T>(h, hier);
 }
 
 // panels, 1/diag, current vectors, control block: what every handle needs whatever built its operators
@@ -454,9 +489,10 @@ int alloc_common(cs_b200_handle* h) {
   return CS_B200_OK;
 }
 
+// host-side setup of a handle whose CSR is resident: row blocks and windows built from host copies of the
+// pattern, the hierarchy by amg_host.hpp
 template <typename T>
-int finish_setup(cs_b200_handle* h, const std::vector<int>& h_rowptr, const std::vector<int>* h_colidx,
-                 const T* h_vals) {
+int finish_setup(cs_b200_handle* h, const std::vector<int>& h_rowptr) {
   std::vector<int> bstart;
   build_row_blocks(h_rowptr, h->n, bstart);
   h->nblocks = (int)bstart.size() - 1;
@@ -467,28 +503,26 @@ int finish_setup(cs_b200_handle* h, const std::vector<int>& h_rowptr, const std:
   int rc0 = alloc_common<T>(h);
   if (rc0) return rc0;
   CK(h, cudaStreamSynchronize(h->stream));
-  std::vector<int> ci_local;
-  std::vector<T> v_local;
+  std::vector<int> h_colidx;
+  std::vector<T> h_vals;
   const bool want_win = h->opts.window >= 0 && (h->opts.window > 0 || h->n >= 20000) && (win_mask() & 1);
   const bool want_amg = h->opts.precond == CS_B200_PRECOND_AMG;
-  if (!h_colidx && (want_win || want_amg)) {  // matrix arrived on the device (NCCL broadcast)
-    ci_local.resize(h->nnz);
-    CK(h, cudaMemcpy(ci_local.data(), h->d_colidx, (size_t)h->nnz * sizeof(int), cudaMemcpyDeviceToHost));
-    h_colidx = &ci_local;
-    if (want_amg) {
-      v_local.resize(h->nnz);
-      CK(h, cudaMemcpy(v_local.data(), h->d_vals, (size_t)h->nnz * sizeof(T), cudaMemcpyDeviceToHost));
-      h_vals = v_local.data();
-    }
+  if (want_win || want_amg) {
+    h_colidx.resize(h->nnz);
+    CK(h, cudaMemcpy(h_colidx.data(), h->d_colidx, (size_t)h->nnz * sizeof(int), cudaMemcpyDeviceToHost));
+  }
+  if (want_amg) {
+    h_vals.resize(h->nnz);
+    CK(h, cudaMemcpy(h_vals.data(), h->d_vals, (size_t)h->nnz * sizeof(T), cudaMemcpyDeviceToHost));
   }
   Tick tick;
   if (want_win) {
-    int rc = build_windowed<T>(h, h->A0, h_rowptr.data(), h_colidx->data(), h->n_pad, (const T*)h->d_dinv);
+    int rc = build_windowed<T>(h, h->A0, h_rowptr.data(), h_colidx.data(), h->n_pad, (const T*)h->d_dinv);
     if (rc) return rc;
     tick("finest operator: windows");
   }
   if (want_amg) {
-    int rc = setup_amg<T>(h, h_rowptr, *h_colidx, h_vals);
+    int rc = setup_amg<T>(h, h_rowptr, h_colidx, h_vals.data());
     if (rc) return rc;
   }
   return cs_b200_reset_currents(h);
@@ -601,9 +635,7 @@ int device_stencil(cs_b200_handle* h, DevCsr& d) {
 // the source is the handle's own matrix), the fp64 values move or are converted
 template <typename TV>
 int adopt_csr(cs_b200_handle* h, csb_dev::DCsr& src, bool duplicate, DevCsr& d, bool windowed, const TV* d_dinv) {
-  d.nrows = (int)src.nrows;
-  d.nnz = src.nnz;
-  d.lpr = (src.nrows > 0 && (double)d.nnz / (double)src.nrows >= 20.0) ? 4 : 1;
+  const int max_rows = size_csr(h, d, src.nrows, src.nnz);
   const size_t np = (size_t)src.nrows + 1, ne = std::max<size_t>(1, (size_t)src.nnz);
   if (duplicate) {
     CK(h, cudaMalloc(&d.rowptr, np * sizeof(int)));
@@ -628,10 +660,6 @@ int adopt_csr(cs_b200_handle* h, csb_dev::DCsr& src, bool duplicate, DevCsr& d, 
       cudaFree(src.val); src.val = nullptr;
     }
   }
-  // small operators (coarse levels): shrink the row blocks so that >= 4 CTAs per SM exist
-  const int unit = d.lpr == 4 ? 8 : 32;
-  int max_rows = (int)((src.nrows + 4 * h->num_sms - 1) / (4 * h->num_sms));
-  max_rows = std::min(NT, std::max(unit, (max_rows + unit - 1) / unit * unit));
   int rc = device_row_blocks(h, d, max_rows);
   if (rc) return rc;
   if (src.nrows == src.ncols && d_dinv != nullptr) {   // square level operator: stencil form if it has one
@@ -647,7 +675,7 @@ int adopt_csr(cs_b200_handle* h, csb_dev::DCsr& src, bool duplicate, DevCsr& d, 
 }
 
 template <typename TV>
-int adopt_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLevel>& lv, bool own0) {
+int make_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLevel>& lv, bool own0) {
   const int nl = (int)hier.levels.size();
   lv.resize(nl);
   Tick lt;
@@ -661,13 +689,7 @@ int adopt_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLe
   for (int l = 0; l < nl; ++l) {
     csb_dev::DLevel& hl = hier.levels[l];
     DevLevel& L = lv[l];
-    L.n = hl.A.nrows;
-    L.n_pad = (L.n + 3) / 4 * 4;
-    L.omega = hl.omega;
-    if (l == 0 && !own0) {
-      L.A = h->A0;  // alias, not owned
-      L.dinv = h->d_dinv;
-    } else {
+    if (begin_level(h, L, l, own0, hl.A.nrows, hl.omega)) {
       CK(h, cudaMalloc(&L.dinv, (size_t)L.n_pad * sizeof(TV)));
       CK(h, cudaMemsetAsync(L.dinv, 0, (size_t)L.n_pad * sizeof(TV), h->stream));
       if (sizeof(TV) == 8) {
@@ -675,18 +697,10 @@ int adopt_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLe
       } else if (csb_dev::convert_values(h->stream, hl.dinv, (float*)L.dinv, L.n)) {
         return set_err(h, CS_B200_ERR_CUDA, "dinv conversion launch failed");
       }
-      const bool win = h->opts.window > 0 || (L.n >= 20000 && (win_mask() & (l == 0 ? 1 : 2)));
-      int rc = adopt_csr<TV>(h, hl.A, l == 0, L.A, win, (const TV*)L.dinv);
+      int rc = adopt_csr<TV>(h, hl.A, l == 0, L.A, level_windowed(h, l, L.n), (const TV*)L.dinv);
       if (rc) return rc;
       mark(l, "A: copy/convert, blocks, windows");
-      if (l > 0) {
-        const size_t pe = (size_t)L.n_pad * h->ktmax * sizeof(TV);
-        void** bufs[] = {&L.x, &L.b, &L.t, &L.y};
-        for (void** bp : bufs) {
-          CK(h, cudaMalloc(bp, pe));
-          CK(h, cudaMemsetAsync(*bp, 0, pe, h->stream));
-        }
-      }
+      if (l > 0 && (rc = level_panels<TV>(h, L))) return rc;
     }
     if (l + 1 < nl) {
       int rc = adopt_csr<TV>(h, hl.P, false, L.P, L.n >= 20000 && (win_mask() & 4), (const TV*)nullptr);
@@ -708,8 +722,10 @@ int adopt_levels(cs_b200_handle* h, csb_dev::DHierarchy& hier, std::vector<DevLe
   return CS_B200_OK;
 }
 
+// Smoothed-aggregation hierarchy built on the device (setup_device.cu).  `job`, the create sequence's level-0
+// seed pass, is handed to build_hierarchy, which consumes it.
 template <typename T>
-int setup_amg_device(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob* job,
+int setup_amg_device(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob*& job,
                      const csb_dev::DeviceSeed* dseed) {
   const bool verbose = std::getenv("CS_B200_VERBOSE") != nullptr;
   csb_dev::DCsr a0;
@@ -722,87 +738,31 @@ int setup_amg_device(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev:
     a0.val = (double*)h->d_vals;
   } else {   // the hierarchy is built in fp64 whatever the handle computes in
     cudaError_t e = cudaMalloc(&tmp64, std::max<size_t>(1, (size_t)h->nnz) * sizeof(double));
-    if (e != cudaSuccess) {
-      csb_dev::seed_discard(job);
+    if (e != cudaSuccess)
       return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (fp64 copy of the matrix)", cudaGetErrorString(e));
-    }
     csb_dev::convert_values(h->stream, (const float*)h->d_vals, tmp64, h->nnz);
     a0.val = tmp64;
   }
   Tick tick;
   csb_dev::DHierarchy hier;
-  int rc = csb_dev::build_hierarchy(h->stream, a0, hp, job, dseed, 12, 200, hier, h->err, verbose);
-  auto done = [&](int code) {
-    cudaStreamSynchronize(h->stream);
-    csb_dev::free_hierarchy(hier);
-    cudaFree(tmp64);
-    return code;
-  };
-  if (rc) return done(rc_dev(h, rc));
-  tick("device hierarchy");
-  h->amg_opc = hier.operator_complexity;
-  const int nl = (int)hier.levels.size();
-  h->mixed = nl > 1 && sizeof(T) == 8 && h->opts.mixed >= 0;
-  if (h->mixed) {
-    rc = adopt_levels<float>(h, hier, h->lv32, true);
-    if (rc) return done(rc);
-    h->lv.resize(nl);
-    for (int l = 0; l < nl; ++l) { h->lv[l].n = hier.levels[l].A.nrows; h->lv[l].omega = hier.levels[l].omega; }
-    h->lv[0].A = h->A0;
-    h->lv[0].dinv = h->d_dinv;
-    const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(float);
-    void** bufs[] = {&h->R32, &h->X32, &h->T32, &h->Z32};
-    for (void** bp : bufs) {
-      cudaError_t e = cudaMalloc(bp, pe);
-      if (e == cudaSuccess) e = cudaMemsetAsync(*bp, 0, pe, h->stream);
-      if (e != cudaSuccess) return done(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (fp32 panels)", cudaGetErrorString(e)));
-    }
-  } else {
-    rc = adopt_levels<T>(h, hier, h->lv, false);
-    if (rc) return done(rc);
-    const size_t pe = (size_t)h->n_pad * h->ktmax * sizeof(T);
-    cudaError_t e = cudaMalloc(&h->Z, pe);
-    if (e == cudaSuccess) e = cudaMemsetAsync(h->Z, 0, pe, h->stream);
-    if (e != cudaSuccess) return done(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (Z panel)", cudaGetErrorString(e)));
+  csb_dev::SeedJob* pre = job;
+  job = nullptr;
+  int rc = rc_dev(h, csb_dev::build_hierarchy(h->stream, a0, hp, pre, dseed, 12, 200, hier, h->err, verbose));
+  if (!rc) {
+    tick("device hierarchy");
+    h->amg_opc = hier.operator_complexity;
+    rc = adopt_hierarchy<T>(h, hier);
   }
-  tick("levels: row blocks + windows");
-  csb_dev::coarse_pinv_wait(hier);
-  tick("coarse pseudo-inverse (wait)");
-  const size_t nc = (size_t)hier.levels.back().A.nrows;
-  if (hier.coarse_pinv.size() == nc * nc && nc > 0) {
-    cudaError_t e = cudaMalloc(&h->d_pinv, nc * nc * sizeof(double));
-    if (e == cudaSuccess) e = h2d(h, h->d_pinv, hier.coarse_pinv.data(), nc * nc * sizeof(double));
-    if (e != cudaSuccess) return done(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (coarse pseudo-inverse)", cudaGetErrorString(e)));
-  }
-  h->amg = nl > 1;
-  return done(CS_B200_OK);
-}
-
-template <typename T>
-int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob* job,
-                    const csb_dev::DeviceSeed* dseed);
-
-template <typename T>
-int finish_setup_device(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob* job,
-                        const csb_dev::DeviceSeed* dseed = nullptr) {
-  h->A0 = DevCsr{h->d_rowptr, h->d_colidx, h->d_vals, nullptr, 0, (int)h->n, h->nnz, 1};
-  Tick tick0;
-  int rc = device_row_blocks(h, h->A0, NT);
-  if (rc) { csb_dev::seed_discard(job); return rc; }
-  h->d_bstart = h->A0.bstart;
-  h->nblocks = h->A0.nblocks;
-  rc = alloc_common<T>(h);
-  if (rc) { csb_dev::seed_discard(job); return rc; }
-  if (tick0.on) { cudaStreamSynchronize(h->stream); tick0("row blocks + panels"); }
-  rc = build_operators<T>(h, hp, job, dseed);
-  if (rc) return rc;
-  return cs_b200_reset_currents(h);
+  cudaStreamSynchronize(h->stream);
+  csb_dev::free_hierarchy(hier);
+  cudaFree(tmp64);
+  return rc;
 }
 
 // 1/diag, the finest operator's stencil / window form, the multigrid hierarchy: everything that depends
 // on the matrix VALUES (re-run by cs_b200_set_grounds after the values changed)
 template <typename T>
-int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob* job,
+int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob*& job,
                     const csb_dev::DeviceSeed* dseed) {
   int rc = CS_B200_OK;
   k_dinv<T><<<std::min<int64_t>((h->n_pad + 255) / 256, 4096), 256, 0, h->stream>>>(
@@ -814,7 +774,7 @@ int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::
   if (want_win || h->opts.stencil > 0) {
     rc = device_stencil<T>(h, h->A0);
     if (!rc && !h->A0.dia && want_win) rc = device_windows<T>(h, h->A0, h->n_pad, (const T*)h->d_dinv);
-    if (rc) { csb_dev::seed_discard(job); return rc; }
+    if (rc) return rc;
     tick(h->A0.dia ? "finest operator: stencil form" : "finest operator: windows");
   }
   if (want_amg) {
@@ -850,13 +810,29 @@ int build_operators(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::
       }
       if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (second r panel)", cudaGetErrorString(e));
     }
-  } else {
-    csb_dev::seed_discard(job);
   }
   Tick tick1;
   csb_dev::trim_pool(h->device);
   tick1("scratch pool released");
   return CS_B200_OK;
+}
+
+// device-side setup of a handle whose CSR is resident: row blocks, panels, then build_operators
+template <typename T>
+int finish_setup_device(cs_b200_handle* h, const csb_dev::HostPattern& hp, csb_dev::SeedJob*& job,
+                        const csb_dev::DeviceSeed* dseed) {
+  h->A0 = DevCsr{h->d_rowptr, h->d_colidx, h->d_vals, nullptr, 0, (int)h->n, h->nnz, 1};
+  Tick tick0;
+  int rc = device_row_blocks(h, h->A0, NT);
+  if (rc) return rc;
+  h->d_bstart = h->A0.bstart;
+  h->nblocks = h->A0.nblocks;
+  rc = alloc_common<T>(h);
+  if (rc) return rc;
+  if (tick0.on) { cudaStreamSynchronize(h->stream); tick0("row blocks + panels"); }
+  rc = build_operators<T>(h, hp, job, dseed);
+  if (rc) return rc;
+  return cs_b200_reset_currents(h);
 }
 
 int common_create(cs_b200_handle* h, const cs_b200_opts* opts) {
@@ -890,14 +866,7 @@ int common_create(cs_b200_handle* h, const cs_b200_opts* opts) {
   CK(h, cudaEventCreate(&h->ev1));
   CK(h, cudaEventCreate(&h->ev2));
   CK(h, cudaEventCreate(&h->ev3));
-  h->n_pad = (h->n + 3) / 4 * 4;
   return CS_B200_OK;
-}
-
-template <typename I>
-void narrow_indices(const I* src, int64_t count, int base, std::vector<int>& dst) {
-  dst.resize(count);
-  for (int64_t i = 0; i < count; ++i) dst[i] = (int)(src[i] - base);
 }
 
 // ---------------------------------------------------------------------------
@@ -2269,8 +2238,7 @@ int set_handleless_error(int code, const char* msg) {
 // ---------------------------------------------------------------------------
 namespace {
 template <typename T>
-int assemble_raster(cs_b200_handle* h, int64_t nrows, int64_t ncols, const T* g_host,
-                           int four, int avg_res, std::vector<int>& rp_host) {
+int assemble_raster(cs_b200_handle* h, int64_t nrows, int64_t ncols, const T* g_host, int four, int avg_res) {
   const int64_t ncell = nrows * ncols;
   T* d_g = nullptr;
   int *d_valid = nullptr, *d_nodeid = nullptr, *d_rowcnt = nullptr;
@@ -2303,9 +2271,8 @@ int assemble_raster(cs_b200_handle* h, int64_t nrows, int64_t ncols, const T* g_
   CKR(cudaGetLastError());
   CKR(cudaMalloc(&h->d_rowptr, (size_t)(n + 1) * sizeof(int)));
   CKR(ras::exclusive_scan(d_rowcnt, h->d_rowptr, n + 1, h->stream));
-  rp_host.resize((size_t)n + 1);
-  CKR(cudaMemcpy(rp_host.data(), h->d_rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyDeviceToHost));
-  const int64_t nnz = rp_host[(size_t)n];
+  int nnz = 0;
+  CKR(cudaMemcpy(&nnz, h->d_rowptr + n, sizeof(int), cudaMemcpyDeviceToHost));
   if (nnz <= 0) { cleanup(); return set_err(h, CS_B200_ERR_ARG, "assembled matrix is empty"); }
   CKR(cudaMalloc(&h->d_colidx, (size_t)nnz * sizeof(int)));
   CKR(cudaMalloc(&h->d_vals, (size_t)nnz * sizeof(T)));
@@ -2317,8 +2284,98 @@ int assemble_raster(cs_b200_handle* h, int64_t nrows, int64_t ncols, const T* g_
   cleanup();
   h->n = n;
   h->nnz = nnz;
-  h->n_pad = (n + 3) / 4 * 4;
   return CS_B200_OK;
+}
+
+// A caller's host CSR onto the handle (h->n rows, h->nnz entries of the handle's dtype): the index arrays go up
+// as they are and are narrowed to int32 0-based on the device, whatever their width and base.  With no rowptr
+// the arrays are only allocated (the ranks that receive the matrix by broadcast).
+int upload_host_csr(cs_b200_handle* h, const void* rowptr, const void* colidx, const void* vals, int index_bits,
+                    int index_base) {
+  const int64_t n = h->n, nnz = h->nnz;
+  CK(h, cudaMalloc(&h->d_rowptr, (size_t)(n + 1) * sizeof(int)));
+  CK(h, cudaMalloc(&h->d_colidx, std::max<size_t>(1, (size_t)nnz) * sizeof(int)));
+  CK(h, cudaMalloc(&h->d_vals, std::max<size_t>(1, (size_t)nnz) * h->esize()));
+  if (!rowptr) return CS_B200_OK;
+  if (index_bits == 32 && index_base == 0) {
+    CK(h, cudaMemcpyAsync(h->d_rowptr, rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+    CK(h, cudaMemcpyAsync(h->d_colidx, colidx, (size_t)nnz * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+  } else {
+    const size_t ib = index_bits / 8;
+    void* raw = nullptr;
+    CK(h, cudaMalloc(&raw, std::max<size_t>((size_t)(n + 1), (size_t)nnz) * ib));
+    cudaError_t e = cudaMemcpyAsync(raw, rowptr, (size_t)(n + 1) * ib, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, n + 1, h->d_rowptr);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(raw, colidx, (size_t)nnz * ib, cudaMemcpyHostToDevice, h->stream);
+    if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, nnz, h->d_colidx);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    cudaFree(raw);
+    CK(h, e);
+  }
+  CK(h, cudaMemcpyAsync(h->d_vals, vals, (size_t)nnz * h->esize(), cudaMemcpyHostToDevice, h->stream));
+  return CS_B200_OK;
+}
+
+// Level-0 aggregation seeds for the device builder, wanted under device setup with AMG and n > 200.  `job` runs
+// the seed pass on a helper thread from the caller's host pattern; `dev` holds seeds an operator source left
+// on the device instead (n + 1 ints, the last the aggregate count).
+struct Seeds {
+  bool wanted = false;
+  csb_dev::SeedJob* job = nullptr;   // the create sequence's: a source may wait on it, never free it
+  int* d_seed = nullptr;             // freed by the create sequence
+  csb_dev::DeviceSeed dev;
+};
+
+// The one create sequence behind every cs_b200_create* entry: a handle of n rows and nnz entries (0, 0 when the
+// source assembles the operator), the seed pass started before the operator arrives so that it hides behind the
+// upload, the operator from `source(h, seeds)` (it leaves d_rowptr / d_colidx / d_vals, n, nnz and owns_matrix
+// on the handle), then one of the two builders (opts.setup: 1 host, else device).  A failure's text goes to
+// cs_b200_last_error(NULL) and, if given, to *err_copy; the handle is destroyed.
+template <class Source>
+int create_handle(int64_t n, int64_t nnz, int dtype, int device, const cs_b200_opts* opts,
+                  const csb_dev::HostPattern& hp, std::string* err_copy, cs_b200_handle** out, Source&& source) {
+  cs_b200_handle* h = new cs_b200_handle();
+  h->n = n; h->nnz = nnz; h->dtype = dtype; h->device = device;
+  Seeds seeds;
+  auto finish = [&](int rc) {
+    csb_dev::seed_discard(seeds.job);
+    cudaFree(seeds.d_seed);
+    if (rc == CS_B200_OK) {
+      cudaEventRecord(h->ev1, h->stream);
+      cudaEventSynchronize(h->ev1);
+      float ms = 0;
+      cudaEventElapsedTime(&ms, h->ev0, h->ev1);
+      h->stats.setup_ms = ms;
+      *out = h;
+      return rc;
+    }
+    g_create_error = h->err;
+    if (err_copy) *err_copy = h->err;
+    cs_b200_destroy(h);
+    return rc;
+  };
+  int rc = common_create(h, opts);
+  if (rc) return finish(rc);
+  cudaEventRecord(h->ev0, h->stream);
+  const bool device_setup = h->opts.setup != 1;
+  seeds.wanted = device_setup && h->opts.precond == CS_B200_PRECOND_AMG && n > 200;
+  if (seeds.wanted && hp.rowptr) seeds.job = csb_dev::seed_start(n, hp);
+  Tick up_tick;
+  rc = source(h, seeds);
+  if (rc) return finish(rc);
+  if (up_tick.on) { cudaStreamSynchronize(h->stream); up_tick("operator on the device"); }
+  h->n_pad = (h->n + 3) / 4 * 4;
+  const bool f64 = dtype == CS_B200_F64;
+  if (device_setup) {
+    const csb_dev::DeviceSeed* dseed = seeds.d_seed ? &seeds.dev : nullptr;
+    return finish(f64 ? finish_setup_device<double>(h, hp, seeds.job, dseed)
+                      : finish_setup_device<float>(h, hp, seeds.job, dseed));
+  }
+  std::vector<int> rp((size_t)h->n + 1);
+  cudaError_t e = cudaMemcpyAsync(rp.data(), h->d_rowptr, rp.size() * sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e != cudaSuccess) return finish(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s reading rowptr", cudaGetErrorString(e)));
+  return finish(f64 ? finish_setup<double>(h, rp) : finish_setup<float>(h, rp));
 }
 
 }  // namespace
@@ -2428,98 +2485,16 @@ int cs_b200_create(int64_t n, int64_t nnz, const void* rowptr, const void* colid
   if (nnz >= (int64_t)1 << 31 || n >= (int64_t)1 << 31)
     return set_err(nullptr, CS_B200_ERR_UNSUPPORTED,
                    "n and nnz must be < 2^31 (device indices are int32)");
-  cs_b200_handle* h = new cs_b200_handle();
-  h->n = n; h->nnz = nnz; h->dtype = dtype; h->device = device;
-  int rc = common_create(h, opts);
-  if (rc) { g_create_error = h->err; cs_b200_destroy(h); return rc; }
-  auto fail = [&](int code) { g_create_error = h->err; cs_b200_destroy(h); return code; };
-  cudaEventRecord(h->ev0, h->stream);
-  const size_t es = h->esize();
-#define CKC(call)                                                                              \
-  do {                                                                                         \
-    cudaError_t _e = (call);                                                                   \
-    if (_e != cudaSuccess) {                                                                   \
-      set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (%s)", cudaGetErrorString(_e), #call);       \
-      return fail(CS_B200_ERR_CUDA);                                                           \
-    }                                                                                          \
-  } while (0)
-  if (h->opts.setup != 1) {
-    // ---- device-side setup: raw index arrays go up as they are and are narrowed on the GPU; the
-    // ordered aggregation seed pass starts right away on a helper thread (it only reads the
-    // caller's arrays) and overlaps the upload
-    const int64_t first = index_bits == 64 ? ((const int64_t*)rowptr)[0] : (int64_t)((const int32_t*)rowptr)[0];
-    const int64_t last = index_bits == 64 ? ((const int64_t*)rowptr)[n] : (int64_t)((const int32_t*)rowptr)[n];
-    if (first - index_base != 0 || last - index_base != nnz) {
-      set_err(h, CS_B200_ERR_ARG, "rowptr does not span [0, nnz] (got %lld..%lld)", (long long)(first - index_base),
-              (long long)(last - index_base));
-      return fail(CS_B200_ERR_ARG);
-    }
-    const csb_dev::HostPattern hp{rowptr, colidx, index_bits, index_base};
-    csb_dev::SeedJob* job = nullptr;
-    Tick up_tick;
-    if (h->opts.precond == CS_B200_PRECOND_AMG && n > 200) job = csb_dev::seed_start(n, hp);
-    auto fail_job = [&](int code) { csb_dev::seed_discard(job); job = nullptr; return fail(code); };
-#define CKJ(call)                                                                              \
-  do {                                                                                         \
-    cudaError_t _e = (call);                                                                   \
-    if (_e != cudaSuccess) {                                                                   \
-      set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (%s)", cudaGetErrorString(_e), #call);       \
-      return fail_job(CS_B200_ERR_CUDA);                                                       \
-    }                                                                                          \
-  } while (0)
-    CKJ(cudaMalloc(&h->d_rowptr, (size_t)(n + 1) * sizeof(int)));
-    CKJ(cudaMalloc(&h->d_colidx, std::max<size_t>(1, (size_t)nnz) * sizeof(int)));
-    CKJ(cudaMalloc(&h->d_vals, std::max<size_t>(1, (size_t)nnz) * es));
-    if (index_bits == 32 && index_base == 0) {
-      CKJ(cudaMemcpyAsync(h->d_rowptr, rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CKJ(cudaMemcpyAsync(h->d_colidx, colidx, (size_t)nnz * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    } else {
-      const size_t ib = index_bits / 8;
-      void* raw = nullptr;
-      CKJ(cudaMalloc(&raw, std::max<size_t>((size_t)(n + 1), (size_t)nnz) * ib));
-      cudaError_t e = cudaMemcpyAsync(raw, rowptr, (size_t)(n + 1) * ib, cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, n + 1, h->d_rowptr);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(raw, colidx, (size_t)nnz * ib, cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, nnz, h->d_colidx);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-      cudaFree(raw);
-      CKJ(e);
-    }
-    CKJ(cudaMemcpyAsync(h->d_vals, vals, (size_t)nnz * es, cudaMemcpyHostToDevice, h->stream));
-#undef CKJ
-    if (up_tick.on) { cudaStreamSynchronize(h->stream); up_tick("upload (narrowed on device)"); }
-    rc = dtype == CS_B200_F64 ? finish_setup_device<double>(h, hp, job) : finish_setup_device<float>(h, hp, job);
-    if (rc) return fail(rc);
-  } else {
-  std::vector<int> rp, ci;
-  if (index_bits == 64) {
-    narrow_indices((const int64_t*)rowptr, n + 1, index_base, rp);
-    narrow_indices((const int64_t*)colidx, nnz, index_base, ci);
-  } else {
-    narrow_indices((const int32_t*)rowptr, n + 1, index_base, rp);
-    narrow_indices((const int32_t*)colidx, nnz, index_base, ci);
-  }
-  if (rp[0] != 0 || rp[n] != nnz) {
-    set_err(h, CS_B200_ERR_ARG, "rowptr does not span [0, nnz] (got %d..%d)", rp[0], rp[n]);
-    return fail(CS_B200_ERR_ARG);
-  }
-  CKC(cudaMalloc(&h->d_rowptr, (size_t)(n + 1) * sizeof(int)));
-  CKC(cudaMalloc(&h->d_colidx, std::max<size_t>(1, (size_t)nnz) * sizeof(int)));
-  CKC(cudaMalloc(&h->d_vals, std::max<size_t>(1, (size_t)nnz) * es));
-  CKC(cudaMemcpyAsync(h->d_rowptr, rp.data(), (size_t)(n + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  CKC(cudaMemcpyAsync(h->d_colidx, ci.data(), (size_t)nnz * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-  CKC(cudaMemcpyAsync(h->d_vals, vals, (size_t)nnz * es, cudaMemcpyHostToDevice, h->stream));
-  rc = dtype == CS_B200_F64 ? finish_setup<double>(h, rp, &ci, (const double*)vals)
-                            : finish_setup<float>(h, rp, &ci, (const float*)vals);
-  if (rc) return fail(rc);
-  }
-  cudaEventRecord(h->ev1, h->stream);
-  cudaEventSynchronize(h->ev1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  h->stats.setup_ms = ms;
-  *out = h;
-  return CS_B200_OK;
+  // the raw values, before any narrowing: the seed pass and the device read rowptr[0 .. n] as the bounds of colidx
+  const int64_t first = index_bits == 64 ? ((const int64_t*)rowptr)[0] : (int64_t)((const int32_t*)rowptr)[0];
+  const int64_t last = index_bits == 64 ? ((const int64_t*)rowptr)[n] : (int64_t)((const int32_t*)rowptr)[n];
+  if (first - index_base != 0 || last - index_base != nnz)
+    return set_err(nullptr, CS_B200_ERR_ARG, "rowptr does not span [0, nnz] (got %lld..%lld)",
+                   (long long)(first - index_base), (long long)(last - index_base));
+  const csb_dev::HostPattern hp{rowptr, colidx, index_bits, index_base};
+  return create_handle(n, nnz, dtype, device, opts, hp, nullptr, out, [&](cs_b200_handle* h, Seeds&) -> int {
+    return upload_host_csr(h, rowptr, colidx, vals, index_bits, index_base);
+  });
 }
 
 int cs_b200_create_from_device(int64_t n, int64_t nnz, const int32_t* d_rowptr,
@@ -2530,36 +2505,13 @@ int cs_b200_create_from_device(int64_t n, int64_t nnz, const int32_t* d_rowptr,
   if (n <= 0 || nnz <= 0 || !d_rowptr || !d_colidx || !d_vals ||
       (dtype != CS_B200_F32 && dtype != CS_B200_F64) || nnz >= (int64_t)1 << 31)
     return set_err(nullptr, CS_B200_ERR_ARG, "bad arguments");
-  cs_b200_handle* h = new cs_b200_handle();
-  h->n = n; h->nnz = nnz; h->dtype = dtype; h->device = device;
-  h->owns_matrix = false;
-  int rc = common_create(h, opts);
-  if (rc) { g_create_error = h->err; cs_b200_destroy(h); return rc; }
-  cudaEventRecord(h->ev0, h->stream);
-  h->d_rowptr = const_cast<int*>(d_rowptr);
-  h->d_colidx = const_cast<int*>(d_colidx);
-  h->d_vals = const_cast<void*>(d_vals);
-  if (h->opts.setup != 1) {
-    const csb_dev::HostPattern hp{};
-    rc = dtype == CS_B200_F64 ? finish_setup_device<double>(h, hp, nullptr) : finish_setup_device<float>(h, hp, nullptr);
-  } else {
-    std::vector<int> rp(n + 1);
-    cudaError_t e = cudaMemcpy(rp.data(), d_rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) {
-      set_err(h, CS_B200_ERR_CUDA, "CUDA error %s reading rowptr", cudaGetErrorString(e));
-      g_create_error = h->err; cs_b200_destroy(h); return CS_B200_ERR_CUDA;
-    }
-    rc = dtype == CS_B200_F64 ? finish_setup<double>(h, rp, nullptr, (const double*)nullptr)
-                              : finish_setup<float>(h, rp, nullptr, (const float*)nullptr);
-  }
-  if (rc) { g_create_error = h->err; cs_b200_destroy(h); return rc; }
-  cudaEventRecord(h->ev1, h->stream);
-  cudaEventSynchronize(h->ev1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  h->stats.setup_ms = ms;
-  *out = h;
-  return CS_B200_OK;
+  return create_handle(n, nnz, dtype, device, opts, {}, nullptr, out, [&](cs_b200_handle* h, Seeds&) -> int {
+    h->owns_matrix = false;
+    h->d_rowptr = const_cast<int*>(d_rowptr);
+    h->d_colidx = const_cast<int*>(d_colidx);
+    h->d_vals = const_cast<void*>(d_vals);
+    return CS_B200_OK;
+  });
 }
 
 int cs_b200_create_from_raster(int64_t nrows, int64_t ncols, const void* g, int dtype,
@@ -2573,35 +2525,15 @@ int cs_b200_create_from_raster(int64_t nrows, int64_t ncols, const void* g, int 
     return set_err(nullptr, CS_B200_ERR_ARG, "bad arguments");
   if (nrows * ncols * 9 >= (int64_t)1 << 31)
     return set_err(nullptr, CS_B200_ERR_UNSUPPORTED, "raster too large: 9 * cells must be < 2^31 (device indices are int32)");
-  cs_b200_handle* h = new cs_b200_handle();
-  h->n = 0; h->nnz = 0; h->dtype = dtype; h->device = device;
-  h->owns_matrix = true;
-  int rc = common_create(h, opts);
-  if (rc) { g_create_error = h->err; cs_b200_destroy(h); return rc; }
-  cudaEventRecord(h->ev0, h->stream);
-  std::vector<int> rp;
-  rc = dtype == CS_B200_F64
-           ? assemble_raster<double>(h, nrows, ncols, (const double*)g, four_neighbors ? 1 : 0, avg_res ? 1 : 0, rp)
-           : assemble_raster<float>(h, nrows, ncols, (const float*)g, four_neighbors ? 1 : 0, avg_res ? 1 : 0, rp);
-  if (!rc) {
-    if (h->opts.setup != 1) {
-      const csb_dev::HostPattern hp{};
-      rc = dtype == CS_B200_F64 ? finish_setup_device<double>(h, hp, nullptr) : finish_setup_device<float>(h, hp, nullptr);
-    } else {
-      rc = dtype == CS_B200_F64 ? finish_setup<double>(h, rp, nullptr, (const double*)nullptr)
-                                : finish_setup<float>(h, rp, nullptr, (const float*)nullptr);
-    }
-  }
-  if (rc) { g_create_error = h->err; cs_b200_destroy(h); return rc; }
-  cudaEventRecord(h->ev1, h->stream);
-  cudaEventSynchronize(h->ev1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  h->stats.setup_ms = ms;
-  if (n_out) *n_out = h->n;
-  if (nnz_out) *nnz_out = h->nnz;
-  *out = h;
-  return CS_B200_OK;
+  return create_handle(0, 0, dtype, device, opts, {}, nullptr, out, [&](cs_b200_handle* h, Seeds&) -> int {
+    const int four = four_neighbors ? 1 : 0, avg = avg_res ? 1 : 0;
+    const int rc = dtype == CS_B200_F64 ? assemble_raster<double>(h, nrows, ncols, (const double*)g, four, avg)
+                                        : assemble_raster<float>(h, nrows, ncols, (const float*)g, four, avg);
+    if (rc) return rc;
+    if (n_out) *n_out = h->n;
+    if (nnz_out) *nnz_out = h->nnz;
+    return CS_B200_OK;
+  });
 }
 
 int cs_b200_create_from_raster_poly(int64_t nrows, int64_t ncols, const void* g, const int32_t* polymap,
@@ -2624,74 +2556,50 @@ int cs_b200_create_from_raster_poly(int64_t nrows, int64_t ncols, const void* g,
     }
     if (max_poly > (1 << 27)) return set_err(nullptr, CS_B200_ERR_UNSUPPORTED, "polygon ids above 2^27 are not supported");
   }
-  cs_b200_handle* h = new cs_b200_handle();
-  h->n = 0; h->nnz = 0; h->dtype = dtype; h->device = device;
-  h->owns_matrix = true;
-  int rc = common_create(h, opts);
-  auto fail = [&](int code) { g_create_error = h->err; cs_b200_destroy(h); return code; };
-  if (rc) return fail(rc);
-  cudaEventRecord(h->ev0, h->stream);
-  double* d_g = nullptr;
-  int* d_poly = nullptr;
-  int* d_node = nullptr;
-  void* d_raw = nullptr;
-  csb_dev::DCsr L;
-  auto cleanup = [&]() { cudaFree(d_g); cudaFree(d_poly); cudaFree(d_node); cudaFree(d_raw); };
-  cudaError_t e = cudaMalloc(&d_g, (size_t)ncell * sizeof(double));
-  if (e == cudaSuccess && dtype == CS_B200_F64) e = h2d(h, d_g, g, (size_t)ncell * sizeof(double));
-  if (e == cudaSuccess && dtype == CS_B200_F32) {
-    e = cudaMalloc(&d_raw, (size_t)ncell * sizeof(float));
-    if (e == cudaSuccess) e = h2d(h, d_raw, g, (size_t)ncell * sizeof(float));
-    if (e == cudaSuccess) e = (cudaError_t)csb_dev::convert_values(h->stream, (const float*)d_raw, d_g, ncell);
-  }
-  if (e == cudaSuccess && polymap) {
-    e = cudaMalloc(&d_poly, (size_t)ncell * sizeof(int));
-    if (e == cudaSuccess) e = h2d(h, d_poly, polymap, (size_t)ncell * sizeof(int));
-  }
-  if (e != cudaSuccess) { cleanup(); set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (raster upload)", cudaGetErrorString(e)); return fail(CS_B200_ERR_CUDA); }
-  rc = csb_dev::assemble_raster_polygons(h->stream, nrows, ncols, d_g, d_poly, max_poly, four_neighbors ? 1 : 0,
-                                         avg_res ? 1 : 0, L, &d_node, h->err);
-  if (rc) { cleanup(); return fail(rc == -1 ? CS_B200_ERR_ARG : rc_dev(h, rc)); }
-  h->n = L.nrows;
-  h->nnz = L.nnz;
-  h->n_pad = (h->n + 3) / 4 * 4;
-  h->d_rowptr = L.ptr;
-  h->d_colidx = L.idx;
-  if (dtype == CS_B200_F64) {
-    h->d_vals = L.val;
-  } else {
-    e = cudaMalloc(&h->d_vals, std::max<size_t>(1, (size_t)L.nnz) * sizeof(float));
-    if (e == cudaSuccess) e = (cudaError_t)csb_dev::convert_values(h->stream, L.val, (float*)h->d_vals, L.nnz);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    cudaFree(L.val);
-    if (e != cudaSuccess) { cleanup(); set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (value conversion)", cudaGetErrorString(e)); return fail(CS_B200_ERR_CUDA); }
-  }
-  if (nodemap_out) {
-    e = cudaMemcpyAsync(nodemap_out, d_node, (size_t)ncell * sizeof(int), cudaMemcpyDeviceToHost, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (e != cudaSuccess) { cleanup(); set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (node map download)", cudaGetErrorString(e)); return fail(CS_B200_ERR_CUDA); }
-  }
-  cleanup();
-  if (h->opts.setup != 1) {
-    const csb_dev::HostPattern hp{};
-    rc = dtype == CS_B200_F64 ? finish_setup_device<double>(h, hp, nullptr) : finish_setup_device<float>(h, hp, nullptr);
-  } else {
-    std::vector<int> rp((size_t)h->n + 1);
-    e = cudaMemcpy(rp.data(), h->d_rowptr, rp.size() * sizeof(int), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { set_err(h, CS_B200_ERR_CUDA, "CUDA error %s reading rowptr", cudaGetErrorString(e)); return fail(CS_B200_ERR_CUDA); }
-    rc = dtype == CS_B200_F64 ? finish_setup<double>(h, rp, nullptr, (const double*)nullptr)
-                              : finish_setup<float>(h, rp, nullptr, (const float*)nullptr);
-  }
-  if (rc) return fail(rc);
-  cudaEventRecord(h->ev1, h->stream);
-  cudaEventSynchronize(h->ev1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  h->stats.setup_ms = ms;
-  if (n_out) *n_out = h->n;
-  if (nnz_out) *nnz_out = h->nnz;
-  *out = h;
-  return CS_B200_OK;
+  return create_handle(0, 0, dtype, device, opts, {}, nullptr, out, [&](cs_b200_handle* h, Seeds&) -> int {
+    double* d_g = nullptr;
+    int* d_poly = nullptr;
+    int* d_node = nullptr;
+    void* d_raw = nullptr;
+    csb_dev::DCsr L;
+    auto cleanup = [&](int rc) { cudaFree(d_g); cudaFree(d_poly); cudaFree(d_node); cudaFree(d_raw); return rc; };
+    cudaError_t e = cudaMalloc(&d_g, (size_t)ncell * sizeof(double));
+    if (e == cudaSuccess && dtype == CS_B200_F64) e = h2d(h, d_g, g, (size_t)ncell * sizeof(double));
+    if (e == cudaSuccess && dtype == CS_B200_F32) {
+      e = cudaMalloc(&d_raw, (size_t)ncell * sizeof(float));
+      if (e == cudaSuccess) e = h2d(h, d_raw, g, (size_t)ncell * sizeof(float));
+      if (e == cudaSuccess) e = (cudaError_t)csb_dev::convert_values(h->stream, (const float*)d_raw, d_g, ncell);
+    }
+    if (e == cudaSuccess && polymap) {
+      e = cudaMalloc(&d_poly, (size_t)ncell * sizeof(int));
+      if (e == cudaSuccess) e = h2d(h, d_poly, polymap, (size_t)ncell * sizeof(int));
+    }
+    if (e != cudaSuccess) return cleanup(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (raster upload)", cudaGetErrorString(e)));
+    int rc = csb_dev::assemble_raster_polygons(h->stream, nrows, ncols, d_g, d_poly, max_poly, four_neighbors ? 1 : 0,
+                                               avg_res ? 1 : 0, L, &d_node, h->err);
+    if (rc) return cleanup(rc == -1 ? CS_B200_ERR_ARG : rc_dev(h, rc));
+    h->n = L.nrows;
+    h->nnz = L.nnz;
+    h->d_rowptr = L.ptr;
+    h->d_colidx = L.idx;
+    if (dtype == CS_B200_F64) {
+      h->d_vals = L.val;
+    } else {
+      e = cudaMalloc(&h->d_vals, std::max<size_t>(1, (size_t)L.nnz) * sizeof(float));
+      if (e == cudaSuccess) e = (cudaError_t)csb_dev::convert_values(h->stream, L.val, (float*)h->d_vals, L.nnz);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+      cudaFree(L.val);
+      if (e != cudaSuccess) return cleanup(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (value conversion)", cudaGetErrorString(e)));
+    }
+    if (nodemap_out) {
+      e = cudaMemcpyAsync(nodemap_out, d_node, (size_t)ncell * sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+      if (e != cudaSuccess) return cleanup(set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (node map download)", cudaGetErrorString(e)));
+    }
+    if (n_out) *n_out = h->n;
+    if (nnz_out) *nnz_out = h->nnz;
+    return cleanup(CS_B200_OK);
+  });
 }
 
 int cs_b200_get_csr(cs_b200_handle* h, int32_t* rowptr, int32_t* colidx, void* vals) {
@@ -2822,9 +2730,9 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   cleanup();
   if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s applying the grounds", cudaGetErrorString(e));
   teardown_operators(h);
-  const csb_dev::HostPattern none{};
-  int rc = h->dtype == CS_B200_F64 ? build_operators<double>(h, none, nullptr, nullptr)
-                                   : build_operators<float>(h, none, nullptr, nullptr);
+  csb_dev::SeedJob* no_job = nullptr;
+  int rc = h->dtype == CS_B200_F64 ? build_operators<double>(h, {}, no_job, nullptr)
+                                   : build_operators<float>(h, {}, no_job, nullptr);
   if (rc) return rc;
   cudaEventRecord(h->ev1, h->stream);
   cudaEventSynchronize(h->ev1);
@@ -3636,111 +3544,44 @@ int cs_b200_create_bcast(cs_b200_comm* c, int root, int64_t n, int64_t nnz, cons
     return comm_err(c, CS_B200_ERR_ARG, "bad create_bcast arguments");
   const bool is_root = c->rank == root;
   if (is_root && (!rowptr || !colidx || !vals)) return comm_err(c, CS_B200_ERR_ARG, "the root rank must pass the matrix");
-  cs_b200_handle* h = new cs_b200_handle();
-  h->n = n; h->nnz = nnz; h->dtype = dtype; h->device = c->device;
-  int rc = common_create(h, opts);
-  auto fail = [&](int code) { c->err = h->err; g_create_error = h->err; cs_b200_destroy(h); return code; };
-  if (rc) return fail(rc);
-  cudaEventRecord(h->ev0, h->stream);
-  const size_t es = h->esize();
-  const bool amg = h->opts.precond == CS_B200_PRECOND_AMG && n > 200 && h->opts.setup != 1;
-  csb_dev::SeedJob* job = nullptr;
-  const csb_dev::HostPattern hp{rowptr, colidx, index_bits, index_base};
-  if (is_root && amg) job = csb_dev::seed_start(n, hp);   // overlaps the upload and the broadcast
-  auto fail_job = [&](int code) { csb_dev::seed_discard(job); job = nullptr; return fail(code); };
-#define CKB(call)                                                                                  \
-  do {                                                                                             \
-    cudaError_t _e = (call);                                                                       \
-    if (_e != cudaSuccess) {                                                                       \
-      set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (%s)", cudaGetErrorString(_e), #call);           \
-      return fail_job(CS_B200_ERR_CUDA);                                                           \
-    }                                                                                              \
-  } while (0)
+  const csb_dev::HostPattern hp = is_root ? csb_dev::HostPattern{rowptr, colidx, index_bits, index_base} : csb_dev::HostPattern{};
+  return create_handle(n, nnz, dtype, c->device, opts, hp, &c->err, out, [&](cs_b200_handle* h, Seeds& seeds) -> int {
+    int rc = upload_host_csr(h, is_root ? rowptr : nullptr, colidx, vals, index_bits, index_base);
+    if (rc) return rc;
+    // one broadcast of the CSR (SURVEY.md 8e), on the handle's stream behind the upload
+    NcclApi& api = nccl_api();
+    const size_t es = h->esize();
 #define CKBN(call)                                                                                 \
   do {                                                                                             \
     int _r = (call);                                                                               \
-    if (_r != 0) {                                                                                 \
-      set_err(h, CS_B200_ERR_CUDA, "NCCL error %s (%s)", nccl_api().GetErrorString(_r), #call);    \
-      return fail_job(CS_B200_ERR_CUDA);                                                           \
-    }                                                                                              \
+    if (_r != 0) return set_err(h, CS_B200_ERR_CUDA, "NCCL error %s (%s)", api.GetErrorString(_r), #call); \
   } while (0)
-  CKB(cudaMalloc(&h->d_rowptr, (size_t)(n + 1) * sizeof(int)));
-  CKB(cudaMalloc(&h->d_colidx, (size_t)nnz * sizeof(int)));
-  CKB(cudaMalloc(&h->d_vals, (size_t)nnz * es));
-  if (is_root) {
-    if (index_bits == 32 && index_base == 0) {
-      CKB(cudaMemcpyAsync(h->d_rowptr, rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-      CKB(cudaMemcpyAsync(h->d_colidx, colidx, (size_t)nnz * sizeof(int), cudaMemcpyHostToDevice, h->stream));
-    } else {
-      const size_t ib = index_bits / 8;
-      void* raw = nullptr;
-      CKB(cudaMalloc(&raw, std::max<size_t>((size_t)(n + 1), (size_t)nnz) * ib));
-      cudaError_t e = cudaMemcpyAsync(raw, rowptr, (size_t)(n + 1) * ib, cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, n + 1, h->d_rowptr);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(raw, colidx, (size_t)nnz * ib, cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = (cudaError_t)csb_dev::narrow_indices(h->stream, raw, index_bits, index_base, nnz, h->d_colidx);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-      cudaFree(raw);
-      CKB(e);
-    }
-    CKB(cudaMemcpyAsync(h->d_vals, vals, (size_t)nnz * es, cudaMemcpyHostToDevice, h->stream));
-  }
-  // one broadcast of the CSR (SURVEY.md 8e), on the handle's stream behind the upload
-  NcclApi& api = nccl_api();
-  CKBN(api.Broadcast(h->d_rowptr, h->d_rowptr, (size_t)(n + 1), NCCL_INT32, root, c->comm, h->stream));
-  CKBN(api.Broadcast(h->d_colidx, h->d_colidx, (size_t)nnz, NCCL_INT32, root, c->comm, h->stream));
-  CKBN(api.Broadcast(h->d_vals, h->d_vals, (size_t)nnz * es, NCCL_INT8, root, c->comm, h->stream));
-  // the root's ordered aggregation seeds travel the same way (n ints) instead of every rank
-  // downloading the pattern and repeating the pass
-  int* d_seed = nullptr;
-  csb_dev::DeviceSeed ds;
-  if (amg) {
-    CKB(cudaMalloc(&d_seed, (size_t)(n + 1) * sizeof(int)));
+    CKBN(api.Broadcast(h->d_rowptr, h->d_rowptr, (size_t)(n + 1), NCCL_INT32, root, c->comm, h->stream));
+    CKBN(api.Broadcast(h->d_colidx, h->d_colidx, (size_t)nnz, NCCL_INT32, root, c->comm, h->stream));
+    CKBN(api.Broadcast(h->d_vals, h->d_vals, (size_t)nnz * es, NCCL_INT8, root, c->comm, h->stream));
+#undef CKBN
+    if (!seeds.wanted) return CS_B200_OK;
+    // the root's ordered aggregation seeds travel the same way (n ints) instead of every rank
+    // downloading the pattern and repeating the pass
+    CK(h, cudaMalloc(&seeds.d_seed, (size_t)(n + 1) * sizeof(int)));
     if (is_root) {
       const int* seed = nullptr;
       int64_t cnt = 0;
-      const int nagg = csb_dev::seed_wait(job, &seed, &cnt);
-      cudaError_t e = cudaMemcpyAsync(d_seed, seed, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = cudaMemcpyAsync(d_seed + n, &nagg, sizeof(int), cudaMemcpyHostToDevice, h->stream);
-      if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-      csb_dev::seed_discard(job);
-      job = nullptr;
-      if (e != cudaSuccess) { cudaFree(d_seed); CKB(e); }
+      const int nagg = csb_dev::seed_wait(seeds.job, &seed, &cnt);
+      CK(h, cudaMemcpyAsync(seeds.d_seed, seed, (size_t)n * sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(h, cudaMemcpyAsync(seeds.d_seed + n, &nagg, sizeof(int), cudaMemcpyHostToDevice, h->stream));
+      CK(h, cudaStreamSynchronize(h->stream));
     }
-    int r = api.Broadcast(d_seed, d_seed, (size_t)(n + 1), NCCL_INT32, root, c->comm, h->stream);
+    int r = api.Broadcast(seeds.d_seed, seeds.d_seed, (size_t)(n + 1), NCCL_INT32, root, c->comm, h->stream);
     int nagg = 0;
-    cudaError_t e = cudaMemcpyAsync(&nagg, d_seed + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+    cudaError_t e = cudaMemcpyAsync(&nagg, seeds.d_seed + n, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
     if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
-    if (r != 0 || e != cudaSuccess) {
-      cudaFree(d_seed);
-      set_err(h, CS_B200_ERR_CUDA, "broadcast of the aggregation seeds failed (%s)", r != 0 ? api.GetErrorString(r) : cudaGetErrorString(e));
-      return fail_job(CS_B200_ERR_CUDA);
-    }
-    ds.d_seed = d_seed;
-    ds.nagg = nagg;
-  }
-#undef CKB
-#undef CKBN
-  if (h->opts.setup != 1) {
-    const csb_dev::HostPattern none{};
-    rc = dtype == CS_B200_F64 ? finish_setup_device<double>(h, none, nullptr, amg ? &ds : nullptr)
-                              : finish_setup_device<float>(h, none, nullptr, amg ? &ds : nullptr);
-  } else {
-    std::vector<int> rp(n + 1);
-    cudaError_t e = cudaMemcpy(rp.data(), h->d_rowptr, (size_t)(n + 1) * sizeof(int), cudaMemcpyDeviceToHost);
-    if (e != cudaSuccess) { cudaFree(d_seed); set_err(h, CS_B200_ERR_CUDA, "CUDA error %s reading rowptr", cudaGetErrorString(e)); return fail(CS_B200_ERR_CUDA); }
-    rc = dtype == CS_B200_F64 ? finish_setup<double>(h, rp, nullptr, (const double*)nullptr)
-                              : finish_setup<float>(h, rp, nullptr, (const float*)nullptr);
-  }
-  cudaFree(d_seed);
-  if (rc) return fail(rc);
-  cudaEventRecord(h->ev1, h->stream);
-  cudaEventSynchronize(h->ev1);
-  float ms = 0;
-  cudaEventElapsedTime(&ms, h->ev0, h->ev1);
-  h->stats.setup_ms = ms;
-  *out = h;
-  return CS_B200_OK;
+    if (r != 0 || e != cudaSuccess)
+      return set_err(h, CS_B200_ERR_CUDA, "broadcast of the aggregation seeds failed (%s)", r != 0 ? api.GetErrorString(r) : cudaGetErrorString(e));
+    seeds.dev.d_seed = seeds.d_seed;
+    seeds.dev.nagg = nagg;
+    return CS_B200_OK;
+  });
 }
 
 }  // extern "C"

@@ -105,24 +105,11 @@ class Comm:
         (n, nnz, is_f64) must be known on every rank (the host broadcasts three integers)."""
         from . import _lib
         from .solver import B200Factor
-        import scipy.sparse as sp
         f = B200Factor.__new__(B200Factor)
-        f._lib = self._lib
-        f._h = C.c_void_p()
-        f.solver = solver
-        f.io_dtype = np.dtype(solver.dtype)
-        f.dtype = np.dtype(solver.device_dtype)
+        f._bind(solver)
         opts = B200Factor._opts(solver, log_transform)
         if matrix is not None:
-            m = sp.csr_matrix(matrix)
-            m.sort_indices()
-            n, nnz = m.shape[0], m.nnz
-            vals = np.ascontiguousarray(m.data, dtype=f.dtype)
-            rp = np.ascontiguousarray(m.indptr)
-            ci = np.ascontiguousarray(m.indices)
-            if ci.dtype != rp.dtype:
-                ci = ci.astype(rp.dtype)
-            bits = 64 if rp.dtype == np.int64 else 32
+            n, nnz, rp, ci, vals, bits = f._host_csr(matrix)
             args = (_lib._ptr(rp), _lib._ptr(ci), _lib._ptr(vals))
         else:
             n, nnz = int(shape[0]), int(shape[1])

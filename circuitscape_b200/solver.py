@@ -111,20 +111,26 @@ class B200Factor:
     def __init__(self, matrix, solver: CUDASolver, log_transform=False):
         self._bind(solver)
         lib = self._lib
-        m = sp.csr_matrix(matrix)
-        m.sort_indices()
-        self.n = m.shape[0]
-        vals = np.ascontiguousarray(m.data, dtype=self.dtype)
-        rowptr = np.ascontiguousarray(m.indptr)
-        colidx = np.ascontiguousarray(m.indices)
-        bits = 64 if rowptr.dtype == np.int64 else 32
-        if colidx.dtype != rowptr.dtype:
-            colidx = colidx.astype(rowptr.dtype)
+        n, nnz, rowptr, colidx, vals, bits = self._host_csr(matrix)
+        self.n = n
         opts = self._opts(solver, log_transform)
-        rc = lib.cs_b200_create(self.n, m.nnz, _lib._ptr(rowptr), _lib._ptr(colidx), _lib._ptr(vals),
+        rc = lib.cs_b200_create(n, nnz, _lib._ptr(rowptr), _lib._ptr(colidx), _lib._ptr(vals),
                                 bits, 0, _lib.dtype_code(self.dtype), solver.device,
                                 C.byref(opts), C.byref(self._h))
         _lib.check(lib, None, rc)
+
+    def _host_csr(self, matrix):
+        """`matrix` as the host CSR cs_b200_create and cs_b200_create_bcast take: (n, nnz, rowptr, colidx,
+        vals, index bits), sorted indices, the index arrays of one integer type, values contiguous in the
+        device's element type."""
+        m = sp.csr_matrix(matrix)
+        m.sort_indices()
+        vals = np.ascontiguousarray(m.data, dtype=self.dtype)
+        rowptr = np.ascontiguousarray(m.indptr)
+        colidx = np.ascontiguousarray(m.indices)
+        if colidx.dtype != rowptr.dtype:
+            colidx = colidx.astype(rowptr.dtype)
+        return m.shape[0], m.nnz, rowptr, colidx, vals, 64 if rowptr.dtype == np.int64 else 32
 
     def _bind(self, solver):
         """The attributes every factor carries before its handle is created: the library, an empty handle, the

@@ -181,12 +181,15 @@ def test_create_with_julia_style_indices(setup, bits, base):
     finally:
         lib.cs_b200_destroy(h)
     assert np.array_equal(R, R0)
-    # a rowptr that does not span [base, nnz + base] is refused, not read out of bounds
-    bad = rp.copy(); bad[-1] += 1
-    h2 = C.c_void_p()
-    rc = lib.cs_b200_create(n, A.nnz, _lib._ptr(bad), _lib._ptr(ci), _lib._ptr(va), bits, base, _lib.F64, 0,
-                            C.byref(opts), C.byref(h2))
-    assert rc == _lib.ERR_ARG and not h2.value
+    # a rowptr that does not span [base, nnz + base] is refused, not read out of bounds; a 64-bit end that is
+    # nnz + base only once narrowed to 32 bits is refused by both builders too
+    for off in ([1, 1 << 32] if bits == 64 else [1]):
+        bad = rp.copy(); bad[-1] += off
+        h2 = C.c_void_p()
+        rc = lib.cs_b200_create(n, A.nnz, _lib._ptr(bad), _lib._ptr(ci), _lib._ptr(va), bits, base, _lib.F64, 0,
+                                C.byref(opts), C.byref(h2))
+        assert rc == _lib.ERR_ARG and not h2.value
+        assert b"does not span" in lib.cs_b200_last_error(None)
 
 
 def test_from_raster_and_from_device_use_device_setup():
