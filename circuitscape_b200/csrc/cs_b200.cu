@@ -30,8 +30,10 @@ namespace {
 
 thread_local std::string g_create_error;
 
+// profile kernel classes: 0 ... 6 the SpMM epilogue MODE (kernels.cuh SP_PLAIN ... SP_ADD), then these
 constexpr int PROF_CLASSES = 20;   // cs_b200_profile_classes_n: 10 kernel classes x (fp64, fp32)
-constexpr int PROF_CGF = 8;        // class of the fused CG step (after the 8 SpMM epilogues)
+constexpr int PROF_PJ = 7;         // class of the fused prolongation + post-smoothing sweep
+constexpr int PROF_CGF = 8;        // class of the fused CG step
 constexpr int PROF_RSW = 9;        // class of the fused residual update + level-0 residual sweep
 
 struct GraphSlot {
@@ -160,8 +162,7 @@ struct cs_b200_handle {
   double prof_ms = 0.0;
   double prof_bytes = 0.0;   // algorithmic bytes of the timed launches (DESIGN.md §4 formula)
   int64_t prof_launches = 0;
-  // the same per kernel class: slot = 2 * MODE + (fp32 ? 1 : 0), MODE 7 = fused prolongation + sweep,
-  // MODE 8 = fused CG step, MODE 9 = fused residual update + level-0 residual sweep
+  // the same per kernel class (PROF_CLASSES): slot = 2 * class + (fp32 ? 1 : 0)
   std::vector<int> prof_slot;           // one entry per event pair in flight
   std::vector<double> prof_pair_bytes;
   double prof_slot_ms[PROF_CLASSES] = {}, prof_slot_bytes[PROF_CLASSES] = {};
@@ -877,12 +878,72 @@ CsrDev<T> view(const DevCsr& m) {
   return CsrDev<T>{m.rowptr, m.colidx, (const T*)m.vals, m.bstart, m.nblocks, m.nrows};
 }
 
+// The bookkeeping of one kernel launch, around the launch it scopes: the launch counters, and on profiled
+// handles an event pair with the launch's class (slot 2 * cls + fp32) and algorithmic bytes (DESIGN.md §4).
+// `timed`: a finest-level launch, counted in spmm_launches and profiled.
+struct ProfScope {
+  cs_b200_handle* h;
+  cudaEvent_t e1 = nullptr;
+  ProfScope(cs_b200_handle* h_, bool timed, int cls, bool fp32, double bytes) : h(h_) {
+    h->stats.kernel_launches++;
+    if (!timed) return;
+    h->stats.spmm_launches++;
+    if (!h->profile) return;
+    if (h->prof_used + 2 > h->prof_ev.size())
+      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
+    const cudaEvent_t e0 = h->prof_ev[h->prof_used++];
+    e1 = h->prof_ev[h->prof_used++];
+    h->prof_bytes += bytes;
+    h->prof_slot.push_back(2 * cls + (fp32 ? 1 : 0));
+    h->prof_pair_bytes.push_back(bytes);
+    cudaEventRecord(e0, h->stream);
+  }
+  ProfScope(const ProfScope&) = delete;
+  ProfScope& operator=(const ProfScope&) = delete;
+  ~ProfScope() { if (e1) cudaEventRecord(e1, h->stream); }
+};
+
+// raise Kernel's dynamic shared-memory limit to `bytes` on the handle's device, once per device (the attribute
+// lives in the device's context); each kernel instantiation keeps its own flags
+template <auto Kernel>
+void set_max_smem_once(const cs_b200_handle* h, int bytes) {
+  static bool once[64] = {};
+  bool& set = once[h->device & 63];
+  if (!set) { cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes); set = true; }
+}
+
+// grid of the stencil kernels on m (k_stencil, k_stencil_pipe, k_stencil_cg*): its tiles of NT / CGn rows by
+// ST_TC raster columns, at most grid_spmm
+template <typename T, int KT>
+int stencil_grid(const cs_b200_handle* h, const DevCsr& m) {
+  constexpr int V16 = 16 / (int)sizeof(T);
+  constexpr int CGn = KT / (KT < V16 ? KT : V16);
+  const int rpp = NT / CGn;
+  const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
+                           ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
+  return (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));
+}
+
+// one resident wave of `kernel` (NT threads, smem bytes) over the (strip of rps rows, column) steps of the stencil
+// operator m: every CTA's run of steps is as long as possible, which keeps the halo columns a CTA rebuilds at the
+// start of each run rare.  Asked per launch, on the handle's device (host-side query; the launches are captured
+// into graphs).
+template <typename Kernel>
+int wave_grid(const cs_b200_handle* h, Kernel kernel, int smem, const DevCsr& m, int rps) {
+  int occ = 0;
+  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kernel, NT, smem);
+  occ = std::max(1, occ);
+  const long long nsteps = (long long)((m.dia_nr + rps - 1) / rps) * (((long long)m.nrows + m.dia_nr - 1) / m.dia_nr);
+  return (int)std::max<long long>(1, std::min<long long>(std::min(h->grid_spmm, h->num_sms * occ), nsteps));
+}
+
+// grid of the 256-thread copy kernels (k_panel_to_cm, k_cm_to_panel, k_combine, k_fill) over nelem elements
+inline int copy_grid(size_t nelem) { return (int)std::min<size_t>(4096, (nelem + 255) / 256); }
+
 template <typename T, int KT, int MODE, bool HALF>
 void launch_stencil_pipe(cs_b200_handle* h, const DiaDev<T>& a, const T* X, T* Y, const SpmmEpi<T>& ep, int sg) {
   constexpr int SMEM = StPipe<T, KT, MODE, HALF>::D::BYTES;
-  static bool once[64] = {};   // per device: the attribute lives in the device's context
-  bool& set = once[h->device & 63];
-  if (!set) { cudaFuncSetAttribute(k_stencil_pipe<T, KT, MODE, HALF>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
+  set_max_smem_once<k_stencil_pipe<T, KT, MODE, HALF>>(h, SMEM);
   k_stencil_pipe<T, KT, MODE, HALF><<<sg, NT, SMEM, h->stream>>>(a, X, Y, ep);
 }
 
@@ -898,71 +959,42 @@ void launch_stencil(cs_b200_handle* h, const DiaDev<T>& a, const T* X, T* Y, con
   else launch_stencil_pipe<T, KT, MODE, false>(h, a, X, Y, ep, sg);
 }
 
+// the TMA-staged windowed kernel (WIDE: 4 lanes per row) on m's windowed row blocks
+template <typename T, int KT, int MODE, bool WIDE>
+void launch_spmm_win(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const SpmmEpi<T>& ep) {
+  constexpr int SMEM = WinSmem2<T, KT, MODE, WIDE>::TOTAL;
+  constexpr int SB = WinMap<T, KT, WIDE>::SB;
+  const WinCsr<T> w{m.win_meta, m.blob, m.has_dinv, m.rowptr, m.colidx, (const T*)m.vals, m.win_nblocks};
+  const int wg = std::max(1, std::min(h->num_sms, (m.win_nblocks + SB - 1) / SB));
+  set_max_smem_once<k_spmm_win<T, KT, MODE, WIDE>>(h, SMEM);
+  k_spmm_win<T, KT, MODE, WIDE><<<wg, WTT, SMEM, h->stream>>>(w, X, Y, ep);
+}
+
 // Y = op(M X) with the fused epilogue MODE (kernels.cuh).  `timed`: counts as a launch of
 // the dominant kernel for the per-launch profile (finest-level operator only).
 template <typename T, int KT, int MODE>
 void launch_spmm_on(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const T* B, const T* dinv,
                     double omega, bool timed) {
   const int grid = std::max(1, std::min(h->grid_spmm, m.nblocks));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const bool prof = h->profile && timed;
-  if (prof) {
-    if (h->prof_used + 2 > h->prof_ev.size()) {
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
-    }
-    e0 = h->prof_ev[h->prof_used++];
-    e1 = h->prof_ev[h->prof_used++];
-    // nnz (s_v + 4) + (n + 1) 4 + X once + Y once (+ B for the residual / sweep epilogues,
-    // + 1/diag for the sweeps)
-    double bytes = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 +
-                   2.0 * (double)m.nrows * KT * sizeof(T);
-    if (MODE == SP_RESNORM || MODE == SP_RES || MODE == SP_JACOBI || MODE == SP_JACOBI_DOT)
-      bytes += (double)m.nrows * KT * sizeof(T);
-    if (MODE == SP_JACOBI || MODE == SP_JACOBI_DOT) bytes += (double)m.nrows * sizeof(T);
-    h->prof_bytes += bytes;
-    h->prof_slot.push_back(2 * MODE + (sizeof(T) == 4 ? 1 : 0));
-    h->prof_pair_bytes.push_back(bytes);
-    cudaEventRecord(e0, h->stream);
-  }
+  // nnz (s_v + 4) + (n + 1) 4 + X once + Y once (+ B for the residual / sweep epilogues,
+  // + 1/diag for the sweeps)
+  double bytes = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 +
+                 2.0 * (double)m.nrows * KT * sizeof(T);
+  if (MODE == SP_RESNORM || MODE == SP_RES || MODE == SP_JACOBI || MODE == SP_JACOBI_DOT)
+    bytes += (double)m.nrows * KT * sizeof(T);
+  if (MODE == SP_JACOBI || MODE == SP_JACOBI_DOT) bytes += (double)m.nrows * sizeof(T);
+  const ProfScope prof(h, timed, MODE, sizeof(T) == 4, bytes);
   const SpmmEpi<T> ep{B, dinv, (T)omega, h->d_ctl, h->d_partials};
   if (m.dia && MODE != SP_ADD) {
-    if constexpr (MODE != SP_ADD) {
-      const DiaDev<T> a = dia_view<T>(m);
-      constexpr int V16 = 16 / (int)sizeof(T);
-      constexpr int CGn = KT / (KT < V16 ? KT : V16);
-      const int rpp = NT / CGn;
-      const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
-                               ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
-      const int sg = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));
-      launch_stencil<T, KT, MODE>(h, a, X, Y, ep, sg);
-    }
+    if constexpr (MODE != SP_ADD) launch_stencil<T, KT, MODE>(h, dia_view<T>(m), X, Y, ep, stencil_grid<T, KT>(h, m));
   } else if (m.win_meta) {
-    const WinCsr<T> w{m.win_meta, m.blob, m.has_dinv, m.rowptr, m.colidx, (const T*)m.vals, m.win_nblocks};
-    if (m.lpr == 4) {
-      constexpr int SMEM = WinSmem2<T, KT, MODE, true>::TOTAL;
-      constexpr int SB = WinMap<T, KT, true>::SB;
-      const int wg = std::max(1, std::min(h->num_sms, (m.win_nblocks + SB - 1) / SB));
-      static bool once[64] = {};   // per device: the attribute lives in the device's context
-      bool& set = once[h->device & 63];
-      if (!set) { cudaFuncSetAttribute(k_spmm_win<T, KT, MODE, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
-      k_spmm_win<T, KT, MODE, true><<<wg, WTT, SMEM, h->stream>>>(w, X, Y, ep);
-    } else {
-      constexpr int SMEM = WinSmem2<T, KT, MODE, false>::TOTAL;
-      constexpr int SB = WinMap<T, KT, false>::SB;
-      const int wg = std::max(1, std::min(h->num_sms, (m.win_nblocks + SB - 1) / SB));
-      static bool once[64] = {};
-      bool& set = once[h->device & 63];
-      if (!set) { cudaFuncSetAttribute(k_spmm_win<T, KT, MODE, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM); set = true; }
-      k_spmm_win<T, KT, MODE, false><<<wg, WTT, SMEM, h->stream>>>(w, X, Y, ep);
-    }
+    if (m.lpr == 4) launch_spmm_win<T, KT, MODE, true>(h, m, X, Y, ep);
+    else launch_spmm_win<T, KT, MODE, false>(h, m, X, Y, ep);
   } else if (m.lpr == 4 && KT * 4 <= 32) {
     k_spmm<T, KT, MODE, (KT * 4 <= 32 ? 4 : 1)><<<grid, NT, 0, h->stream>>>(view<T>(m), X, Y, ep);
   } else {
     k_spmm<T, KT, MODE, 1><<<grid, NT, 0, h->stream>>>(view<T>(m), X, Y, ep);
   }
-  if (prof) cudaEventRecord(e1, h->stream);
-  h->stats.kernel_launches++;
-  if (timed) h->stats.spmm_launches++;
 }
 
 template <typename T, int KT, int MODE>
@@ -991,18 +1023,15 @@ void harvest_profile(cs_b200_handle* h) {
 }
 
 template <typename T, int KT>
-int ew_grid(cs_b200_handle* h) {
-  const size_t nelem = (size_t)h->n_pad * KT;
-  const size_t per = (size_t)NT * Vec<T>::N;
-  return (int)std::min<size_t>(h->grid_ew, (nelem + per - 1) / per);
-}
-
-template <typename T, int KT>
 int ew_grid_n(cs_b200_handle* h, int64_t n_pad) {
   const size_t nelem = (size_t)n_pad * KT;
   const size_t per = (size_t)NT * Vec<T>::N;
   return (int)std::max<size_t>(1, std::min<size_t>(h->grid_ew, (nelem + per - 1) / per));
 }
+
+// the finest level's
+template <typename T, int KT>
+int ew_grid(cs_b200_handle* h) { return ew_grid_n<T, KT>(h, h->n_pad); }
 
 // T = B - A (omega D^-1 B) on a stencil-form level
 template <typename T, int KT>
@@ -1010,30 +1039,10 @@ void launch_stencil_res0(cs_b200_handle* h, DevLevel& L, const T* B, T* Tout, bo
   const DevCsr& m = L.A;
   const DiaDev<T> a = dia_view<T>(m);
   const SpmmEpi<T> ep{B, (const T*)L.dinv, (T)L.omega, h->d_ctl, h->d_partials};
-  constexpr int V16 = 16 / (int)sizeof(T);
-  constexpr int CGn = KT / (KT < V16 ? KT : V16);
-  const int rpp = NT / CGn;
-  const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
-                           ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
-  const int sg = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const bool prof = h->profile && timed;
-  if (prof) {
-    if (h->prof_used + 2 > h->prof_ev.size())
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
-    e0 = h->prof_ev[h->prof_used++];
-    e1 = h->prof_ev[h->prof_used++];
-    // what it replaces: the residual SpMM on A (X, B read, T written); the zero-guess sweep is folded in
-    const double fb = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 + 3.0 * (double)m.nrows * KT * sizeof(T);
-    h->prof_bytes += fb;
-    h->prof_slot.push_back(2 * (int)SP_RES + (sizeof(T) == 4 ? 1 : 0));
-    h->prof_pair_bytes.push_back(fb);
-    cudaEventRecord(e0, h->stream);
-  }
-  launch_stencil<T, KT, SP_RES0>(h, a, nullptr, Tout, ep, sg);
-  if (prof) cudaEventRecord(e1, h->stream);
-  h->stats.kernel_launches++;
-  if (timed) h->stats.spmm_launches++;
+  // what it replaces: the residual SpMM on A (X, B read, T written); the zero-guess sweep is folded in
+  const double fb = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 + 3.0 * (double)m.nrows * KT * sizeof(T);
+  const ProfScope prof(h, timed, SP_RES, sizeof(T) == 4, fb);
+  launch_stencil<T, KT, SP_RES0>(h, a, nullptr, Tout, ep, stencil_grid<T, KT>(h, m));
 }
 
 // fused upward step of a stencil-form level (kernels.cuh k_stencil_prolong_jacobi):
@@ -1048,36 +1057,14 @@ void launch_prolong_jacobi(cs_b200_handle* h, DevLevel& L, const T* Yc, const T*
   constexpr int SMEM = S::SMEM;
   constexpr int MINB = sizeof(T) == 4 ? PJ_MINB_F32 : PJ_MINB_F64;
   static_assert(SMEM <= 48 * 1024, "the strip buffers fit the default dynamic shared memory");
-  // one resident wave: every CTA's run of (strip, column) steps is as long as possible, which keeps the
-  // halo columns a CTA rebuilds at the start of each run rare
-  // asked per launch, on the handle's device (host-side query; the launches are captured into graphs)
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_stencil_prolong_jacobi<T, KT, MODE, MINB>, NT, SMEM);
-  occ = std::max(1, occ);
-  const long long nsteps = (long long)((m.dia_nr + S::RPS - 1) / S::RPS) *
-                           (((long long)m.nrows + m.dia_nr - 1) / m.dia_nr);
-  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min(h->grid_spmm, h->num_sms * occ), nsteps));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  const bool prof = h->profile && timed;
-  if (prof) {
-    if (h->prof_used + 2 > h->prof_ev.size())
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
-    e0 = h->prof_ev[h->prof_used++];
-    e1 = h->prof_ev[h->prof_used++];
-    // the two launches it replaces: SP_ADD on P (nnz_P (s+4) + (n+1) 4 + Yc + X read + X write) and the
-    // Jacobi sweep on A (nnz (s+4) + (n+1) 4 + X + Y + B + 1/diag)
-    const double fb = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 + 3.0 * (double)m.nrows * KT * sizeof(T) +
-                      (double)m.nrows * sizeof(T) + (double)L.P.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 +
-                      2.0 * (double)m.nrows * KT * sizeof(T);
-    h->prof_bytes += fb;
-    h->prof_slot.push_back(2 * 7 + (sizeof(T) == 4 ? 1 : 0));
-    h->prof_pair_bytes.push_back(fb);
-    cudaEventRecord(e0, h->stream);
-  }
+  const int grid = wave_grid(h, k_stencil_prolong_jacobi<T, KT, MODE, MINB>, SMEM, m, S::RPS);
+  // the two launches it replaces: SP_ADD on P (nnz_P (s+4) + (n+1) 4 + Yc + X read + X write) and the
+  // Jacobi sweep on A (nnz (s+4) + (n+1) 4 + X + Y + B + 1/diag)
+  const double fb = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 + 3.0 * (double)m.nrows * KT * sizeof(T) +
+                    (double)m.nrows * sizeof(T) + (double)L.P.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 +
+                    2.0 * (double)m.nrows * KT * sizeof(T);
+  const ProfScope prof(h, timed, PROF_PJ, sizeof(T) == 4, fb);
   k_stencil_prolong_jacobi<T, KT, MODE, MINB><<<grid, NT, SMEM, h->stream>>>(a, p, Yc, X0, Yout, ep);
-  if (prof) cudaEventRecord(e1, h->stream);
-  h->stats.kernel_launches++;
-  if (timed) h->stats.spmm_launches++;
 }
 
 // z = M^-1 r : one V(1,1) cycle, damped Jacobi, on panels of width KT.
@@ -1199,12 +1186,7 @@ inline bool fused_res(const cs_b200_handle* h) {
 template <typename T, int KT, typename TV, bool HALF, bool STORE_AP>
 void launch_stencil_cg_pipe(cs_b200_handle* h, const DiaDev<T>& a, const TV* Z, int sg) {
   constexpr int SMEM = StPipeCg<T, KT, TV, HALF>::D::BYTES;
-  static bool once[64] = {};
-  bool& set = once[h->device & 63];
-  if (!set) {
-    cudaFuncSetAttribute(k_stencil_cg_pipe<T, KT, TV, HALF, STORE_AP>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    set = true;
-  }
+  set_max_smem_once<k_stencil_cg_pipe<T, KT, TV, HALF, STORE_AP>>(h, SMEM);
   k_stencil_cg_pipe<T, KT, TV, HALF, STORE_AP><<<sg, NT, SMEM, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X,
                                                                             (T*)h->AP, h->d_ctl, h->d_partials);
 }
@@ -1215,27 +1197,12 @@ template <typename T, int KT, typename TV>
 void launch_stencil_cg(cs_b200_handle* h, const TV* Z, bool store_ap) {
   const DevCsr& m = h->A0;
   const DiaDev<T> a = dia_view<T>(m);
-  constexpr int V16 = 16 / (int)sizeof(T);
-  constexpr int CGn = KT / (KT < V16 ? KT : V16);
-  const int rpp = NT / CGn;
-  const long long ntiles = (long long)((m.dia_nr + rpp - 1) / rpp) *
-                           ((((long long)m.nrows + m.dia_nr - 1) / m.dia_nr + ST_TC - 1) / ST_TC);
-  const int sg = (int)std::max<long long>(1, std::min<long long>(h->grid_spmm, ntiles));   // = k_stencil<SP_CG>'s
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (h->profile) {
-    if (h->prof_used + 2 > h->prof_ev.size())
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
-    e0 = h->prof_ev[h->prof_used++];
-    e1 = h->prof_ev[h->prof_used++];
-    // 9 diagonals, Z and p_{it-1} in, AP (store_ap) and p_it out; X in + out and p_{it-2} in on every other step
-    const double pe = (double)m.nrows * KT * sizeof(T);
-    const double fb = (double)m.nrows * 9 * sizeof(T) + (double)m.nrows * KT * sizeof(TV) + (store_ap ? 3.0 : 2.0) * pe +
-                      1.5 * pe;
-    h->prof_bytes += fb;
-    h->prof_slot.push_back(2 * PROF_CGF + (sizeof(T) == 4 ? 1 : 0));
-    h->prof_pair_bytes.push_back(fb);
-    cudaEventRecord(e0, h->stream);
-  }
+  const int sg = stencil_grid<T, KT>(h, m);   // = k_stencil<SP_CG>'s
+  // 9 diagonals, Z and p_{it-1} in, AP (store_ap) and p_it out; X in + out and p_{it-2} in on every other step
+  const double pe = (double)m.nrows * KT * sizeof(T);
+  const double fb = (double)m.nrows * 9 * sizeof(T) + (double)m.nrows * KT * sizeof(TV) + (store_ap ? 3.0 : 2.0) * pe +
+                    1.5 * pe;
+  const ProfScope prof(h, true, PROF_CGF, sizeof(T) == 4, fb);
   if (stencil_pipe()) {
     if (!store_ap) {   // fused_res: fp64 with an fp32 cycle, half form
       if constexpr (sizeof(T) == 8 && sizeof(TV) == 4) launch_stencil_cg_pipe<T, KT, TV, true, false>(h, a, Z, sg);
@@ -1246,9 +1213,6 @@ void launch_stencil_cg(cs_b200_handle* h, const TV* Z, bool store_ap) {
     k_stencil_cg<T, KT, TV><<<sg, NT, 0, h->stream>>>(a, Z, (T*)h->P2, (T*)h->P, (T*)h->X, (T*)h->AP, h->d_ctl,
                                                        h->d_partials);
   }
-  if (h->profile) cudaEventRecord(e1, h->stream);
-  h->stats.kernel_launches++;
-  h->stats.spmm_launches++;
 }
 
 // r -= alpha A p, r32 = (float) r and the level-0 residual T32 of the fp32 cycle (kernels.cuh
@@ -1259,39 +1223,45 @@ void launch_res_update(cs_b200_handle* h) {
   DevLevel& L = h->lv32[0];
   using SH = RuShape<T, float, KT>;
   constexpr int SMEM = SH::D::BYTES;
-  static bool once[64] = {};
-  bool& set = once[h->device & 63];
-  if (!set) {
-    cudaFuncSetAttribute(k_stencil_res_update<T, float, KT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SMEM);
-    set = true;
-  }
-  // one resident wave, as launch_prolong_jacobi: long runs keep the halo columns rebuilt at their ends rare
-  int occ = 0;
-  cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_stencil_res_update<T, float, KT>, NT, SMEM);
-  occ = std::max(1, occ);
-  const long long nsteps = (long long)((m.dia_nr + SH::RPS - 1) / SH::RPS) *
-                           (((long long)m.nrows + m.dia_nr - 1) / m.dia_nr);
-  const int grid = (int)std::max<long long>(1, std::min<long long>(std::min(h->grid_spmm, h->num_sms * occ), nsteps));
-  cudaEvent_t e0 = nullptr, e1 = nullptr;
-  if (h->profile) {
-    if (h->prof_used + 2 > h->prof_ev.size())
-      for (int i = 0; i < 2; ++i) { cudaEvent_t e; cudaEventCreate(&e); h->prof_ev.push_back(e); }
-    e0 = h->prof_ev[h->prof_used++];
-    e1 = h->prof_ev[h->prof_used++];
-    // p, r in and r out (T), R32 and T32 out (float), the 5 upper diagonals (T), the float 1/diag
-    const double nr = (double)m.nrows;
-    const double fb = nr * KT * (3.0 * sizeof(T) + 2.0 * sizeof(float)) + nr * 5 * sizeof(T) + nr * sizeof(float);
-    h->prof_bytes += fb;
-    h->prof_slot.push_back(2 * PROF_RSW + (sizeof(T) == 4 ? 1 : 0));
-    h->prof_pair_bytes.push_back(fb);
-    cudaEventRecord(e0, h->stream);
-  }
+  set_max_smem_once<k_stencil_res_update<T, float, KT>>(h, SMEM);
+  const int grid = wave_grid(h, k_stencil_res_update<T, float, KT>, SMEM, m, SH::RPS);
+  // p, r in and r out (T), R32 and T32 out (float), the 5 upper diagonals (T), the float 1/diag
+  const double nr = (double)m.nrows;
+  const double fb = nr * KT * (3.0 * sizeof(T) + 2.0 * sizeof(float)) + nr * 5 * sizeof(T) + nr * sizeof(float);
+  const ProfScope prof(h, true, PROF_RSW, sizeof(T) == 4, fb);
   k_stencil_res_update<T, float, KT><<<grid, NT, SMEM, h->stream>>>(
       dia_view<T>(m), (const float*)L.dinv, (float)L.omega, (const T*)h->P2, (const T*)h->P,
       (T*)h->R, (T*)h->R2, (float*)h->R32, (float*)h->T32, h->d_ctl);
-  if (h->profile) cudaEventRecord(e1, h->stream);
+}
+
+// r -= alpha Ap with the finest pre-smoothing folded in, into the cycle's own precision (k_cg_update_r0): the fp32
+// r32 and x0 panels of a mixed handle, else x0 in the stage panel; no x0 where it stays implicit
+template <typename T, int KT>
+void launch_update_r0(cs_b200_handle* h) {
+  const size_t nelem = (size_t)h->n_pad * KT;
+  const int g = ew_grid<T, KT>(h);
+  if (h->mixed)
+    k_cg_update_r0<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
+                                                          (T)h->lv[0].omega, (T*)h->R,
+                                                          implicit_x0(h->lv32[0]) ? nullptr : (float*)h->X32,
+                                                          (float*)h->R32, h->d_ctl);
+  else
+    k_cg_update_r0<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv, (T)h->lv[0].omega,
+                                                      (T*)h->R, implicit_x0(h->lv[0]) ? nullptr : (T*)h->stage, nullptr,
+                                                      h->d_ctl);
   h->stats.kernel_launches++;
-  h->stats.spmm_launches++;
+}
+
+// the deferred x += alpha p with p = z + beta p (k_cg_update_xp2), z the cycle's output: Z32 on mixed handles
+template <typename T, int KT>
+void launch_update_xp2(cs_b200_handle* h) {
+  const size_t nelem = (size_t)h->n_pad * KT;
+  const int g = ew_grid<T, KT>(h);
+  if (h->mixed)
+    k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P, h->d_ctl);
+  else
+    k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
+  h->stats.kernel_launches++;
 }
 
 template <typename T, int KT>
@@ -1299,7 +1269,7 @@ void launch_iteration(cs_b200_handle* h) {
   const size_t nelem = (size_t)h->n_pad * KT;
   const int g = ew_grid<T, KT>(h);
   const bool fused = fused_cg(h);
-  const bool fres = sizeof(T) == 8 && fused_res(h);   // mixed handles are fp64 ones
+  const bool fres = sizeof(T) == 8 && fused_res(h);   // fused_res: mixed handles, which are fp64 ones
   if (fused) {
     if (h->mixed) launch_stencil_cg<T, KT, float>(h, (const float*)h->Z32, !fres);
     else launch_stencil_cg<T, KT, T>(h, (const T*)h->Z, true);
@@ -1318,33 +1288,14 @@ void launch_iteration(cs_b200_handle* h) {
     // r -= alpha Ap with the finest pre-smoothing folded in; V-cycle; then the deferred
     // x += alpha p together with p = z + beta p  (9 instead of 11 panel passes), which the fused
     // CG step of the next iteration does instead
-    if (h->mixed) {
-      if (fres) {
-        if constexpr (sizeof(T) == 8) launch_res_update<T, KT>(h);
-      } else {
-        k_cg_update_r0<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
-                                                              (T)h->lv[0].omega, (T*)h->R,
-                                                              implicit_x0(h->lv32[0]) ? nullptr : (float*)h->X32,
-                                                              (float*)h->R32, h->d_ctl);
-        h->stats.kernel_launches++;
-      }
-      launch_vcycle<T, KT>(h, true, fres);
-      mask_z<T, KT>(h);
-      if (!fused)
-        k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
-                                                               h->d_ctl);
+    if (fres) {
+      if constexpr (sizeof(T) == 8) launch_res_update<T, KT>(h);
     } else {
-      k_cg_update_r0<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->AP, (const T*)h->d_dinv,
-                                                        (T)h->lv[0].omega, (T*)h->R,
-                                                        implicit_x0(h->lv[0]) ? nullptr : (T*)h->stage, nullptr,
-                                                        h->d_ctl);
-      h->stats.kernel_launches++;
-      launch_vcycle<T, KT>(h, true);
-      mask_z<T, KT>(h);
-      if (!fused)
-        k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
+      launch_update_r0<T, KT>(h);
     }
-    if (!fused) h->stats.kernel_launches++;
+    launch_vcycle<T, KT>(h, true, fres);
+    mask_z<T, KT>(h);
+    if (!fused) launch_update_xp2<T, KT>(h);
   }
 }
 
@@ -1458,21 +1409,14 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     CK(h, cudaMemsetAsync(h->P, 0, nelem * sizeof(T), h->stream));
     CK(h, cudaMemcpyAsync(h->R, h->B, nelem * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
     k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, rtol, atol, imax, 40);
+    h->stats.kernel_launches++;
     if (h->mixed) {
       k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
-      launch_vcycle<T, KT>(h, false);
-      mask_z<T, KT>(h);
-      if (!fused)
-        k_cg_update_xp2<T, KT, float><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X, (T*)h->P,
-                                                               h->d_ctl);
       h->stats.kernel_launches++;
-    } else {
-      launch_vcycle<T, KT>(h, false);
-      mask_z<T, KT>(h);
-      if (!fused)
-        k_cg_update_xp2<T, KT, T><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->Z, (T*)h->X, (T*)h->P, h->d_ctl);
     }
-    h->stats.kernel_launches += fused ? 1 : 2;
+    launch_vcycle<T, KT>(h, false);
+    mask_z<T, KT>(h);
+    if (!fused) launch_update_xp2<T, KT>(h);
   }
   CK(h, cudaGetLastError());
   const int chunk = h->amg ? std::min(h->opts.check_every, 4) : h->opts.check_every;
@@ -1531,6 +1475,26 @@ int next_kt(int64_t remaining, int ktmax) {
     default: { constexpr int KT = 8; CALL; } break; \
   }
 
+// f(T{}) in the handle's element type T
+template <typename F>
+decltype(auto) with_type(const cs_b200_handle* h, F&& f) {
+  return h->dtype == CS_B200_F64 ? f(double{}) : f(float{});
+}
+
+// f(KT) for panel width kt (1, 2, 4, 8), KT a std::integral_constant
+template <typename F>
+decltype(auto) with_width(int kt, F&& f) {
+  DISPATCH_KT(kt, return f(std::integral_constant<int, KT>{}));
+}
+
+// f(T{}, KT): with_type, then with_width
+template <typename F>
+decltype(auto) with_type_width(const cs_b200_handle* h, int kt, F&& f) {
+  return with_type(h, [&](auto t) -> decltype(auto) {
+    return with_width(kt, [&](auto KT) -> decltype(auto) { return f(t, KT); });
+  });
+}
+
 // The column driver of the batched solve entries: walks a call's columns in panels, collects every
 // column's residual-gate and itmax status, and maps them to the call's return code.
 struct ColumnDriver {
@@ -1544,9 +1508,7 @@ struct ColumnDriver {
   int run(int64_t c_begin, int64_t c_end, Panel&& panel) {
     for (int64_t c0 = c_begin; c0 < c_end;) {
       const int kt = next_kt(c_end - c0, h->ktmax);
-      int rc = 0;
-      DISPATCH_KT(kt, (rc = panel(std::integral_constant<int, KT>{}, c0)));
-      if (rc) return rc;
+      if (int rc = with_width(kt, [&](auto KT) { return panel(KT, c0); })) return rc;
       c0 += kt;
     }
     return CS_B200_OK;
@@ -1744,7 +1706,7 @@ int upload_probe(cs_b200_handle* h, int64_t nprobe, const int64_t* probe) {
 template <typename T, int KT>
 int download_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int volt_shift) {
   CK(h, cudaGetLastError());
-  const int tg = (int)std::min<size_t>(4096, ((size_t)h->n_pad * KT + 255) / 256);
+  const int tg = copy_grid((size_t)h->n_pad * KT);
   auto download = [&](const void* panel, int shift, T* out) -> int {
     k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)panel, (T*)h->stage,
                                                     h->d_ctl, shift);
@@ -1834,7 +1796,7 @@ int point_panel(cs_b200_handle* h, int64_t x0, const int64_t* nodes, double rtol
   if (point_iters)
     for (int c = 0; c < KT; ++c) point_iters[x0 - 1 + c] = h->h_ctl->iters[c];
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int tg = copy_grid(nelem);
   k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n_pad, (const T*)h->X,
                                                   U + (size_t)(x0 - 1) * h->n_pad, h->d_ctl, 1);
   h->stats.kernel_launches += 2;
@@ -1861,7 +1823,7 @@ int combine_panel(cs_b200_handle* h, int64_t c0, const int64_t* nodes, const int
   CK(h, h2d(h, d_ci, ci, KT * sizeof(int)));
   CK(h, h2d(h, d_cj, cj, KT * sizeof(int)));
   h->stats.h2d_bytes += 2.0 * KT * sizeof(int);
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int tg = copy_grid(nelem);
   k_combine<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n_pad, U, d_ci, d_cj, (T*)h->X);
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
   k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
@@ -1915,7 +1877,7 @@ int rhs_panel(cs_b200_handle* h, int ip, int64_t c0, T* lhs, double rtol, int64_
   const int s = ip & 1;
   if (int rc = upload_ctl(h, KT, [](int) { return ColCtl{-1, -1, 0.0}; })) return rc;
   CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int tg = copy_grid(nelem);
   CK(h, cudaStreamWaitEvent(h->stream, h->ev_in[s], 0));
   k_cm_to_panel<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->io_in[s],
                                                   (T*)h->B, KT);
@@ -2212,7 +2174,7 @@ int solve_call(cs_b200_handle* h, Solve&& solve) {
   if (!h) return set_err(h, CS_B200_ERR_ARG, "null handle");
   begin_call(h);
   ColumnDriver cols{h};
-  const int rc = cols.verdict(h->dtype == CS_B200_F64 ? solve(double{}, cols) : solve(float{}, cols));
+  const int rc = cols.verdict(with_type(h, [&](auto t) { return solve(t, cols); }));
   end_call(h);
   return rc;
 }
@@ -2437,22 +2399,17 @@ template <typename T, int KT>
 int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
   const size_t bytes = (size_t)h->n * KT * sizeof(T);
   const size_t nelem = (size_t)h->n_pad * KT;
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int tg = copy_grid(nelem);
   const int g = ew_grid<T, KT>(h);
   CK(h, cudaMemcpyAsync(h->stage, r, bytes, cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaMemsetAsync(h->R, 0, nelem * sizeof(T), h->stream));
   k_cm_to_panel<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->stage, (T*)h->R, KT);
   k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, 0.0, 0.0, 1, 40);
-  const T* zp = (const T*)h->Z;
-  if (h->mixed) {
-    k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
-    launch_vcycle<T, KT>(h, false);
-    k_convert<float, T><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X);
-    zp = (const T*)h->X;
-  } else {
-    launch_vcycle<T, KT>(h, false);   // uses h->stage as its finest x: staging is done by now
-  }
-  k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, zp, (T*)h->stage, h->d_ctl, 0);
+  if (h->mixed) k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
+  launch_vcycle<T, KT>(h, false);   // the fp64 cycle uses h->stage as its finest x: staging is done by now
+  if (h->mixed) k_convert<float, T><<<g, NT, 0, h->stream>>>(nelem, (const float*)h->Z32, (T*)h->X);
+  k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)(h->mixed ? h->X : h->Z),
+                                                  (T*)h->stage, h->d_ctl, 0);
   CK(h, cudaGetLastError());
   CK(h, cudaMemcpyAsync(z, h->stage, bytes, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaMemcpyAsync(h->h_ctl, h->d_ctl, sizeof(PanelCtl), cudaMemcpyDeviceToHost, h->stream));
@@ -2714,12 +2671,10 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   }
   if (finite_g || dirichlet) {
     const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
-    if (h->dtype == CS_B200_F64)
-      k_apply_grounds<double><<<g, 256, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (double*)h->d_vals,
-                                                        (const double*)d_g, d_m);
-    else
-      k_apply_grounds<float><<<g, 256, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (float*)h->d_vals,
-                                                       (const float*)d_g, d_m);
+    with_type(h, [&](auto t) {
+      using T = decltype(t);
+      k_apply_grounds<T><<<g, 256, 0, h->stream>>>((int)h->n, h->d_rowptr, h->d_colidx, (T*)h->d_vals, (const T*)d_g, d_m);
+    });
   }
   cudaError_t e = cudaGetLastError();
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
@@ -2731,9 +2686,7 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s applying the grounds", cudaGetErrorString(e));
   teardown_operators(h);
   csb_dev::SeedJob* no_job = nullptr;
-  int rc = h->dtype == CS_B200_F64 ? build_operators<double>(h, {}, no_job, nullptr)
-                                   : build_operators<float>(h, {}, no_job, nullptr);
-  if (rc) return rc;
+  if (int rc = with_type(h, [&](auto t) { return build_operators<decltype(t)>(h, {}, no_job, nullptr); })) return rc;
   cudaEventRecord(h->ev1, h->stream);
   cudaEventSynchronize(h->ev1);
   float ms = 0;
@@ -2785,10 +2738,10 @@ int cs_b200_reset_currents(cs_b200_handle* h) {
   cudaSetDevice(h->device);
   CK(h, cudaMemsetAsync(h->d_cum, 0, (size_t)h->n_pad * h->esize(), h->stream));
   const int g = (int)std::min<int64_t>(4096, (h->n_pad + 255) / 256);
-  if (h->dtype == CS_B200_F64)
-    k_fill<double><<<g, 256, 0, h->stream>>>((double*)h->d_max, (size_t)h->n_pad, -9999.0);
-  else
-    k_fill<float><<<g, 256, 0, h->stream>>>((float*)h->d_max, (size_t)h->n_pad, -9999.0f);
+  with_type(h, [&](auto t) {
+    using T = decltype(t);
+    k_fill<T><<<g, 256, 0, h->stream>>>((T*)h->d_max, (size_t)h->n_pad, T(-9999));
+  });
   if (h->d_cum_branch)
     CK(h, cudaMemsetAsync(h->d_cum_branch, 0, (size_t)std::max<int64_t>(h->nb, 1) * h->esize(), h->stream));
   CK(h, cudaGetLastError());
@@ -2861,12 +2814,10 @@ int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
   const int ge = (int)std::max<int64_t>(1, std::min<int64_t>((h->nnz / CHUNK + 255) / 256, (int64_t)h->num_sms * 32));
   const void* vals = h->d_vals0 ? h->d_vals0 : h->d_vals;    // pristine values: grounds do not split
   k_cc_init<<<g, 256, 0, h->stream>>>(n, parent);
-  if (h->dtype == CS_B200_F64)
-    k_cc_hook<double><<<ge, 256, 0, h->stream>>>(n, (int)h->nnz, h->d_rowptr, h->d_colidx, (const double*)vals,
-                                                 parent, CHUNK);
-  else
-    k_cc_hook<float><<<ge, 256, 0, h->stream>>>(n, (int)h->nnz, h->d_rowptr, h->d_colidx, (const float*)vals,
-                                                parent, CHUNK);
+  with_type(h, [&](auto t) {
+    using T = decltype(t);
+    k_cc_hook<T><<<ge, 256, 0, h->stream>>>(n, (int)h->nnz, h->d_rowptr, h->d_colidx, (const T*)vals, parent, CHUNK);
+  });
   k_cc_compress<<<g, 256, 0, h->stream>>>(n, parent, lab, root);
   cudaError_t e = cub::DeviceScan::ExclusiveSum(s + off_tmp, tb, root, idx, n, h->stream);
   int total = 0, last_flag = 0;
@@ -2947,12 +2898,10 @@ int cs_b200_spmv(cs_b200_handle* h, const void* x, void* y, int reps, double* ms
   const size_t bytes = (size_t)h->n * h->esize();
   CK(h, cudaMemcpyAsync(h->X, x, bytes, cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaEventRecord(h->ev2, h->stream));
-  for (int r = 0; r < reps; ++r) {
-    if (h->dtype == CS_B200_F64)
-      launch_spmm<double, 1, 0>(h, (const double*)h->X, (double*)h->AP, nullptr);
-    else
-      launch_spmm<float, 1, 0>(h, (const float*)h->X, (float*)h->AP, nullptr);
-  }
+  with_type(h, [&](auto t) {
+    using T = decltype(t);
+    for (int r = 0; r < reps; ++r) launch_spmm<T, 1, SP_PLAIN>(h, (const T*)h->X, (T*)h->AP, nullptr);
+  });
   CK(h, cudaGetLastError());
   CK(h, cudaEventRecord(h->ev3, h->stream));
   CK(h, cudaMemcpyAsync(y, h->AP, bytes, cudaMemcpyDeviceToHost, h->stream));
@@ -2973,22 +2922,22 @@ int cs_b200_spmm(cs_b200_handle* h, int k, const void* x, void* y) {
   begin_call(h);
   const size_t bytes = (size_t)h->n * k * h->esize();
   const size_t nelem = (size_t)h->n_pad * k;
-  const int tg = (int)std::min<size_t>(4096, (nelem + 255) / 256);
+  const int tg = copy_grid(nelem);
   CK(h, cudaMemcpyAsync(h->stage, x, bytes, cudaMemcpyHostToDevice, h->stream));
   CK(h, cudaMemsetAsync(h->X, 0, nelem * h->esize(), h->stream));
-  const bool f64 = h->dtype == CS_B200_F64;
-  if (f64) { DISPATCH_KT(k, (k_cm_to_panel<double, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const double*)h->stage, (double*)h->X, KT))); }
-  else { DISPATCH_KT(k, (k_cm_to_panel<float, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const float*)h->stage, (float*)h->X, KT))); }
-  if (add) {
-    CK(h, cudaMemcpyAsync(h->AP, h->X, nelem * h->esize(), cudaMemcpyDeviceToDevice, h->stream));
-    if (f64) { DISPATCH_KT(k, (launch_spmm<double, KT, SP_ADD>(h, (const double*)h->X, (double*)h->AP, (const double*)h->AP))); }
-    else { DISPATCH_KT(k, (launch_spmm<float, KT, SP_ADD>(h, (const float*)h->X, (float*)h->AP, (const float*)h->AP))); }
-  } else {
-  if (f64) { DISPATCH_KT(k, (launch_spmm<double, KT, SP_PLAIN>(h, (const double*)h->X, (double*)h->AP, nullptr))); }
-  else { DISPATCH_KT(k, (launch_spmm<float, KT, SP_PLAIN>(h, (const float*)h->X, (float*)h->AP, nullptr))); }
-  }
-  if (f64) { DISPATCH_KT(k, (k_panel_to_cm<double, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const double*)h->AP, (double*)h->stage, h->d_ctl, 0))); }
-  else { DISPATCH_KT(k, (k_panel_to_cm<float, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const float*)h->AP, (float*)h->stage, h->d_ctl, 0))); }
+  const int rc = with_type_width(h, k, [&](auto t, auto KT) -> int {
+    using T = decltype(t);
+    k_cm_to_panel<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->stage, (T*)h->X, KT);
+    if (add) {
+      CK(h, cudaMemcpyAsync(h->AP, h->X, nelem * h->esize(), cudaMemcpyDeviceToDevice, h->stream));
+      launch_spmm<T, KT, SP_ADD>(h, (const T*)h->X, (T*)h->AP, (const T*)h->AP);
+    } else {
+      launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->AP, nullptr);
+    }
+    k_panel_to_cm<T, KT><<<tg, 256, 0, h->stream>>>((int)h->n, (size_t)h->n, (const T*)h->AP, (T*)h->stage, h->d_ctl, 0);
+    return CS_B200_OK;
+  });
+  if (rc) return rc;
   CK(h, cudaGetLastError());
   CK(h, cudaMemcpyAsync(y, h->stage, bytes, cudaMemcpyDeviceToHost, h->stream));
   CK(h, cudaStreamSynchronize(h->stream));
@@ -3001,9 +2950,7 @@ int cs_b200_apply_precond(cs_b200_handle* h, int k, const void* r, void* z, doub
     return set_err(h, CS_B200_ERR_ARG, "bad apply_precond arguments");
   if (!h->amg) return set_err(h, CS_B200_ERR_UNSUPPORTED, "apply_precond: the handle has no multigrid preconditioner");
   begin_call(h);
-  int rc = CS_B200_OK;
-  if (h->dtype == CS_B200_F64) { DISPATCH_KT(k, (rc = apply_precond_t<double, KT>(h, r, z, rz))); }
-  else { DISPATCH_KT(k, (rc = apply_precond_t<float, KT>(h, r, z, rz))); }
+  const int rc = with_type_width(h, k, [&](auto t, auto KT) { return apply_precond_t<decltype(t), KT>(h, r, z, rz); });
   end_call(h);
   return rc;
 }
@@ -3014,13 +2961,16 @@ int cs_b200_bench_spmm(cs_b200_handle* h, int k, int reps, int flush_l2, double*
   begin_call(h);
   if (flush_l2) { int rc = ensure_flush(h); if (rc) return rc; }
   const size_t pe = (size_t)h->n_pad * k;
-  const int g = (int)std::min<size_t>(4096, (pe + 255) / 256);
-  if (h->dtype == CS_B200_F64) k_fill<double><<<g, 256, 0, h->stream>>>((double*)h->X, pe, 1.0);
-  else k_fill<float><<<g, 256, 0, h->stream>>>((float*)h->X, pe, 1.0f);
+  with_type(h, [&](auto t) {
+    using T = decltype(t);
+    k_fill<T><<<copy_grid(pe), 256, 0, h->stream>>>((T*)h->X, pe, T(1));
+  });
   double total = 0;
   auto one = [&]() {
-    if (h->dtype == CS_B200_F64) { DISPATCH_KT(k, (launch_spmm<double, KT, 0>(h, (const double*)h->X, (double*)h->AP, nullptr))); }
-    else { DISPATCH_KT(k, (launch_spmm<float, KT, 0>(h, (const float*)h->X, (float*)h->AP, nullptr))); }
+    with_type_width(h, k, [&](auto t, auto KT) {
+      using T = decltype(t);
+      launch_spmm<T, KT, SP_PLAIN>(h, (const T*)h->X, (T*)h->AP, nullptr);
+    });
   };
   one();  // warm-up
   if (flush_l2) {
@@ -3065,15 +3015,18 @@ int cs_b200_bench_cg_iter(cs_b200_handle* h, int k, int reps, double* ms_per_rep
   CK(h, cudaMemcpyAsync(h->d_ctl, hc, sizeof(PanelCtl), cudaMemcpyHostToDevice, h->stream));
   const size_t nelem = (size_t)h->n_pad * k;
   CK(h, cudaMemsetAsync(h->B, 0, nelem * h->esize(), h->stream));
-  const bool f64 = h->dtype == CS_B200_F64;
-#define BOTH(CALLD, CALLF) do { if (f64) { DISPATCH_KT(k, CALLD); } else { DISPATCH_KT(k, CALLF); } } while (0)
-  BOTH((k_pair_rhs<double, KT><<<1, 32, 0, h->stream>>>((double*)h->B, h->d_ctl)),
-       (k_pair_rhs<float, KT><<<1, 32, 0, h->stream>>>((float*)h->B, h->d_ctl)));
-  BOTH((k_cg_init<double, KT><<<ew_grid<double, KT>(h), NT, 0, h->stream>>>(nelem, (const double*)h->B, (const double*)h->d_dinv, (double*)h->X, (double*)h->R, (double*)h->P, h->d_ctl, h->d_partials, 0.0, 0.0, 1 << 30)),
-       (k_cg_init<float, KT><<<ew_grid<float, KT>(h), NT, 0, h->stream>>>(nelem, (const float*)h->B, (const float*)h->d_dinv, (float*)h->X, (float*)h->R, (float*)h->P, h->d_ctl, h->d_partials, 0.0, 0.0, 1 << 30)));
-  for (int w = 0; w < 3; ++w) BOTH((launch_iteration<double, KT>(h)), (launch_iteration<float, KT>(h)));
-  CK(h, cudaEventRecord(h->ev2, h->stream));
-  for (int r = 0; r < reps; ++r) BOTH((launch_iteration<double, KT>(h)), (launch_iteration<float, KT>(h)));
+  const int rc = with_type_width(h, k, [&](auto t, auto KT) -> int {
+    using T = decltype(t);
+    k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
+    k_cg_init<T, KT><<<ew_grid<T, KT>(h), NT, 0, h->stream>>>(nelem, (const T*)h->B, (const T*)h->d_dinv, (T*)h->X,
+                                                              (T*)h->R, (T*)h->P, h->d_ctl, h->d_partials, 0.0, 0.0,
+                                                              1 << 30);
+    for (int w = 0; w < 3; ++w) launch_iteration<T, KT>(h);
+    CK(h, cudaEventRecord(h->ev2, h->stream));
+    for (int r = 0; r < reps; ++r) launch_iteration<T, KT>(h);
+    return CS_B200_OK;
+  });
+  if (rc) return rc;
   CK(h, cudaEventRecord(h->ev3, h->stream));
   CK(h, cudaEventSynchronize(h->ev3));
   CK(h, cudaGetLastError());

@@ -13,7 +13,11 @@ output and with volt, curr, accumulate, weights (and probe rows).  One configura
 entry at rtol 0.5 / itmax 1 (residual gate) and rtol 1e-14 / itmax 12 (itmax stop), and one region
 pair has no conducting path.
 
+With --profile every call runs once more with the per-launch profile on, and its record also holds the
+profile's accounting: per kernel class the algorithmic bytes and launches, and profile_bytes() (no times).
+
     python profiles/entry_digest.py --out digest.jsonl          # one JSON line per call
+    python profiles/entry_digest.py --profile --out digest.jsonl
     python profiles/entry_digest.py --compare a.jsonl b.jsonl   # differences between two runs; exit 1 if any
 """
 import argparse
@@ -95,7 +99,7 @@ def calls(x, full, **lim):
                                               probe=x["probe"] if full else None, **opt, **lim), full)]
 
 
-def run_call(f, method, kw, accumulates):
+def run_call(f, method, kw, accumulates, profile=False):
     rec = {}
     try:
         out = getattr(f, method)(**kw)
@@ -111,10 +115,21 @@ def run_call(f, method, kw, accumulates):
         cum, mx = f.read_currents()
         rec["maps"] = [digest(cum), digest(mx)]
         f.reset_currents()
+    if profile:
+        f.profile_spmm(True)
+        try:
+            getattr(f, method)(**kw)
+        except Exception:                                    # noqa: BLE001 -- recorded above
+            pass
+        rec["profile"] = dict(classes={c: [b, n] for c, (_, b, n) in sorted(f.profile_classes().items())},
+                              bytes=f.profile_bytes())
+        f.profile_spmm(False)
+        if accumulates:
+            f.reset_currents()
     return rec
 
 
-def run(out_path):
+def run(out_path, profile=False):
     import circuitscape_b200 as cb
     from circuitscape_b200 import solver as S
     with open(out_path, "w") as fh:
@@ -130,12 +145,12 @@ def run(out_path):
                         for full in (False, True):
                             for name, method, kw, acc in calls(x, full):
                                 case = f"{oname}({form})/{cname}/{loop}/{'full' if full else 'bare'}/{name}"
-                                emit(case, run_call(f, method, kw, acc))
+                                emit(case, run_call(f, method, kw, acc, profile))
                         if oname == "stencil" and cname == "f64" and loop is True:
                             for tag, lim in (("gate", dict(rtol=0.5, itmax=1)), ("itmax", dict(rtol=1e-14, itmax=12))):
                                 for name, method, kw, acc in calls(x, True, **lim):
                                     kw.setdefault("raise_on_residual", False)
-                                    emit(f"{oname}/{cname}/{tag}/{name}", run_call(f, method, kw, acc))
+                                    emit(f"{oname}/{cname}/{tag}/{name}", run_call(f, method, kw, acc, profile))
         # a region pair with no conducting path: set 2 is a 2 x 2 island of unit conductance (4 neighbours),
         # so L 1 is exactly zero on it and the flux into it is exactly zero
         g = 1.0 / np.random.default_rng(8).uniform(1.0, 10.0, size=(60, 50))
@@ -146,7 +161,7 @@ def run(out_path):
             sets = [np.sort(nodemap[r0:r0 + 5, c0:c0 + 5].ravel() - 1) for r0, c0 in ((0, 0), (30, 0))]
             sets.append(np.sort(nodemap[49:51, 39:41].ravel() - 1))
             kw = dict(sets=sets, set_a=np.array([0, 0, 1]), set_b=np.array([1, 2, 2]), want_volt=True)
-            emit("split/region_no_path", run_call(f, "solve_region_pairs", kw, False))
+            emit("split/region_no_path", run_call(f, "solve_region_pairs", kw, False, profile))
 
 
 def compare(a_path, b_path):
@@ -162,7 +177,7 @@ def compare(a_path, b_path):
     for case in sorted(set(a) & set(b)):
         ra, rb = a[case], b[case]
         ended[ra["ended"].split(":")[0]] = ended.get(ra["ended"].split(":")[0], 0) + 1
-        for key in ("ended", "last_error", "arrays", "maps"):
+        for key in ("ended", "last_error", "arrays", "maps", "profile"):
             if ra.get(key) != rb.get(key):
                 print("DIFF", case, key, ra.get(key), rb.get(key))
                 diffs += 1
@@ -181,8 +196,9 @@ if __name__ == "__main__":
     ap = argparse.ArgumentParser()
     ap.add_argument("--out")
     ap.add_argument("--compare", nargs=2)
+    ap.add_argument("--profile", action="store_true", help="also record the per-class profile accounting")
     args = ap.parse_args()
     if args.compare:
         sys.exit(1 if compare(*args.compare) else 0)
     else:
-        run(args.out)
+        run(args.out, args.profile)
