@@ -818,6 +818,69 @@ def compute_omniscape_currents(conductances, sources, grounds, cs_cfg, want_volt
     return out
 
 
+@dataclass
+class MovingWindowMap:
+    """Result of moving_window_current_map."""
+    current: np.ndarray            # (nrows, ncols) float64: the windows' currents summed at their positions
+    iterations: np.ndarray         # per window, as OmniscapeBatch.iterations
+    relres: np.ndarray             # per window, as OmniscapeBatch.relres
+
+
+def moving_window_current_map(conductance, source, targets, radius, cs_cfg, *, source_scale=None, ground=np.inf,
+                              circular=True, solver=None, max_batch_bytes=1 << 30) -> MovingWindowMap:
+    """Omniscape's moving-window loop on the device (cs_b200_solve_moving_windows): for every target, the
+    (2 radius + 1)^2 window centred on it is cut from the landscape, solved as compute_omniscape_current
+    solves it, and its current raster is added into one landscape map at the window's position, in target
+    order, in float64.
+
+    conductance / source: 2-D landscape rasters of one shape, row-major (NODATA, 0 and NaN conductance =
+    no node).  targets: (nwin, 2) 0-based (row, col) cells of the landscape.  A window cell is a node when
+    it lies inside the landscape on a node and, with `circular`, within distance `radius` of the target.
+    The window's sources are source_scale[w] * source there; its only ground is `ground[w]` (a conductance,
+    > 0; Inf = direct ground) at the target.  source_scale / ground: None / a scalar / one value per target.
+    Settings (`connect_four_neighbors_only`, rtol, itmax, device) are those of compute_omniscape_currents;
+    float32 rasters stay float32 on the way in when both are float32.  Windows go to the device in batches
+    of at most `max_batch_bytes` (S.advanced_batch_bytes per window, at least one window); the map does not
+    depend on the split.  A window whose component fails the 1e-4 gate raises SolverResidualError naming
+    it (`.window`)."""
+    g, s = np.asarray(conductance), np.asarray(source)
+    for a, name in ((g, "conductance"), (s, "source")):
+        if a.ndim != 2 or a.size == 0 or not (np.issubdtype(a.dtype, np.number) or a.dtype == bool):
+            raise ValueError(f"{name}: expected a non-empty numeric 2-D raster, got shape {a.shape} dtype {a.dtype}")
+    if g.shape != s.shape:
+        raise ValueError(f"conductance {g.shape} and source {s.shape} differ")
+    t = np.asarray(targets)
+    if t.size == 0:
+        t = t.reshape(0, 2)
+    if t.ndim != 2 or t.shape[1] != 2 or not np.issubdtype(t.dtype, np.integer):
+        raise ValueError(f"targets: expected an integer (nwin, 2) array of (row, col), got shape {t.shape} "
+                         f"dtype {t.dtype}")
+    nwin = len(t)
+
+    def per_window(v, name):
+        a = np.asarray(v, dtype=np.float64)
+        if a.ndim == 0:
+            return np.full(nwin, float(a))
+        if a.shape != (nwin,):
+            raise ValueError(f"{name}: expected a scalar or {nwin} values, got shape {a.shape}")
+        return a
+
+    scale = None if source_scale is None else per_window(source_scale, "source_scale")
+    gnd = per_window(ground, "ground")
+    if max_batch_bytes <= 0:
+        raise ValueError("max_batch_bytes must be positive")
+    solver = solver if solver is not None else get_solver(cs_cfg)
+    dtype = np.float32 if g.dtype == np.float32 and s.dtype == np.float32 else np.float64
+    res = S.solve_moving_windows(g.astype(dtype, copy=False), s.astype(dtype, copy=False), t[:, 0], t[:, 1],
+                                 radius, circular, scale, gnd, _flag(cs_cfg, "connect_four_neighbors_only"),
+                                 solver.device, solver.rtol, solver.itmax, max_batch_bytes)
+    if res["rc"] == _lib.ERR_RESIDUAL:
+        err = S.SolverResidualError(res["msg"])
+        err.window = res["first_failed"]
+        raise err
+    return MovingWindowMap(res["cum"], res["iters"], res["relres"])
+
+
 def resolve_conflicts(sources, grounds, policy):
     """src/raster/advanced.jl:119-149 (`rmvall` only zeroes the sources -- pinned upstream by
     test/internal.jl:130-135)."""

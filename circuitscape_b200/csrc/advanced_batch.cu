@@ -24,7 +24,9 @@
 #include <cuda_runtime.h>
 
 #include <cub/block/block_scan.cuh>
+#include <cub/device/device_radix_sort.cuh>
 
+#include <algorithm>
 #include <climits>
 #include <cmath>
 #include <cstdarg>
@@ -373,6 +375,226 @@ cudaError_t launch(int nwin, Shape s, const void* g, const void* src, const void
 
 size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 
+// ---------------------------------------------------------------------------------------------------
+// Moving windows cut from one resident landscape (cs_b200_solve_moving_windows).  Per batch of
+// consecutive windows: k_window_cut writes the g / src / gnd stacks k_advanced_batch reads, the batch
+// is solved, and k_window_accumulate adds the staged currents into the landscape map.  The map is
+// split into TILE x TILE tiles; each tile is one CTA that owns its cells and adds the windows touching
+// it in window order, from lists built expand - sort - compress: every window writes (tile, window)
+// for the tiles its square overlaps (k_window_tiles), a stable radix sort by tile keeps window order
+// inside a tile, and k_tile_bounds marks where each tile's run starts and ends.  The map stays on the
+// device across batches and each cell is one fixed chain of fp64 adds from +0.0, so the result does
+// not depend on the batch split.
+// ---------------------------------------------------------------------------------------------------
+constexpr int TILE = 32;
+constexpr int TILE_COLS = BT / TILE;            // tile columns one CTA pass covers
+constexpr int TILE_PASSES = TILE / TILE_COLS;   // cells per thread
+
+struct Land {
+  int nrows, ncols;    // landscape, column-major
+  int radius, side;    // side = 2 radius + 1
+  int circular;
+  int tiles_r, ntiles; // tiles down a column, tiles in all
+  int span;            // most tiles a window overlaps along one axis
+};
+
+// window w's g / src / gnd in k_advanced_batch's layout (window-major, column-major inside)
+template <typename T>
+__global__ void __launch_bounds__(BT)
+k_window_cut(Land L, int w0, const T* __restrict__ G, const T* __restrict__ S, const int* __restrict__ trow,
+             const int* __restrict__ tcol, const double* __restrict__ scale, const double* __restrict__ gnd,
+             T* __restrict__ g_all, T* __restrict__ src_all, T* __restrict__ gnd_all) {
+  const int w = w0 + blockIdx.x, R = L.radius, W = L.side, n = W * W;
+  const int r0 = trow[w] - R, c0 = tcol[w] - R;
+  const double sc = scale ? scale[w] : 1.0;
+  const T gc = gnd ? (T)gnd[w] : (T)INFINITY;
+  const int64_t base = (int64_t)blockIdx.x * n;
+  for (int i = threadIdx.x; i < n; i += BT) {
+    const int dr = i % W - R, dc = i / W - R, r = r0 + R + dr, c = c0 + R + dc;
+    T gv = 0, sv = 0, nv = 0;
+    if (r >= 0 && r < L.nrows && c >= 0 && c < L.ncols && (!L.circular || dr * dr + dc * dc <= R * R)) {
+      const int64_t j = (int64_t)c * L.nrows + r;
+      const T gl = G[j];
+      if ((double)gl > 0.0) {
+        gv = gl;
+        sv = (T)(sc * (double)S[j]);
+        if (dr == 0 && dc == 0) nv = gc;
+      }
+    }
+    g_all[base + i] = gv;
+    src_all[base + i] = sv;
+    gnd_all[base + i] = nv;
+  }
+}
+
+// (tile, window-in-batch) for every tile window w0 + wl overlaps; span^2 slots per window, the unused
+// ones keyed ntiles so that they sort behind every tile
+__global__ void k_window_tiles(Land L, int w0, int nb, const int* __restrict__ trow, const int* __restrict__ tcol,
+                               unsigned* __restrict__ key, int* __restrict__ val) {
+  const int per = L.span * L.span;
+  const int64_t p = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (p >= (int64_t)nb * per) return;
+  const int wl = (int)(p / per), k = (int)(p % per), w = w0 + wl;
+  const int r0 = max(trow[w] - L.radius, 0), r1 = min(trow[w] + L.radius, L.nrows - 1);
+  const int c0 = max(tcol[w] - L.radius, 0), c1 = min(tcol[w] + L.radius, L.ncols - 1);
+  const int ti = r0 / TILE + k % L.span, tj = c0 / TILE + k / L.span;
+  key[p] = (ti <= r1 / TILE && tj <= c1 / TILE) ? (unsigned)(ti + tj * L.tiles_r) : (unsigned)L.ntiles;
+  val[p] = wl;
+}
+
+// run [beg[t], end[t]) of tile t in the sorted pairs (beg = end = 0 for a tile no window touches)
+__global__ void k_tile_bounds(int np, const unsigned* __restrict__ key, unsigned ntiles, int* __restrict__ beg,
+                              int* __restrict__ end) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= np) return;
+  const unsigned k = key[i];
+  if (k >= ntiles) return;
+  if (i == 0 || key[i - 1] != k) beg[k] = i;
+  if (i == np - 1 || key[i + 1] != k) end[k] = i + 1;
+}
+
+// one CTA per tile: each thread owns TILE_PASSES cells of the tile and adds the staged window currents
+// of the tile's windows in window order
+__global__ void __launch_bounds__(BT)
+k_window_accumulate(Land L, int w0, const int* __restrict__ trow, const int* __restrict__ tcol,
+                    const int* __restrict__ beg, const int* __restrict__ end, const int* __restrict__ wins,
+                    const double* __restrict__ cur_all, double* __restrict__ cum) {
+  const int t = blockIdx.x, b = beg[t], e = end[t];
+  if (b == e) return;
+  const int W = L.side, n = W * W;
+  const int r = (t % L.tiles_r) * TILE + threadIdx.x % TILE;
+  const int cbase = (t / L.tiles_r) * TILE + threadIdx.x / TILE;
+  const bool rin = r < L.nrows;
+  double acc[TILE_PASSES];
+#pragma unroll
+  for (int k = 0; k < TILE_PASSES; ++k) {
+    const int c = cbase + k * TILE_COLS;
+    acc[k] = rin && c < L.ncols ? cum[(int64_t)c * L.nrows + r] : 0.0;
+  }
+  for (int q = b; q < e; ++q) {
+    const int wl = wins[q], w = w0 + wl;
+    const int dr = r - (trow[w] - L.radius), dc0 = cbase - (tcol[w] - L.radius);
+    const double* __restrict__ cur = cur_all + (int64_t)wl * n;
+#pragma unroll
+    for (int k = 0; k < TILE_PASSES; ++k) {
+      const int dc = dc0 + k * TILE_COLS;
+      if (rin && cbase + k * TILE_COLS < L.ncols && dr >= 0 && dr < W && dc >= 0 && dc < W)
+        acc[k] += cur[dr + dc * W];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < TILE_PASSES; ++k) {
+    const int c = cbase + k * TILE_COLS;
+    if (rin && c < L.ncols) cum[(int64_t)c * L.nrows + r] = acc[k];
+  }
+}
+
+// device buffers of one call, freed when it returns
+struct DevBufs {
+  std::vector<void*> ptrs;
+  ~DevBufs() {
+    for (void* q : ptrs) cudaFree(q);
+  }
+  template <typename X>
+  cudaError_t get(X** out, size_t count) {
+    void* q = nullptr;
+    const cudaError_t e = cudaMalloc(&q, count ? count * sizeof(X) : 1);
+    if (e == cudaSuccess) ptrs.push_back(q);
+    *out = (X*)q;
+    return e;
+  }
+};
+
+struct Stream {
+  cudaStream_t s = nullptr;
+  ~Stream() {
+    if (s) cudaStreamDestroy(s);
+  }
+};
+
+#define CKM(call)                                                                                \
+  do {                                                                                           \
+    cudaError_t _e = (call);                                                                     \
+    if (_e != cudaSuccess)                                                                       \
+      return set_err(CS_B200_ERR_CUDA, "CUDA error %s at %s:%d (%s)", cudaGetErrorString(_e), \
+                     __FILE__, __LINE__, #call);                                                 \
+  } while (0)
+
+// the batches of cs_b200_solve_moving_windows; wo receives every window's WinOut
+template <typename T>
+int moving_windows(const Land& L, int nwin, int bw, const void* g, const void* src, const std::vector<int>& trow,
+                   const std::vector<int>& tcol, const double* scale, const double* gnd, int four, double rtol,
+                   long long itmax, double* cum, std::vector<WinOut>& wo) {
+  const size_t cells = (size_t)L.nrows * L.ncols, ncell = (size_t)L.side * L.side, per = (size_t)L.span * L.span;
+  const Shape s{L.side, L.side, (int)ncell, four};
+  const double atol = std::sqrt(2.220446049250313e-16);   // sqrt(eps(Float64)), as cs_b200_solve_advanced_batch
+  int nbits = 1;
+  while (nbits < 32 && (1ull << nbits) <= (unsigned long long)L.ntiles) ++nbits;   // keys 0 .. ntiles
+  Stream st;
+  DevBufs d;
+  T *dG, *dS, *wg, *ws, *wn;
+  double *dcum, *dscale = nullptr, *dgnd = nullptr, *wcur, *wvec;
+  int *dtr, *dtc, *wlab, *wflag, *wlist, *val_in, *val_out, *beg, *end;
+  unsigned *key_in, *key_out;
+  WinOut* dout;
+  unsigned char* tmp = nullptr;
+  size_t tmp_bytes = 0;
+  CKM(cudaStreamCreateWithFlags(&st.s, cudaStreamNonBlocking));
+  CKM(d.get(&dG, cells));
+  CKM(d.get(&dS, cells));
+  CKM(d.get(&dcum, cells));
+  CKM(d.get(&dtr, (size_t)nwin));
+  CKM(d.get(&dtc, (size_t)nwin));
+  if (scale) CKM(d.get(&dscale, (size_t)nwin));
+  if (gnd) CKM(d.get(&dgnd, (size_t)nwin));
+  CKM(d.get(&wg, bw * ncell));
+  CKM(d.get(&ws, bw * ncell));
+  CKM(d.get(&wn, bw * ncell));
+  CKM(d.get(&wcur, bw * ncell));
+  CKM(d.get(&wvec, bw * ncell * NVEC));
+  CKM(d.get(&wlab, bw * ncell));
+  CKM(d.get(&wflag, bw * ncell));
+  CKM(d.get(&wlist, bw * ncell));
+  CKM(d.get(&dout, (size_t)bw));
+  CKM(d.get(&key_in, bw * per));
+  CKM(d.get(&key_out, bw * per));
+  CKM(d.get(&val_in, bw * per));
+  CKM(d.get(&val_out, bw * per));
+  CKM(d.get(&beg, (size_t)L.ntiles));
+  CKM(d.get(&end, (size_t)L.ntiles));
+  CKM(cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, key_in, key_out, val_in, val_out, (int)(bw * per), 0,
+                                      nbits, st.s));
+  CKM(d.get(&tmp, tmp_bytes));
+
+  CKM(cudaMemcpyAsync(dG, g, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
+  CKM(cudaMemcpyAsync(dS, src, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
+  CKM(cudaMemsetAsync(dcum, 0, cells * sizeof(double), st.s));
+  CKM(cudaMemcpyAsync(dtr, trow.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
+  CKM(cudaMemcpyAsync(dtc, tcol.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
+  if (scale) CKM(cudaMemcpyAsync(dscale, scale, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  if (gnd) CKM(cudaMemcpyAsync(dgnd, gnd, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  for (int w0 = 0; w0 < nwin; w0 += bw) {
+    const int nb = std::min(bw, nwin - w0), np = (int)(nb * per);
+    k_window_cut<T><<<nb, BT, 0, st.s>>>(L, w0, dG, dS, dtr, dtc, dscale, dgnd, wg, ws, wn);
+    CKM(cudaGetLastError());
+    CKM((launch<T>(nb, s, wg, ws, wn, rtol, atol, itmax, wcur, nullptr, wvec, wlab, wflag, wlist, dout, st.s)));
+    k_window_tiles<<<(np + BT - 1) / BT, BT, 0, st.s>>>(L, w0, nb, dtr, dtc, key_in, val_in);
+    CKM(cudaGetLastError());
+    size_t tb = tmp_bytes;
+    CKM(cub::DeviceRadixSort::SortPairs(tmp, tb, key_in, key_out, val_in, val_out, np, 0, nbits, st.s));
+    CKM(cudaMemsetAsync(beg, 0, (size_t)L.ntiles * sizeof(int), st.s));
+    CKM(cudaMemsetAsync(end, 0, (size_t)L.ntiles * sizeof(int), st.s));
+    k_tile_bounds<<<(np + BT - 1) / BT, BT, 0, st.s>>>(np, key_out, (unsigned)L.ntiles, beg, end);
+    CKM(cudaGetLastError());
+    k_window_accumulate<<<L.ntiles, BT, 0, st.s>>>(L, w0, dtr, dtc, beg, end, val_out, wcur, dcum);
+    CKM(cudaGetLastError());
+    CKM(cudaMemcpyAsync(wo.data() + w0, dout, (size_t)nb * sizeof(WinOut), cudaMemcpyDeviceToHost, st.s));
+  }
+  CKM(cudaMemcpyAsync(cum, dcum, cells * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+  CKM(cudaStreamSynchronize(st.s));
+  return CS_B200_OK;
+}
+
 }  // namespace
 
 #define CKB(call)                                                                              \
@@ -472,4 +694,91 @@ done:
   if (dbuf) cudaFree(dbuf);
   if (st) cudaStreamDestroy(st);
   return rc;
+}
+
+extern "C" int cs_b200_solve_moving_windows(int64_t nrows, int64_t ncols, const void* g, const void* src, int dtype,
+                                            int64_t nwin, const int64_t* target_rows, const int64_t* target_cols,
+                                            int64_t radius, int circular, const double* source_scale,
+                                            const double* ground, int four_neighbors, int device, double rtol,
+                                            int64_t itmax, int64_t max_batch_bytes, double* cum, int64_t* iters,
+                                            double* relres, int64_t* first_failed) {
+  if (first_failed) *first_failed = -1;
+  if (nrows < 1 || ncols < 1 || nrows > INT_MAX / ncols)
+    return set_err(CS_B200_ERR_ARG, "bad landscape shape %lld x %lld (at most INT_MAX cells)", (long long)nrows,
+                   (long long)ncols);
+  if (radius < 0 || 2 * radius + 1 > 46340)   // (2R+1)^2 cells per window must fit an int
+    return set_err(CS_B200_ERR_ARG, "bad radius %lld (0 <= radius, (2 radius + 1)^2 <= INT_MAX)", (long long)radius);
+  if (nwin < 0 || nwin > INT_MAX) return set_err(CS_B200_ERR_ARG, "bad window count %lld", (long long)nwin);
+  if (dtype != CS_B200_F32 && dtype != CS_B200_F64) return set_err(CS_B200_ERR_ARG, "bad dtype %d", dtype);
+  if (!(rtol >= 0.0) || itmax < 0)
+    return set_err(CS_B200_ERR_ARG, "bad rtol %g / itmax %lld", rtol, (long long)itmax);
+  if (max_batch_bytes <= 0) return set_err(CS_B200_ERR_ARG, "bad max_batch_bytes %lld", (long long)max_batch_bytes);
+  if (!g || !src || !cum || (nwin > 0 && (!target_rows || !target_cols)))
+    return set_err(CS_B200_ERR_ARG, "g, src, cum, target_rows and target_cols must not be NULL");
+  std::vector<int> trow((size_t)nwin), tcol((size_t)nwin);
+  for (int64_t w = 0; w < nwin; ++w) {
+    if (target_rows[w] < 0 || target_rows[w] >= nrows || target_cols[w] < 0 || target_cols[w] >= ncols)
+      return set_err(CS_B200_ERR_ARG, "target %lld at (%lld, %lld) outside the %lld x %lld landscape", (long long)w,
+                     (long long)target_rows[w], (long long)target_cols[w], (long long)nrows, (long long)ncols);
+    if (ground && !(ground[w] > 0.0))
+      return set_err(CS_B200_ERR_ARG, "ground[%lld] = %g: target grounds must be > 0 (Inf = direct)", (long long)w,
+                     ground[w]);
+    if (source_scale && !std::isfinite(source_scale[w]))
+      return set_err(CS_B200_ERR_ARG, "source_scale[%lld] = %g is not finite", (long long)w, source_scale[w]);
+    trow[w] = (int)target_rows[w];
+    tcol[w] = (int)target_cols[w];
+  }
+  const size_t cells = (size_t)nrows * ncols;
+  std::fill(cum, cum + cells, 0.0);
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return set_err(CS_B200_ERR_CUDA, "no CUDA device available (%s): libcsb200 has no CPU fallback",
+                   cudaGetErrorString(e));
+  if (device < 0 || device >= ndev)
+    return set_err(CS_B200_ERR_ARG, "device %d out of range (0..%d)", device, ndev - 1);
+  if (nwin == 0) return CS_B200_OK;
+
+  Land L;
+  L.nrows = (int)nrows;
+  L.ncols = (int)ncols;
+  L.radius = (int)radius;
+  L.side = 2 * L.radius + 1;
+  L.circular = circular ? 1 : 0;
+  L.tiles_r = (L.nrows + TILE - 1) / TILE;
+  L.ntiles = L.tiles_r * ((L.ncols + TILE - 1) / TILE);
+  L.span = std::min((L.side + TILE - 1) / TILE + 1, std::max(L.tiles_r, L.ntiles / L.tiles_r));
+  // windows per batch: the device bytes of one window's stack, solver.advanced_batch_bytes(ncell, itemsize,
+  // False) -- the inputs, the current raster, NVEC fp64 CG vectors, three int32 label arrays and its WinOut
+  const size_t isz = dtype == CS_B200_F64 ? 8 : 4, ncell = (size_t)L.side * L.side;
+  const size_t per = ncell * (3 * isz + 8 + NVEC * 8 + 3 * 4) + sizeof(WinOut);
+  const size_t pairs = (size_t)L.span * L.span;
+  const size_t bw = std::max<size_t>(1, std::min({(size_t)max_batch_bytes / per, (size_t)nwin, INT_MAX / pairs}));
+  std::vector<WinOut> wo((size_t)nwin);
+  e = cudaSetDevice(device);
+  if (e != cudaSuccess) return set_err(CS_B200_ERR_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
+  const int rc = dtype == CS_B200_F64
+                     ? moving_windows<double>(L, (int)nwin, (int)bw, g, src, trow, tcol, source_scale, ground,
+                                              four_neighbors ? 1 : 0, rtol, (long long)itmax, cum, wo)
+                     : moving_windows<float>(L, (int)nwin, (int)bw, g, src, trow, tcol, source_scale, ground,
+                                             four_neighbors ? 1 : 0, rtol, (long long)itmax, cum, wo);
+  if (rc != CS_B200_OK) return rc;
+
+  int64_t bad = -1;
+  int worst = WIN_OK;
+  for (int64_t w = 0; w < nwin; ++w) {
+    if (iters) iters[w] = wo[w].iters;
+    if (relres) relres[w] = wo[w].relres;
+    if (wo[w].status > worst) { worst = wo[w].status; bad = w; }
+  }
+  if (first_failed) *first_failed = bad;
+  if (worst == WIN_RESIDUAL)
+    return set_err(CS_B200_ERR_RESIDUAL,
+                   "CUDA PCG solver residual %g exceeds tolerance %g for window %lld (%d iterations)",
+                   wo[bad].fail_relres, kGate, (long long)bad, wo[bad].fail_iters);
+  if (worst == WIN_MAXITER)
+    return set_err(CS_B200_ERR_MAXITER,
+                   "CUDA PCG solver reached itmax = %lld before rtol for window %lld (residual %g)",
+                   (long long)itmax, (long long)bad, wo[bad].fail_relres);
+  return CS_B200_OK;
 }

@@ -591,7 +591,8 @@ class B200Factor:
 
 def advanced_batch_bytes(ncell, itemsize, want_volt):
     """Device bytes cs_b200_solve_advanced_batch allocates per window of `ncell` cells: the three
-    inputs, the current (and voltage) raster, five fp64 CG vectors and three int32 label arrays."""
+    inputs, the current (and voltage) raster, five fp64 CG vectors and three int32 label arrays.
+    cs_b200_solve_moving_windows sizes its batches by the same formula (want_volt False)."""
     return ncell * (3 * itemsize + 8 * (2 if want_volt else 1) + 5 * 8 + 3 * 4) + 32
 
 
@@ -621,6 +622,39 @@ def solve_advanced_batch(g, src, gnd, four_neighbors, device, rtol, itmax, want_
         msg = lib.cs_b200_last_error(None).decode()
     return dict(cur=cur.transpose(0, 2, 1), volt=None if volt is None else volt.transpose(0, 2, 1),
                 iters=iters, relres=relres, rc=rc, first_failed=int(bad.value), msg=msg)
+
+
+def solve_moving_windows(g, src, target_rows, target_cols, radius, circular, source_scale, ground, four_neighbors,
+                         device, rtol, itmax, max_batch_bytes):
+    """One cs_b200_solve_moving_windows call: landscape rasters g / src (nrows, ncols) of one float dtype
+    (float32 or float64), targets (nwin,) each, source_scale / ground (nwin,) float64 or None (all 1 / all
+    Inf).  Windows are batched under max_batch_bytes at advanced_batch_bytes(ncell, itemsize, False) each.
+    Returns dict with cum (nrows, ncols) float64, iters, relres (nwin,), rc (OK, ERR_RESIDUAL or
+    ERR_MAXITER), first_failed (global window index or -1) and msg; other failures raise."""
+    lib = _lib.load()
+    nr, nc = g.shape
+    dt = _lib.dtype_code(g.dtype)
+    # column-major rasters: (ncols, nrows) in C order
+    g_, s_ = (np.ascontiguousarray(np.asarray(a, dtype=g.dtype).T) for a in (g, src))
+    tr, tc = (np.ascontiguousarray(t, dtype=np.int64) for t in (target_rows, target_cols))
+    nwin = len(tr)
+    cum = np.empty((nc, nr), dtype=np.float64)
+    iters = np.zeros(nwin, dtype=np.int64)
+    relres = np.zeros(nwin, dtype=np.float64)
+    bad = C.c_int64(-1)
+    rc = lib.cs_b200_solve_moving_windows(nr, nc, _lib._ptr(g_), _lib._ptr(s_), dt, nwin, _lib._ptr(tr),
+                                          _lib._ptr(tc), int(radius), 1 if circular else 0,
+                                          _lib._ptr(_opt(source_scale, np.float64)), _lib._ptr(_opt(ground, np.float64)),
+                                          1 if four_neighbors else 0, device, float(rtol), int(itmax),
+                                          int(max_batch_bytes), _lib._ptr(cum), _lib._ptr(iters), _lib._ptr(relres),
+                                          C.byref(bad))
+    msg = ""
+    if rc not in (_lib.OK, _lib.ERR_RESIDUAL, _lib.ERR_MAXITER):
+        _lib.check(lib, None, rc)
+    if rc != _lib.OK:
+        msg = lib.cs_b200_last_error(None).decode()
+    return dict(cum=np.ascontiguousarray(cum.T), iters=iters, relres=relres, rc=rc, first_failed=int(bad.value),
+                msg=msg)
 
 
 # ---------------------------------------------------------------------------

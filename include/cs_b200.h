@@ -361,6 +361,37 @@ int cs_b200_solve_advanced_batch(int64_t nwin, int64_t nrows, int64_t ncols, con
                                  int64_t itmax, void* cur, void* volt, int64_t* iters, double* relres,
                                  int64_t* first_failed);
 
+/* Omniscape's moving-window loop over one landscape: the windows of cs_b200_solve_advanced_batch cut on
+ * the device from resident rasters, their currents summed into one landscape map on the device.
+ *   g, src: host, nrows x ncols, column-major (cell r + c * nrows, as cs_b200_create_from_raster),
+ *           element type `dtype`; uploaded once.
+ *   Window w (nwin of them) is the (2 radius + 1)^2 square centred on the target (target_rows[w],
+ *   target_cols[w]), 0-based; its cell (i, j) is landscape cell (tr - radius + i, tc - radius + j).  A
+ *   cell is a node when that position is inside the landscape, g > 0 there (0, NODATA -9999 and NaN are
+ *   not), and, when `circular`, (i - radius)^2 + (j - radius)^2 <= radius^2.  On the nodes the window's
+ *   conductance is g, its source (T)(source_scale[w] * src) and its ground ground[w] at the centre cell
+ *   only (a conductance: Inf = direct ground); every other cell has g = 0.  Each window is then solved
+ *   exactly as one window of cs_b200_solve_advanced_batch (four_neighbors, rtol, itmax, gate).
+ *   source_scale: NULL (all 1) or nwin finite values.  ground: NULL (all Inf) or nwin values > 0.
+ *   cum:  host, nrows x ncols fp64, column-major: cum[r, c] = sum over w, in window order, of window w's
+ *         current at (r - tr + radius, c - tc + radius), from +0.0 -- bit-identical whatever the batch
+ *         split and on repeats (fixed order, no floating-point atomics).  Zero when nwin = 0.
+ *   iters[nwin], relres[nwin], first_failed: as in cs_b200_solve_advanced_batch; may be NULL.
+ * Windows go to the device in batches of consecutive windows, as many as fit max_batch_bytes at the
+ * per-window device bytes of cs_b200_solve_advanced_batch (at least one); the rasters and cum stay on
+ * the device for the whole call, so host memory is O(landscape + nwin).
+ * CS_B200_ERR_RESIDUAL / CS_B200_ERR_MAXITER name the first window (global index) that failed the gate /
+ * ran into itmax in *first_failed and in cs_b200_last_error(NULL); every output is still written.
+ * CS_B200_ERR_ARG before any device work: a bad shape, more than INT_MAX landscape or window cells, a
+ * negative radius, a target outside the landscape, a ground <= 0 or NaN, a scale that is NaN or Inf, a
+ * NULL required pointer, max_batch_bytes <= 0, a bad dtype, rtol or itmax.                               */
+int cs_b200_solve_moving_windows(int64_t nrows, int64_t ncols, const void* g, const void* src, int dtype,
+                                 int64_t nwin, const int64_t* target_rows, const int64_t* target_cols,
+                                 int64_t radius, int circular, const double* source_scale, const double* ground,
+                                 int four_neighbors, int device, double rtol, int64_t itmax,
+                                 int64_t max_batch_bytes, double* cum, int64_t* iters, double* relres,
+                                 int64_t* first_failed);
+
 /* Cumulative / max node-current vectors (n values of dtype each; either may be
  * NULL).  max is initialised to -9999 like src/utils.jl:124.                        */
 int cs_b200_read_currents(cs_b200_handle* h, void* cum, void* max);
