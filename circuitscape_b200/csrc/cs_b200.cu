@@ -150,6 +150,7 @@ struct cs_b200_handle {
   // Region panels mask AP and Z inside the PCG loop, so they get graph slots of their own; those graphs
   // capture d_rg_seg / d_rg_rows and are dropped whenever the buffers are reallocated.
   bool rg_on = false;                // the panel being solved is a region panel
+  bool pair_b = false;               // its right-hand side is ctl's pairs rule, B not written (stage_pair_rhs)
   int* d_rg_seg = nullptr;
   int* d_rg_rows = nullptr;
   size_t rg_cap = 0;
@@ -974,17 +975,18 @@ void launch_spmm_win(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const
 // the dominant kernel for the per-launch profile (finest-level operator only).
 template <typename T, int KT, int MODE>
 void launch_spmm_on(cs_b200_handle* h, const DevCsr& m, const T* X, T* Y, const T* B, const T* dinv,
-                    double omega, bool timed) {
+                    double omega, bool timed, bool pair_b = false) {
   const int grid = std::max(1, std::min(h->grid_spmm, m.nblocks));
   // nnz (s_v + 4) + (n + 1) 4 + X once + Y once (+ B for the residual / sweep epilogues,
-  // + 1/diag for the sweeps)
+  // + 1/diag for the sweeps); pair_b (stencil residual gate of a pairs panel): neither B nor Y
   double bytes = (double)m.nnz * (sizeof(T) + 4) + (double)(m.nrows + 1) * 4 +
                  2.0 * (double)m.nrows * KT * sizeof(T);
   if (MODE == SP_RESNORM || MODE == SP_RES || MODE == SP_JACOBI || MODE == SP_JACOBI_DOT)
     bytes += (double)m.nrows * KT * sizeof(T);
   if (MODE == SP_JACOBI || MODE == SP_JACOBI_DOT) bytes += (double)m.nrows * sizeof(T);
+  if (pair_b) bytes -= 2.0 * (double)m.nrows * KT * sizeof(T);
   const ProfScope prof(h, timed, MODE, sizeof(T) == 4, bytes);
-  const SpmmEpi<T> ep{B, dinv, (T)omega, h->d_ctl, h->d_partials};
+  const SpmmEpi<T> ep{B, dinv, (T)omega, h->d_ctl, h->d_partials, pair_b ? 1 : 0};
   if (m.dia && MODE != SP_ADD) {
     if constexpr (MODE != SP_ADD) launch_stencil<T, KT, MODE>(h, dia_view<T>(m), X, Y, ep, stencil_grid<T, KT>(h, m));
   } else if (m.win_meta) {
@@ -1181,6 +1183,16 @@ inline bool fused_cg(const cs_b200_handle* h) {
 // update, so they keep k_cg_update_r0
 inline bool fused_res(const cs_b200_handle* h) {
   return fused_cg(h) && h->R2 && !h->rg_on && fused_res_form(h);
+}
+
+// The passes around a fused AMG-PCG panel's loop (pipelined stencil kernels): X and P are not zero-filled (the
+// CG step and k_cg_x_tail read the zeros they would hold as zeros), r and r32 come from one pass
+// (k_panel_start), and a pairs panel writes no B: its start pass and residual gate take b from ctl, and the gate
+// stores no B - A X (nothing reads it after a pairs panel).  CS_B200_NO_FUSED_PANEL_ENDS keeps the fills,
+// B, the copy and the conversion for A/B runs.
+inline bool panel_ends(const cs_b200_handle* h) {
+  static const bool off = std::getenv("CS_B200_NO_FUSED_PANEL_ENDS") != nullptr;
+  return !off && fused_cg(h) && stencil_pipe();
 }
 
 template <typename T, int KT, typename TV, bool HALF, bool STORE_AP>
@@ -1381,8 +1393,9 @@ int run_loop(cs_b200_handle* h) {
   return CS_B200_OK;
 }
 
-// Solve A X = B for the panel whose B is already staged and whose ctl (src/dst/weight)
-// has been uploaded.  Leaves X = solution, AP = B - A X, ctl (host copy) updated.
+// Solve A X = B for the panel whose B is already staged (or, h->pair_b, whose b is the pairs rule of ctl) and
+// whose ctl (src/dst/weight) has been uploaded.  Leaves X = solution, ctl (host copy) updated (resid, bnorm) and
+// AP = B - A X, except on a pair_b panel, where AP is not written (nothing reads it after a pairs panel).
 template <typename T, int KT>
 int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
   const size_t nelem = (size_t)h->n_pad * KT;
@@ -1403,16 +1416,25 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
   } else {
     // x = 0, p = 0, r = b ; z = M^-1 r (V-cycle; its last kernel sets rho0, tolerances,
     // activity because ctl->init = 1) ; p = z + 0*p  (fused CG step: formed by the first step, which
-    // reads the zeroed P as p_{-1} with beta = 0)
+    // takes p_{-1} = 0 with beta = 0 -- read from the zero-filled P, or under panel_ends staged as zeros with
+    // P not filled)
     const bool fused = fused_cg(h);
-    CK(h, cudaMemsetAsync(h->X, 0, nelem * sizeof(T), h->stream));
-    CK(h, cudaMemsetAsync(h->P, 0, nelem * sizeof(T), h->stream));
-    CK(h, cudaMemcpyAsync(h->R, h->B, nelem * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
-    k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, rtol, atol, imax, 40);
-    h->stats.kernel_launches++;
-    if (h->mixed) {
-      k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
+    if (panel_ends(h)) {
+      // x = 0 and p = 0 stay implicit; r (and r32) in one pass, from ctl on a pairs panel
+      k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, rtol, atol, imax, 40);
+      k_panel_start<T, KT><<<g, NT, 0, h->stream>>>(nelem, h->pair_b ? nullptr : (const T*)h->B, (T*)h->R,
+                                                    h->mixed ? (float*)h->R32 : nullptr, h->d_ctl);
+      h->stats.kernel_launches += 2;
+    } else {
+      CK(h, cudaMemsetAsync(h->X, 0, nelem * sizeof(T), h->stream));
+      CK(h, cudaMemsetAsync(h->P, 0, nelem * sizeof(T), h->stream));
+      CK(h, cudaMemcpyAsync(h->R, h->B, nelem * sizeof(T), cudaMemcpyDeviceToDevice, h->stream));
+      k_set_ctl<<<1, 1, 0, h->stream>>>(h->d_ctl, rtol, atol, imax, 40);
       h->stats.kernel_launches++;
+      if (h->mixed) {
+        k_convert<T, float><<<g, NT, 0, h->stream>>>(nelem, (const T*)h->R, (float*)h->R32);
+        h->stats.kernel_launches++;
+      }
     }
     launch_vcycle<T, KT>(h, false);
     mask_z<T, KT>(h);
@@ -1448,7 +1470,9 @@ int solve_panel(cs_b200_handle* h, double rtol, int64_t itmax) {
     k_resnorm<T, KT><<<g, NT, 0, h->stream>>>(nelem, (size_t)h->n * KT, (const T*)h->AP, (const T*)h->B, h->d_ctl, h->d_partials);
     h->stats.kernel_launches++;
   } else {
-    launch_spmm<T, KT, 2>(h, (const T*)h->X, (T*)h->AP, (const T*)h->B);
+    // pair_b: b from ctl, AP not written
+    launch_spmm_on<T, KT, SP_RESNORM>(h, h->A0, (const T*)h->X, (T*)h->AP, (const T*)h->B, (const T*)h->d_dinv, 0.0,
+                                      true, h->pair_b);
   }
   CK(h, cudaGetLastError());
   CK(h, cudaEventRecord(h->ev3, h->stream));
@@ -1521,6 +1545,7 @@ struct ColumnDriver {
     h->rg_on = masked;
     const int rc = solve_panel<T, KT>(h, rtol, itmax);
     h->rg_on = false;
+    h->pair_b = false;
     if (!rc) gather(KT, c0, iters, relres, itmax);
     return rc;
   }
@@ -1732,6 +1757,18 @@ int currents_and_outputs(cs_b200_handle* h, int64_t c0, T* curr, T* volt, int ac
 }
 
 // ---- the column kinds ------------------------------------------------------------------------
+// B of a pairs panel, -1 at src and +1 at dst (k_pair_rhs); under panel_ends B is not written and the panel's
+// start pass and residual gate take b from ctl (pair_b, cleared by ColumnDriver::solve)
+template <typename T, int KT>
+int stage_pair_rhs(cs_b200_handle* h) {
+  h->pair_b = panel_ends(h);
+  if (h->pair_b) return CS_B200_OK;
+  CK(h, cudaMemsetAsync(h->B, 0, (size_t)h->n_pad * KT * sizeof(T), h->stream));
+  k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
+  h->stats.kernel_launches++;
+  return CS_B200_OK;
+}
+
 template <typename T, int KT>
 int pairs_panel(cs_b200_handle* h, int64_t c0, const int64_t* src, const int64_t* dst,
                 const double* weight, double rtol, int64_t itmax, T* R, T* volt, T* curr,
@@ -1740,9 +1777,7 @@ int pairs_panel(cs_b200_handle* h, int64_t c0, const int64_t* src, const int64_t
         return ColCtl{src[c0 + c], dst[c0 + c], col_weight(weight, c0 + c)};
       }))
     return rc;
-  CK(h, cudaMemsetAsync(h->B, 0, (size_t)h->n_pad * KT * sizeof(T), h->stream));
-  k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
-  h->stats.kernel_launches++;
+  if (int rc = stage_pair_rhs<T, KT>(h)) return rc;
   if (int rc = cols.solve<T, KT>(c0, rtol, itmax, iters, relres)) return rc;
   k_pair_extract<T, KT><<<1, 32, 0, h->stream>>>((const T*)h->X, h->d_ctl);
   h->stats.kernel_launches++;
@@ -1789,9 +1824,7 @@ int point_panel(cs_b200_handle* h, int64_t x0, const int64_t* nodes, double rtol
                 int64_t* point_iters, ColumnDriver& cols) {
   const size_t nelem = (size_t)h->n_pad * KT;
   if (int rc = upload_ctl(h, KT, [&](int c) { return ColCtl{nodes[0], nodes[x0 + c], 1.0}; })) return rc;
-  CK(h, cudaMemsetAsync(h->B, 0, nelem * sizeof(T), h->stream));
-  k_pair_rhs<T, KT><<<1, 32, 0, h->stream>>>((T*)h->B, h->d_ctl);
-  h->stats.kernel_launches++;
+  if (int rc = stage_pair_rhs<T, KT>(h)) return rc;
   if (int rc = cols.solve<T, KT>(0, rtol, itmax, nullptr, nullptr)) return rc;
   if (point_iters)
     for (int c = 0; c < KT; ++c) point_iters[x0 - 1 + c] = h->h_ctl->iters[c];

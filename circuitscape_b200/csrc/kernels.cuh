@@ -4,8 +4,10 @@
 // per GPU; every solver vector is a *panel*: n_pad x KT row-major (KT in {1,2,4,8}
 // right-hand sides interleaved per node) so one SpMM gather of a neighbour reads
 // KT*sizeof(T) contiguous bytes and the 12 B/nnz matrix stream is paid once per KT
-// right-hand sides.  n_pad = n rounded up to 4 rows; pad rows are zero everywhere so
-// the element-wise kernels can use 16-byte vectors without tails.
+// right-hand sides.  n_pad = n rounded up to 4 rows, so the element-wise kernels can use
+// 16-byte vectors without tails; pad rows are zero except in X and P of a panel that
+// starts from implicit zeros (cs_b200.cu panel_ends), where they are never read into a
+// result: the stencil kernels stage rows >= n as zeros, every other reader of X stops at row n.
 // All reductions are deterministic: warp tree -> per-CTA partial in a fixed slot ->
 // combined in a fixed order by the last CTA to finish (ticket counter), which also
 // derives the CG scalars on the device -- no host round trip, no float atomics.
@@ -279,7 +281,24 @@ template <typename T> struct SpmmEpi {
   T omega;
   PanelCtl* ctl;
   double* partials;
+  int pair_b;          // k_stencil_pipe SP_RESNORM: b is ctl's pairs rule (pair_rhs_val), B not read, Y not stored
 };
+
+// entry (row, c) of a pairs panel's right-hand side: -1 at src, +1 at dst where both are nodes and differ
+// (core.jl:224-226, 459-460); what k_pair_rhs leaves in a zeroed B.  Host-callable for the CPU check of
+// k_panel_start (tests/panel_start_harness.cu).
+template <typename T>
+__host__ __device__ __forceinline__ T pair_rhs_val(const PanelCtl* ctl, long long row, int c) {
+  const long long s = ctl->src[c], d = ctl->dst[c];
+  if (s < 0 || d < 0 || s == d) return T(0);
+  return row == d ? T(1) : row == s ? T(-1) : T(0);
+}
+
+// element e of a KT-wide pairs panel (row e / KT, column e % KT), as k_panel_start forms it
+template <typename T, int KT>
+__host__ __device__ __forceinline__ T pair_rhs_at(const PanelCtl* ctl, size_t e) {
+  return pair_rhs_val<T>(ctl, (long long)(e / KT), (int)(e % KT));
+}
 
 template <typename T, int MODE>
 __device__ __forceinline__ void spmm_epilogue(int row, size_t o, T acc, const T* __restrict__ X,
@@ -1262,9 +1281,10 @@ template <int N> __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-// rows [g0, g0 + NROWS) of a panel of W values per row, zero outside [0, n); chunks of min(16, row) bytes
+// rows [g0, g0 + NROWS) of a panel of W values per row, zero outside [0, n); chunks of min(16, row) bytes.
+// !live: all zero, src not read (a panel known to hold zeros)
 template <typename U, int W, int NROWS>
-__device__ __forceinline__ void cp_rows(U* dst, const U* src, long long g0, int n) {
+__device__ __forceinline__ void cp_rows(U* dst, const U* src, long long g0, int n, bool live = true) {
   constexpr int RB = W * (int)sizeof(U);
   constexpr int CH = RB < 16 ? RB : 16;
   constexpr int CPR = RB / CH;
@@ -1274,7 +1294,7 @@ __device__ __forceinline__ void cp_rows(U* dst, const U* src, long long g0, int 
     const int q = q0 + (int)threadIdx.x;
     if (NCH % NT == 0 || q < NCH) {
       const long long g = g0 + q / CPR;
-      const bool ok = g >= 0 && g < n;
+      const bool ok = live && g >= 0 && g < n;
       cp_async_zfill<CH>(reinterpret_cast<char*>(dst) + q * CH,
                          reinterpret_cast<const char*>(src + (ok ? g : 0) * W) + (q % CPR) * CH, ok);
     }
@@ -1444,7 +1464,8 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
       unsigned char* os = oring + lo * SP::OWN;
       const long long row0 = (long long)(s.c - 1) * nr + s.r0;
       if (!HALF) cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
-      if (SP::NEEDB) cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), ep.B, row0, n);
+      if (SP::NEEDB && !(MODE == SP_RESNORM && ep.pair_b))
+        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), ep.B, row0, n);
       if (SP::NEEDD) cp_rows<T, 1, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OB), ep.dinv, row0, n);
     }
   };
@@ -1484,7 +1505,12 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
     }
     const size_t o = (size_t)row * KT + c0;
     T out[CPT], bb[CPT];
-    if (SP::NEEDB) ldvec<T, CPT>(reinterpret_cast<const T*>(os + SP::OD) + rl * KT + c0, bb);
+    if (MODE == SP_RESNORM && ep.pair_b) {
+#pragma unroll
+      for (int i = 0; i < CPT; ++i) bb[i] = pair_rhs_val<T>(ep.ctl, row, c0 + i);
+    } else if (SP::NEEDB) {
+      ldvec<T, CPT>(reinterpret_cast<const T*>(os + SP::OD) + rl * KT + c0, bb);
+    }
     T dv = T(0);
     if (SP::NEEDD) dv = ep.omega * reinterpret_cast<const T*>(os + SP::OD + SP::OB)[rl];
 #pragma unroll
@@ -1509,7 +1535,7 @@ k_stencil_pipe(const DiaDev<T> A, const T* __restrict__ X, T* __restrict__ Y, co
         if (MODE == SP_JACOBI_DOT) dot0[i] += (double)bb[i] * (double)yn;
       }
     }
-    stvec<T, CPT>(Y + o, out);
+    if (!(MODE == SP_RESNORM && ep.pair_b)) stvec<T, CPT>(Y + o, out);
   };
   stencil_pipe<S, RPP>(n, nr, issue, compute);
 
@@ -1581,6 +1607,9 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
   const int cg = tid % (KT / CPT), rl = tid / (KT / CPT), c0 = cg * CPT;
   const int n = A.n, nr = A.nr;
   const bool pair = it & 1;
+  // a panel starts from x = 0, p_{-1} = 0: p_{it-1} at it = 0 and x, p_{it-2} at it = 1 are staged as zeros, not
+  // read, so the start of a panel need not fill X and P (panel_ends)
+  const bool p_live = it != 0, x_live = it != 1;
   T be[CPT], a1[CPT], a2[CPT];                  // beta_it ; alpha_{it-1}, alpha_{it-2}
 #pragma unroll
   for (int i = 0; i < CPT; ++i) {
@@ -1595,7 +1624,7 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
   auto issue = [&](const StStep& s, int lp, int lo) {
     unsigned char* ps = pring + lp * SP::PANEL;
     const long long g0 = (long long)s.c * nr + s.r0 - 1;
-    cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), Pold, g0, n);
+    cp_rows<T, KT, RPP + 2>(reinterpret_cast<T*>(ps), Pold, g0, n, p_live);
     cp_rows<TV, KT, RPP + 2>(reinterpret_cast<TV*>(ps + SP::PP), Z, g0, n);
     if (HALF) {
       int u0, u1;
@@ -1607,8 +1636,8 @@ k_stencil_cg_pipe(const DiaDev<T> A, const TV* __restrict__ Z, T* Pb0, T* Pb1, T
       const long long row0 = (long long)(s.c - 1) * nr + s.r0;
       if (!HALF) cp_diag<T, RPP>(reinterpret_cast<T*>(os), A, row0);
       if (pair) {
-        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), X, row0, n);
-        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OX), Pd, row0, n);
+        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD), X, row0, n, x_live);
+        cp_rows<T, KT, RPP>(reinterpret_cast<T*>(os + SP::OD + SP::OX), Pd, row0, n, x_live);
       }
     }
   };
@@ -2383,7 +2412,8 @@ k_cg_update_xp2(size_t nelem, const TV* __restrict__ Z, T* __restrict__ X, T* __
 }
 
 // after a loop of K = ctl->iter fused CG steps (k_stencil_cg): the x updates still pending, in order --
-// p_{K-1}, preceded by p_{K-2} when K is odd (the last pair went in at step K - 2)
+// p_{K-1}, preceded by p_{K-2} when K is odd (the last pair went in at step K - 2).  x is the panel's zero start
+// while K <= 1 and p_{-1} is zero (K = 0): those are not read, as in the CG step, so X and P need no fill.
 template <typename T, int KT>
 __global__ void __launch_bounds__(NT)
 k_cg_x_tail(size_t nelem, const T* __restrict__ Pb0, const T* __restrict__ Pb1, T* __restrict__ X,
@@ -2391,6 +2421,7 @@ k_cg_x_tail(size_t nelem, const T* __restrict__ Pb0, const T* __restrict__ Pb1, 
   constexpr int VEC = Vec<T>::N;
   const int K = ctl->iter;
   const bool two = K & 1;
+  const bool x_live = K > 1, p_live = K > 0;   // x_live: also p_{K-2} is not p_{-1}
   const T* p2 = (K & 1) ? Pb1 : Pb0;         // p_{K-2} (j = -1: the zero p_{-1} with alpha 0)
   const T* p1 = (K & 1) ? Pb0 : Pb1;         // p_{K-1}
   const size_t e0 = ((size_t)blockIdx.x * NT + threadIdx.x) * VEC;
@@ -2403,10 +2434,12 @@ k_cg_x_tail(size_t nelem, const T* __restrict__ Pb0, const T* __restrict__ Pb1, 
   }
   for (size_t e = e0; e < nelem; e += stride) {
     T x[VEC], q1[VEC], q2[VEC];
-    vload(X + e, x);
-    vload(p1 + e, q1);
+#pragma unroll
+    for (int i = 0; i < VEC; ++i) x[i] = q1[i] = q2[i] = T(0);
+    if (x_live) vload(X + e, x);
+    if (p_live) vload(p1 + e, q1);
     if (two) {
-      vload(p2 + e, q2);
+      if (x_live) vload(p2 + e, q2);           // K = 1: p_{-1}
 #pragma unroll
       for (int i = 0; i < VEC; ++i) x[i] += a2[i] * q2[i];
     }
@@ -2422,6 +2455,33 @@ __global__ void __launch_bounds__(NT)
 k_convert(size_t nelem, const TI* __restrict__ in, TO* __restrict__ out) {
   for (size_t e = (size_t)blockIdx.x * NT + threadIdx.x; e < nelem; e += (size_t)gridDim.x * NT)
     out[e] = (TO)in[e];
+}
+
+// start of a fused AMG-PCG panel in one pass: r = b into R and, on mixed handles, r32 = (float) r into R32 (R32
+// null otherwise).  b: B, or with B null the pairs rule of ctl (pair_rhs_val), so a pairs panel never writes B.
+// The values are those of filling B, copying it to R and k_convert.
+template <typename T, int KT>
+__global__ void __launch_bounds__(NT)
+k_panel_start(size_t nelem, const T* __restrict__ B, T* __restrict__ R, float* __restrict__ R32,
+              const PanelCtl* __restrict__ ctl) {
+  constexpr int VEC = Vec<T>::N;
+  const size_t stride = (size_t)gridDim.x * NT * VEC;
+  for (size_t e = ((size_t)blockIdx.x * NT + threadIdx.x) * VEC; e < nelem; e += stride) {
+    T r[VEC];
+    if (B) {
+      vload(B + e, r);
+    } else {
+#pragma unroll
+      for (int i = 0; i < VEC; ++i) r[i] = pair_rhs_at<T, KT>(ctl, e + i);
+    }
+    vstore(R + e, r);
+    if (R32) {
+      if constexpr (VEC == 2)
+        *reinterpret_cast<float2*>(R32 + e) = make_float2((float)r[0], (float)r[1]);
+      else
+        *reinterpret_cast<float4*>(R32 + e) = make_float4((float)r[0], (float)r[1], (float)r[2], (float)r[3]);
+    }
+  }
 }
 
 // first (zero-guess) damped-Jacobi sweep of a level:  X = omega * Dinv * B
