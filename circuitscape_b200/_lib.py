@@ -113,6 +113,11 @@ _PROTOS = {
     "cs_b200_branch_index": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_void_p, C.c_void_p]),
     "cs_b200_read_branch_currents": (C.c_int, [_H, C.c_void_p]),
     "cs_b200_components": (C.c_int, [_H, C.POINTER(C.c_int64), C.c_void_p]),
+    "cs_b200_plan_advanced": (C.c_int, [_H, C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                        C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_int64), C.POINTER(C.c_int64),
+                                        C.POINTER(C.c_int64), C.POINTER(C.c_int)]),
+    "cs_b200_read_advanced_plan": (C.c_int, [_H, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p, C.c_void_p]),
     "cs_b200_read_currents": (C.c_int, [_H, C.c_void_p, C.c_void_p]),
     "cs_b200_reset_currents": (C.c_int, [_H]),
     "cs_b200_currents_device_ptrs": (C.c_int, [_H, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p)]),

@@ -1176,14 +1176,30 @@ def plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of):
 
 
 def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, four_neighbors, avg_res, sink):
-    """src/raster/pairwise.jl:72-135 on one whole-raster operator (see raster_pairwise)."""
+    """src/raster/pairwise.jl:72-135 on one whole-raster operator (see raster_pairwise).  With
+    CUDASolver(front_end_on_device=True) the node map and component labels come from that handle (created first)
+    instead of a host graph; the per-pair path still builds its own."""
     from . import graph
     o = flags.outputflags
     want_maps = _any_map(o)
     per_pair_curr = o.write_cur_maps and not o.write_cum_cur_map_only
-    nodemap = graph.construct_node_map(cellmap, polymap)
-    _, comp_of = _component_labels(graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors))
-    plan = plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of)
+    factor = None
+    if getattr(solver, "front_end_on_device", False):       # node map and labels from the whole-raster handle
+        factor, nodemap = S.construct_raster_factor(cellmap, polymap, solver, four_neighbors=four_neighbors,
+                                                    avg_res=avg_res, log_transform=o.log_transform_maps)
+        try:
+            nodemap = np.asarray(nodemap, dtype=np.int64)
+            comp_of = factor.components()[1]
+            plan = plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of)
+        except BaseException:
+            factor.close()
+            raise
+        if not plan.batched:
+            factor.close()
+    else:
+        nodemap = graph.construct_node_map(cellmap, polymap)
+        _, comp_of = _component_labels(graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors))
+        plan = plan_region_pairs(cellmap, polymap, points_rc, exclude, nodemap, comp_of)
     pts = plan.ids
     P = len(pts)
     R = -np.ones((P, P))
@@ -1191,7 +1207,9 @@ def _focal_region_pairs(cellmap, polymap, points_rc, exclude, flags, solver, fou
     out.cum_curmap = np.zeros(cellmap.shape)
     out.max_curmap = np.full(cellmap.shape, NODATA) if o.write_max_cur_maps else None
     if plan.batched:
-        with _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res, o.log_transform_maps) as factor:
+        if factor is None:
+            factor = _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res, o.log_transform_maps)
+        with factor:
             used = sorted({pts[i] for i, _ in plan.batched} | {pts[j] for _, j in plan.batched})
             slot = {p: s for s, p in enumerate(used)}
             sets = [plan.sets[p] for p in used]
@@ -1494,8 +1512,8 @@ def plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, streng
     return plan
 
 
-def _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solver, four_neighbors, avg_res):
-    """Solve the plan's columns on one whole-raster handle.  one-to-all and all-to-one iterations with
+def _onetoall_columns(plan, factor, nodemap, comp_of, one_to_all, o, solver):
+    """Solve the plan's columns on the open whole-raster handle `factor`.  one-to-all and all-to-one iterations with
     several ground rows: cs_b200_solve_grounded (Dirichlet rows at the grounds); all-to-one with one ground
     row: the singular form of cs_b200_solve_sources (ref = the ground), whose voltages outside the
     component are zeroed here.  Node currents go into the handle's cumulative / max vectors.
@@ -1504,39 +1522,38 @@ def _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solv
     want_c = o.write_cur_maps or o.write_cum_cur_map_only
     served = {}
     iters = 0
-    with _raster_factor(gmap, newpoly, nodemap, solver, four_neighbors, avg_res) as factor:
-        factor.reset_currents()
-        singular = lambda c: (not one_to_all) and len(c.ground) == 1
-        for kind in (False, True):
-            cols = [c for c in plan.columns if singular(c) == kind]
-            for sl in _panels(len(cols), solver):
-                chunk = cols[sl]
-                if kind:
-                    res = factor.solve_sources(
-                        [(np.r_[c.rows, c.ground], np.r_[c.vals, -c.vals.sum()]) for c in chunk],
-                        [int(c.ground[0]) for c in chunk], want_volt=want_v, want_curr=want_c, accumulate=True)
-                else:
-                    res = factor.solve_grounded([c.ground for c in chunk], np.arange(len(chunk)),
-                                                [(c.rows, c.vals) for c in chunk], want_volt=want_v,
-                                                want_curr=want_c, accumulate=True)
-                iters += int(res["iters"].sum())
-                for col, c in enumerate(chunk):
-                    val = 0.0
-                    if one_to_all:
-                        val = float(res["src_volt"][col]) / c.strength
-                        val = -1.0 if np.isclose(val, 0) else val               # advanced.jl:252-263
-                    out = comp_of != c.comp
-                    vm = cm = None
-                    if want_v:
-                        v = np.asarray(res["volt"][:, col], dtype=np.float64).copy()
-                        v[out] = 0.0
-                        vm = _scatter(v, nodemap)
-                    if want_c:
-                        cur = np.asarray(res["curr"][:, col], dtype=np.float64).copy()
-                        cur[out] = 0.0
-                        cm = _scatter(cur, nodemap)
-                    served[c.i] = (val, vm, cm)
-        cum, mx = factor.read_currents(want_max=o.write_max_cur_maps)
+    factor.reset_currents()
+    singular = lambda c: (not one_to_all) and len(c.ground) == 1
+    for kind in (False, True):
+        cols = [c for c in plan.columns if singular(c) == kind]
+        for sl in _panels(len(cols), solver):
+            chunk = cols[sl]
+            if kind:
+                res = factor.solve_sources(
+                    [(np.r_[c.rows, c.ground], np.r_[c.vals, -c.vals.sum()]) for c in chunk],
+                    [int(c.ground[0]) for c in chunk], want_volt=want_v, want_curr=want_c, accumulate=True)
+            else:
+                res = factor.solve_grounded([c.ground for c in chunk], np.arange(len(chunk)),
+                                            [(c.rows, c.vals) for c in chunk], want_volt=want_v,
+                                            want_curr=want_c, accumulate=True)
+            iters += int(res["iters"].sum())
+            for col, c in enumerate(chunk):
+                val = 0.0
+                if one_to_all:
+                    val = float(res["src_volt"][col]) / c.strength
+                    val = -1.0 if np.isclose(val, 0) else val               # advanced.jl:252-263
+                out = comp_of != c.comp
+                vm = cm = None
+                if want_v:
+                    v = np.asarray(res["volt"][:, col], dtype=np.float64).copy()
+                    v[out] = 0.0
+                    vm = _scatter(v, nodemap)
+                if want_c:
+                    cur = np.asarray(res["curr"][:, col], dtype=np.float64).copy()
+                    cur[out] = 0.0
+                    cm = _scatter(cur, nodemap)
+                served[c.i] = (val, vm, cm)
+    cum, mx = factor.read_currents(want_max=o.write_max_cur_maps)
     cmap = _scatter(np.asarray(cum, dtype=np.float64), nodemap)
     mmap = None if mx is None or not plan.columns else _scatter(np.asarray(mx, dtype=np.float64), nodemap)
     return served, cmap, mmap, iters
@@ -1584,7 +1601,10 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
                     four_neighbors=False, avg_res=False) -> OneToAllOutput:
     """src/raster/onetoall.jl:13-167.  One advanced-mode solve per focal id: one-to-all = unit
     (or variable-strength) source at the focal node, every other focal node a direct ground;
-    all-to-one = the reverse.  Every solve goes through `multiple_solver` -> hook #3."""
+    all-to-one = the reverse.  Every solve goes through `multiple_solver` -> hook #3.  With
+    CUDASolver(onetoall_raster=True, front_end_on_device=True) and no include / exclude list the whole-raster handle
+    is created first and gives the node map and component labels; the host graph is built only when some iteration
+    takes the loop."""
     from . import graph
     solver = solver or get_solver(cfg)
     if one_to_all is None:
@@ -1605,18 +1625,34 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
     point_map[rr - 1, cc_ - 1] = ids
     uniq = list(dict.fromkeys(int(p) for p in ids))
     newpoly = graph.create_new_polymap(gmap, polymap, points_rc, point_map)
-    nodemap = graph.construct_node_map(gmap, newpoly)
-    adj = graph.construct_graph(gmap, nodemap, avg_res, four_neighbors)
     device, plan = {}, None
-    if getattr(solver, "onetoall_raster", False):       # precedence over batch_one_to_all / batch_all_to_one
-        comp_of = _component_labels(adj.copy())[1]
-        plan = plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths, inc)
-        if plan.columns:
-            device = dict(zip(("served", "cum", "max", "iters"),
-                              _onetoall_columns(plan, gmap, newpoly, nodemap, comp_of, one_to_all, o, solver,
-                                                four_neighbors, avg_res)))
+    onetoall_raster = getattr(solver, "onetoall_raster", False)   # precedence over batch_one_to_all / batch_all_to_one
+    columns = lambda factor: dict(zip(("served", "cum", "max", "iters"),
+                                      _onetoall_columns(plan, factor, nodemap, comp_of, one_to_all, o, solver)))
+    if onetoall_raster and inc is None and getattr(solver, "front_end_on_device", False):
+        # node map and component labels from the whole-raster handle; the host graph only for the loop's iterations
+        factor, nodemap = S.construct_raster_factor(gmap, newpoly, solver, four_neighbors=four_neighbors,
+                                                    avg_res=avg_res)
+        with factor:
+            nodemap = np.asarray(nodemap, dtype=np.int64)
+            comp_of = factor.components()[1]
+            plan = plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths, inc)
+            if plan.columns:
+                device = columns(factor)
         if not plan.per_iteration:
             return _onetoall_output(plan, device, gmap, o)
+        adj = graph.construct_graph(gmap, nodemap, avg_res, four_neighbors)
+    else:
+        nodemap = graph.construct_node_map(gmap, newpoly)
+        adj = graph.construct_graph(gmap, nodemap, avg_res, four_neighbors)
+        if onetoall_raster:
+            comp_of = _component_labels(adj.copy())[1]
+            plan = plan_onetoall(gmap, newpoly, points_rc, nodemap, comp_of, one_to_all, strengths, inc)
+            if plan.columns:
+                with _raster_factor(gmap, newpoly, nodemap, solver, four_neighbors, avg_res) as factor:
+                    device = columns(factor)
+            if not plan.per_iteration:
+                return _onetoall_output(plan, device, gmap, o)
     comps = graph.connected_components(adj)
     G = graph.laplacian(adj)
     first = {p: int(np.nonzero(ids == p)[0][0]) for p in uniq}
@@ -1731,6 +1767,34 @@ def onetoall_kernel(data: RasterData, flags: Flags, cfg, solver=None, one_to_all
 # ---------------------------------------------------------------------------
 # raster advanced mode on one whole-raster operator  (src/raster/advanced.jl:17-80, 151-305)
 # ---------------------------------------------------------------------------
+def _advanced_front_end_device(data, solver, four_neighbors, avg_res, policy):
+    """raster_advanced's front end on the whole-raster handle (CUDASolver(front_end_on_device=True)): the node map
+    from the create, the columns from B200Factor.plan_advanced, which also applies the finite grounds.  No host
+    graph.  Returns (open factor, nodemap, n, columns as raster_advanced builds them, solved components)."""
+    factor, nodemap = S.construct_raster_factor(data.cellmap, data.polymap, solver, four_neighbors=four_neighbors,
+                                                avg_res=avg_res)
+    try:
+        nodemap = np.asarray(nodemap, dtype=np.int64)
+        plan = factor.plan_advanced(nodemap, data.source_map, data.ground_map, policy)
+        col_of_row = np.asarray(plan["col_of_row"], dtype=np.int64)
+        k = len(plan["col_comp"])
+        # each column's rows, ascending: the rows of its component (the rows of col -1 belong to no column)
+        groups = np.split(np.argsort(col_of_row, kind="stable"),
+                          np.cumsum(np.bincount(col_of_row + 1, minlength=k + 1))[:-1])[1:]
+        sp_, sq = plan["set_ptr"], plan["src_ptr"]
+        columns = []
+        for j, rows in enumerate(groups):
+            lm = None
+            if data.polymap is not None and not _local_map_is_global(nodemap, col_of_row, j, data.polymap):
+                lm = construct_local_node_map(nodemap, rows + 1, data.polymap)
+            columns.append((rows, plan["set_rows"][sp_[j]:sp_[j + 1]], plan["src_rows"][sq[j]:sq[j + 1]],
+                            plan["src_vals"][sq[j]:sq[j + 1]], lm))
+    except BaseException:
+        factor.close()
+        raise
+    return factor, nodemap, factor.n, columns, int(plan["nsolved"])
+
+
 def raster_advanced(data: RasterData, flags: Flags, cfg, solver=None, four_neighbors=False,
                     avg_res=False) -> AdvancedOutput:
     """src/raster/advanced.jl raster_advanced / compute_advanced_data / advanced_kernel: every connected
@@ -1741,40 +1805,51 @@ def raster_advanced(data: RasterData, flags: Flags, cfg, solver=None, four_neigh
     io.jl delivers them (ground conductances, Inf for direct grounds, unit currents applied); the policy is
     cfg's remove_src_or_gnd.  Returns AdvancedOutput: voltmap (the column voltages scattered by the node
     map), curmap (the node currents summed over the columns, no log transform or nodata), voltages per node,
-    and result: the voltage raster, or the 1 x 1 [-1] when no component was solved (advanced.jl:246-249)."""
+    and result: the voltage raster, or the 1 x 1 [-1] when no component was solved (advanced.jl:246-249).
+    With CUDASolver(front_end_on_device=True) the handle is created first and its plan_advanced gives the columns
+    and applies the finite grounds (_advanced_front_end_device): no host graph, labels or node values."""
     from . import graph
     solver = solver or get_solver(cfg)
     cellmap, polymap = data.cellmap, data.polymap
-    nodemap = graph.construct_node_map(cellmap, polymap)
-    adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
-    n = adj.shape[0]
-    ncomp, comp_of = _component_labels(adj)
-    s, g, f = sources_and_grounds_from_maps(np.asarray(data.source_map, dtype=np.float64),
-                                            np.asarray(data.ground_map, dtype=np.float64), nodemap, n,
-                                            cfg.get("remove_src_or_gnd", "keepall"))
-    order = np.argsort(comp_of, kind="stable")
-    comps = np.split(order, np.cumsum(np.bincount(comp_of, minlength=ncomp))[:-1]) if n else []
-    # one column per solved component: (its rows, Inf-ground rows, source rows, values, local node map or
-    # None when construct_local_node_map numbers the component like the node map, utils.jl:10-30)
-    columns, solved = [], 0
-    for ci, rows in enumerate(comps):
-        if s[rows].sum() == 0 or g[rows].sum() == 0:                  # advanced.jl:194-196
-            continue
-        solved += 1
-        inf = g[rows] == np.inf
-        src = rows[(s[rows] != 0) & ~inf]                             # sources on Inf grounds are deleted
-        if not len(src):
-            continue                                                  # b = 0: the component stays at 0 V
-        lm = None
-        if polymap is not None and not _local_map_is_global(nodemap, comp_of, ci, polymap):
-            lm = construct_local_node_map(nodemap, rows + 1, polymap)
-        columns.append((rows, rows[inf], src, s[src], lm))
+    policy = cfg.get("remove_src_or_gnd", "keepall")
+    factor, f = None, None
+    t0 = time.perf_counter()
+    if getattr(solver, "front_end_on_device", False):
+        factor, nodemap, n, columns, solved = _advanced_front_end_device(data, solver, four_neighbors, avg_res, policy)
+    else:
+        nodemap = graph.construct_node_map(cellmap, polymap)
+        adj = graph.construct_graph(cellmap, nodemap, avg_res, four_neighbors)
+        n = adj.shape[0]
+        ncomp, comp_of = _component_labels(adj)
+        s, g, f = sources_and_grounds_from_maps(np.asarray(data.source_map, dtype=np.float64),
+                                                np.asarray(data.ground_map, dtype=np.float64), nodemap, n, policy)
+        order = np.argsort(comp_of, kind="stable")
+        comps = np.split(order, np.cumsum(np.bincount(comp_of, minlength=ncomp))[:-1]) if n else []
+        # one column per solved component: (its rows, Inf-ground rows, source rows, values, local node map or
+        # None when construct_local_node_map numbers the component like the node map, utils.jl:10-30)
+        columns, solved = [], 0
+        for ci, rows in enumerate(comps):
+            if s[rows].sum() == 0 or g[rows].sum() == 0:              # advanced.jl:194-196
+                continue
+            solved += 1
+            inf = g[rows] == np.inf
+            src = rows[(s[rows] != 0) & ~inf]                         # sources on Inf grounds are deleted
+            if not len(src):
+                continue                                              # b = 0: the component stays at 0 V
+            lm = None
+            if polymap is not None and not _local_map_is_global(nodemap, comp_of, ci, polymap):
+                lm = construct_local_node_map(nodemap, rows + 1, polymap)
+            columns.append((rows, rows[inf], src, s[src], lm))
     out = AdvancedOutput(np.zeros(n), np.zeros(nodemap.shape), np.zeros(nodemap.shape), num_solves=solved)
     out.stats = dict(setup_s=0.0, solve_s=0.0, columns=len(columns))
+    if not columns and factor is not None:
+        factor.close()
     if columns:
-        t0 = time.perf_counter()
-        with _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res) as factor:
-            if f[0] != NODATA:
+        if factor is None:
+            t0 = time.perf_counter()
+            factor = _raster_factor(cellmap, polymap, nodemap, solver, four_neighbors, avg_res)
+        with factor:
+            if f is not None and f[0] != NODATA:
                 factor.set_grounds(finite=f)
             t1 = time.perf_counter()
             factor.reset_currents()

@@ -4,7 +4,9 @@
 #include "../../include/cs_b200.h"
 
 #include <cuda_runtime.h>
+#include <cub/device/device_radix_sort.cuh>
 #include <cub/device/device_scan.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 #include <chrono>
@@ -93,6 +95,10 @@ struct cs_b200_handle {
   bool owns_matrix = true;
   void* d_vals0 = nullptr;           // pristine values while grounds are applied (cs_b200_set_grounds)
   void* d_fg = nullptr;              // the finite grounds of the last cs_b200_set_grounds, or null
+  // cs_b200_plan_advanced's plan until cs_b200_read_advanced_plan: col_comp, set_ptr, set_rows, src_ptr,
+  // src_rows (int64), src_vals (fp64), col_of_row (n int32), back to back in one allocation
+  void* d_plan = nullptr;
+  int64_t plan_ncol = 0, plan_nset = 0, plan_nsrc = 0;
   void* d_dinv = nullptr;
   int* d_bstart = nullptr;
   int nblocks = 0;
@@ -2453,6 +2459,43 @@ int apply_precond_t(cs_b200_handle* h, const void* r, void* z, double* rz) {
 }
 
 
+// cs_b200_plan_advanced's stream-ordered scratch, released (after the stream) on every return
+struct PoolScratch {
+  cudaStream_t s;
+  std::vector<void*> p;
+  explicit PoolScratch(cudaStream_t s_) : s(s_) {}
+  template <typename X>
+  cudaError_t get(X** out, size_t count) {
+    void* q = nullptr;
+    cudaError_t e = cudaMallocAsync(&q, std::max<size_t>(count * sizeof(X), 1), s);
+    if (e == cudaSuccess) p.push_back(q);
+    *out = (X*)q;
+    return e;
+  }
+  ~PoolScratch() { for (void* q : p) cudaFreeAsync(q, s); cudaStreamSynchronize(s); }
+};
+
+static int nbits_for(unsigned v) { int b = 1; while (b < 32 && (v >> b)) ++b; return b; }
+
+// the plan's arrays inside d_plan (see cs_b200_handle)
+struct PlanView {
+  long long *col_comp, *set_ptr, *set_rows, *src_ptr, *src_rows;
+  double* src_vals;
+  int* col_of_row;
+  size_t bytes;
+  PlanView(void* base, int64_t ncol, int64_t nset, int64_t nsrc, int64_t n) {
+    long long* q = (long long*)base;
+    col_comp = q; q += ncol;
+    set_ptr = q; q += ncol + 1;
+    set_rows = q; q += nset;
+    src_ptr = q; q += ncol + 1;
+    src_rows = q; q += nsrc;
+    src_vals = (double*)q; q += nsrc;
+    col_of_row = (int*)q;
+    bytes = (size_t)((char*)(col_of_row + n) - (char*)base);
+  }
+};
+
 extern "C" {
 
 int cs_b200_version(void) { return 1008; }
@@ -2670,39 +2713,33 @@ int cs_b200_level_csr(cs_b200_handle* h, int level, int which, int32_t* rowptr, 
   return CS_B200_OK;
 }
 
-int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* dirichlet) {
-  if (!h) return CS_B200_ERR_ARG;
+// Whether the handle can take cs_b200_set_grounds (error text set when not).
+static int grounds_supported(cs_b200_handle* h) {
   if (h->opts.setup == 1)
     return set_err(h, CS_B200_ERR_UNSUPPORTED, "cs_b200_set_grounds needs the device-side setup (opts.setup != 1)");
   if (!h->owns_matrix)
     return set_err(h, CS_B200_ERR_UNSUPPORTED, "cs_b200_set_grounds: the handle borrows its matrix (create_from_device)");
-  cudaSetDevice(h->device);
-  h->err.clear();
-  const size_t es = h->esize();
-  const size_t vb = std::max<size_t>(1, (size_t)h->nnz) * es;
-  cudaEventRecord(h->ev0, h->stream);
+  return CS_B200_OK;
+}
+
+// cs_b200_set_grounds once its arguments are on the device: the pristine values restored, d_g (n values of the
+// handle's type, or null) added to the diagonal and kept as the handle's finite grounds, the rows of d_m (n
+// bytes, or null) tied to ground, then 1/diag, the stencil / window records and the hierarchy rebuilt.  Takes
+// over d_g and d_m (cudaMalloc'ed).  setup_ms runs from ev0, which the caller records.
+static int apply_grounds(cs_b200_handle* h, void* d_g, unsigned char* d_m) {
+  const size_t vb = std::max<size_t>(1, (size_t)h->nnz) * h->esize();
+  auto cleanup = [&]() { cudaFree(d_g); cudaFree(d_m); };
   cudaFree(h->d_fg);                 // the previous call's finite grounds; this call's replace them
   h->d_fg = nullptr;
+  cudaError_t e0 = cudaSuccess;
   if (!h->d_vals0) {
-    CK(h, cudaMalloc(&h->d_vals0, vb));
-    CK(h, cudaMemcpyAsync(h->d_vals0, h->d_vals, vb, cudaMemcpyDeviceToDevice, h->stream));
+    e0 = cudaMalloc(&h->d_vals0, vb);
+    if (e0 == cudaSuccess) e0 = cudaMemcpyAsync(h->d_vals0, h->d_vals, vb, cudaMemcpyDeviceToDevice, h->stream);
   } else {
-    CK(h, cudaMemcpyAsync(h->d_vals, h->d_vals0, vb, cudaMemcpyDeviceToDevice, h->stream));
+    e0 = cudaMemcpyAsync(h->d_vals, h->d_vals0, vb, cudaMemcpyDeviceToDevice, h->stream);
   }
-  void* d_g = nullptr;
-  unsigned char* d_m = nullptr;
-  auto cleanup = [&]() { cudaFree(d_g); cudaFree(d_m); };
-  if (finite_g) {
-    cudaError_t e = cudaMalloc(&d_g, (size_t)h->n * es);
-    if (e == cudaSuccess) e = h2d(h, d_g, finite_g, (size_t)h->n * es);
-    if (e != cudaSuccess) { cleanup(); return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (finite grounds)", cudaGetErrorString(e)); }
-  }
-  if (dirichlet) {
-    cudaError_t e = cudaMalloc(&d_m, (size_t)h->n);
-    if (e == cudaSuccess) e = h2d(h, d_m, dirichlet, (size_t)h->n);
-    if (e != cudaSuccess) { cleanup(); return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (Dirichlet mask)", cudaGetErrorString(e)); }
-  }
-  if (finite_g || dirichlet) {
+  if (e0 != cudaSuccess) { cleanup(); return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (pristine values)", cudaGetErrorString(e0)); }
+  if (d_g || d_m) {
     const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
     with_type(h, [&](auto t) {
       using T = decltype(t);
@@ -2728,6 +2765,29 @@ int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* 
   return CS_B200_OK;
 }
 
+int cs_b200_set_grounds(cs_b200_handle* h, const void* finite_g, const uint8_t* dirichlet) {
+  if (!h) return CS_B200_ERR_ARG;
+  if (int rc = grounds_supported(h)) return rc;
+  cudaSetDevice(h->device);
+  h->err.clear();
+  const size_t es = h->esize();
+  cudaEventRecord(h->ev0, h->stream);
+  void* d_g = nullptr;
+  unsigned char* d_m = nullptr;
+  auto cleanup = [&]() { cudaFree(d_g); cudaFree(d_m); };
+  if (finite_g) {
+    cudaError_t e = cudaMalloc(&d_g, (size_t)h->n * es);
+    if (e == cudaSuccess) e = h2d(h, d_g, finite_g, (size_t)h->n * es);
+    if (e != cudaSuccess) { cleanup(); return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (finite grounds)", cudaGetErrorString(e)); }
+  }
+  if (dirichlet) {
+    cudaError_t e = cudaMalloc(&d_m, (size_t)h->n);
+    if (e == cudaSuccess) e = h2d(h, d_m, dirichlet, (size_t)h->n);
+    if (e != cudaSuccess) { cleanup(); return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (Dirichlet mask)", cudaGetErrorString(e)); }
+  }
+  return apply_grounds(h, d_g, d_m);
+}
+
 int cs_b200_get_dims(const cs_b200_handle* h, int64_t* n, int64_t* nnz) {
   if (!h) return CS_B200_ERR_ARG;
   if (n) *n = h->n;
@@ -2742,6 +2802,7 @@ void cs_b200_destroy(cs_b200_handle* h) {
   if (h->owns_matrix) { cudaFree(h->d_rowptr); cudaFree(h->d_colidx); cudaFree(h->d_vals); }
   cudaFree(h->d_vals0);
   cudaFree(h->d_fg);
+  cudaFree(h->d_plan);
   cudaFree(h->d_bptr); cudaFree(h->d_cum_branch); cudaFree(h->d_branch_stage);
   void* bufs[] = {h->d_dinv, h->d_bstart, h->X, h->R, h->R2, h->P, h->P2, h->AP, h->B, h->stage,
                   h->d_cum, h->d_max, h->d_ctl, h->d_partials, h->d_flush};
@@ -2823,15 +2884,14 @@ int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* h
   return CS_B200_OK;
 }
 
-int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
-  if (!h || !ncomp) return set_err(h, CS_B200_ERR_ARG, "bad components arguments");
-  cudaSetDevice(h->device);
-  h->err.clear();
+// The labels of cs_b200_components on the device: ncomp, and with `out` non-null each row's label in out (n int32
+// on the device; the stream is synchronised on return).
+static int label_components(cs_b200_handle* h, int64_t* ncomp, int* out) {
   const int n = (int)h->n;
   *ncomp = 0;
   if (n == 0) return CS_B200_OK;
   // scratch from the stream-ordered pool, released before return: parent, root flags, their exclusive scan,
-  // each row's root, then its label (n each) and cub's temporary storage
+  // each row's root, then its label (n each, the last one in `out` when given) and cub's temporary storage
   size_t tb = 0;
   CK(h, cub::DeviceScan::ExclusiveSum(nullptr, tb, (const int*)nullptr, (int*)nullptr, n, h->stream));
   const size_t ib = (size_t)n * sizeof(int), ia = (ib + 255) & ~(size_t)255;
@@ -2841,7 +2901,7 @@ int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
   int* parent = (int*)s;
   int* root = (int*)(s + off_root);
   int* idx = (int*)(s + off_idx);
-  int* lab = (int*)(s + off_lab);
+  int* lab = out ? out : (int*)(s + off_lab);
   const int g = (int)std::min<int64_t>((h->n + 255) / 256, (int64_t)h->num_sms * 32);
   constexpr int CHUNK = 16;
   const int ge = (int)std::max<int64_t>(1, std::min<int64_t>((h->nnz / CHUNK + 255) / 256, (int64_t)h->num_sms * 32));
@@ -2855,17 +2915,225 @@ int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
   cudaError_t e = cub::DeviceScan::ExclusiveSum(s + off_tmp, tb, root, idx, n, h->stream);
   int total = 0, last_flag = 0;
   if (e == cudaSuccess) {
-    if (comp_of) k_cc_label<<<g, 256, 0, h->stream>>>(n, lab, idx);
+    if (out) k_cc_label<<<g, 256, 0, h->stream>>>(n, lab, idx);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaMemcpyAsync(&total, idx + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
   if (e == cudaSuccess) e = cudaMemcpyAsync(&last_flag, root + n - 1, sizeof(int), cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess && comp_of) e = cudaMemcpyAsync(comp_of, lab, ib, cudaMemcpyDeviceToHost, h->stream);
   cudaFreeAsync(s, h->stream);
   if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
   if (e != cudaSuccess) return set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (components)", cudaGetErrorString(e));
-  h->stats.kernel_launches += comp_of ? 5 : 4;
+  h->stats.kernel_launches += out ? 5 : 4;
   *ncomp = (int64_t)total + last_flag;
+  return CS_B200_OK;
+}
+
+int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of) {
+  if (!h || !ncomp) return set_err(h, CS_B200_ERR_ARG, "bad components arguments");
+  cudaSetDevice(h->device);
+  h->err.clear();
+  *ncomp = 0;
+  if (h->n == 0) return CS_B200_OK;
+  int* lab = nullptr;
+  if (comp_of) CK(h, cudaMallocAsync((void**)&lab, (size_t)h->n * sizeof(int), h->stream));
+  int rc = label_components(h, ncomp, lab);
+  if (rc == CS_B200_OK && comp_of) {
+    cudaError_t e = cudaMemcpyAsync(comp_of, lab, (size_t)h->n * sizeof(int), cudaMemcpyDeviceToHost, h->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    if (e != cudaSuccess) rc = set_err(h, CS_B200_ERR_CUDA, "CUDA error %s (components)", cudaGetErrorString(e));
+  }
+  if (lab) { cudaFreeAsync(lab, h->stream); cudaStreamSynchronize(h->stream); }
+  return rc;
+}
+
+int cs_b200_plan_advanced(cs_b200_handle* h, int64_t nrows, int64_t ncols, const int32_t* nodemap,
+                          const void* src, const void* gnd, int dtype, int policy,
+                          int64_t* ncol, int64_t* nsolved, int64_t* nset_rows, int64_t* nsrc_rows,
+                          int* finite_applied) {
+  if (!h) return CS_B200_ERR_ARG;
+  if (!nodemap || !src || !gnd || !ncol || !nsolved || !nset_rows || !nsrc_rows || !finite_applied)
+    return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: a NULL argument");
+  if (dtype != CS_B200_F32 && dtype != CS_B200_F64)
+    return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: bad dtype %d", dtype);
+  if (policy < 0 || policy > 3)
+    return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: bad policy %d (0 keepall ... 3 rmvall)", policy);
+  // at most 2^30 cells: every index, grid-stride step and launch size below stays inside int32
+  if (nrows <= 0 || ncols <= 0 || nrows > (int64_t(1) << 30) / ncols)
+    return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: a %lld x %lld raster does not fit (2^30 cells at most)",
+                   (long long)nrows, (long long)ncols);
+  cudaSetDevice(h->device);
+  h->err.clear();
+  cudaFree(h->d_plan);                // a second plan replaces the first
+  h->d_plan = nullptr;
+  h->plan_ncol = h->plan_nset = h->plan_nsrc = 0;
+  const int ncell = (int)(nrows * ncols), n = (int)h->n;
+  const size_t ms = dtype == CS_B200_F64 ? 8 : 4;
+  cudaStream_t st = h->stream;
+  const int g = (int)std::min<int64_t>((std::max(ncell, n) + 255) / 256, (int64_t)h->num_sms * 32);
+  PoolScratch sc(st);
+  int *d_nm, *cnt, *ptr, *val, *val2, *flags;
+  unsigned *key, *key2;
+  void *d_src, *d_gnd;
+  double *s, *gv;
+  CK(h, sc.get(&d_nm, ncell));
+  CK(h, sc.get((char**)&d_src, ncell * ms));
+  CK(h, sc.get((char**)&d_gnd, ncell * ms));
+  CK(h, sc.get(&key, ncell)); CK(h, sc.get(&key2, ncell));
+  CK(h, sc.get(&val, ncell)); CK(h, sc.get(&val2, ncell));
+  CK(h, sc.get(&cnt, (size_t)n + 1)); CK(h, sc.get(&ptr, (size_t)n + 1));
+  CK(h, sc.get(&s, n)); CK(h, sc.get(&gv, n));
+  CK(h, sc.get(&flags, 2));
+  void* d_f = nullptr;               // the finite grounds: the handle keeps them when they are applied
+  CK(h, cudaMalloc(&d_f, std::max<size_t>((size_t)n, 1) * h->esize()));
+  struct FreeF { void*& p; ~FreeF() { cudaFree(p); } } free_f{d_f};
+  CK(h, cudaMemcpyAsync(d_nm, nodemap, (size_t)ncell * sizeof(int), cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemcpyAsync(d_src, src, (size_t)ncell * ms, cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemcpyAsync(d_gnd, gnd, (size_t)ncell * ms, cudaMemcpyHostToDevice, st));
+  CK(h, cudaMemsetAsync(cnt, 0, ((size_t)n + 1) * sizeof(int), st));
+  CK(h, cudaMemsetAsync(flags, 0, 2 * sizeof(int), st));
+  // expand: every cell keyed by its node in row-major order; stable radix sort: each node's cells in np.add.at's
+  // order; compress: the node's range from the exclusive scan of the cell counts
+  k_adv_cells<<<g, 256, 0, st>>>(ncell, (int)nrows, (int)ncols, n, d_nm, key, val, cnt, flags);
+  CK(h, cudaGetLastError());
+  const int kb = nbits_for((unsigned)n);
+  size_t tb = 0, tb2 = 0;
+  CK(h, cub::DeviceRadixSort::SortPairs(nullptr, tb, key, key2, val, val2, ncell, 0, kb, st));
+  CK(h, cub::DeviceScan::ExclusiveSum(nullptr, tb2, cnt, ptr, n + 1, st));
+  char* tmp;
+  CK(h, sc.get(&tmp, std::max(tb, tb2)));
+  CK(h, cub::DeviceRadixSort::SortPairs(tmp, tb, key, key2, val, val2, ncell, 0, kb, st));
+  CK(h, cub::DeviceScan::ExclusiveSum(tmp, tb2, cnt, ptr, n + 1, st));
+  with_type(h, [&](auto t) {
+    using T = decltype(t);
+    if (dtype == CS_B200_F64)
+      k_adv_node_values<double, T><<<g, 256, 0, st>>>(n, (int)nrows, (int)ncols, ptr, val2, (const double*)d_src,
+                                                      (const double*)d_gnd, policy, s, gv, (T*)d_f, flags);
+    else
+      k_adv_node_values<float, T><<<g, 256, 0, st>>>(n, (int)nrows, (int)ncols, ptr, val2, (const float*)d_src,
+                                                     (const float*)d_gnd, policy, s, gv, (T*)d_f, flags);
+  });
+  CK(h, cudaGetLastError());
+  int hf[2] = {0, 0};
+  CK(h, cudaMemcpyAsync(hf, flags, sizeof hf, cudaMemcpyDeviceToHost, st));
+  CK(h, cudaStreamSynchronize(st));
+  h->stats.kernel_launches += 2;
+  if (hf[0] & 1) return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: a node map entry outside [0, %d]", n);
+  if (hf[0] & 2) return set_err(h, CS_B200_ERR_ARG, "cs_b200_plan_advanced: a node of the handle has no cell");
+  if (hf[1])                         // finite grounds to apply: the handle must take them before any plan is kept
+    if (int rc = grounds_supported(h)) return rc;
+  // components of the pristine operator; each component's rows ascending (stable sort of 0 ... n-1 by label)
+  int64_t nc64 = 0;
+  int *lab, *lab2, *rows, *ccnt, *cptr;
+  CK(h, sc.get(&lab, n)); CK(h, sc.get(&lab2, n)); CK(h, sc.get(&rows, n));
+  if (int rc = label_components(h, &nc64, lab)) return rc;
+  const int ncomp = (int)nc64;
+  CK(h, sc.get(&ccnt, (size_t)ncomp + 1)); CK(h, sc.get(&cptr, (size_t)ncomp + 1));
+  CK(h, cudaMemsetAsync(ccnt, 0, ((size_t)ncomp + 1) * sizeof(int), st));
+  k_adv_rows<<<g, 256, 0, st>>>(n, lab, key, val, ccnt);
+  CK(h, cudaGetLastError());
+  const int lb = nbits_for((unsigned)ncomp);
+  size_t tb4 = 0;
+  CK(h, cub::DeviceRadixSort::SortPairs(nullptr, tb4, key, key2, val, rows, n, 0, lb, st));
+  char* tmp4;
+  CK(h, sc.get(&tmp4, tb4));
+  CK(h, cub::DeviceRadixSort::SortPairs(tmp4, tb4, key, key2, val, rows, n, 0, lb, st));
+  CK(h, cub::DeviceScan::ExclusiveSum(tmp, tb2, ccnt, cptr, ncomp + 1, st));
+  // the nonzero terms of each component's two sums, compacted in position order, for numpy's summation tree
+  auto cub2 = [&](auto&& call) -> cudaError_t {   // cub's size query, its scratch, then the call
+    size_t bytes = 0;
+    cudaError_t e = call((void*)nullptr, bytes);
+    char* t = nullptr;
+    if (e == cudaSuccess) e = sc.get(&t, bytes);
+    return e == cudaSuccess ? call((void*)t, bytes) : e;
+  };
+  int *nzs, *nzg, *ninf, *nsrcc, *zs_ptr, *zg_ptr, *zs_pos, *zg_pos, *nsel;
+  unsigned char *fs, *fgz;
+  for (int** a : {&nzs, &nzg, &ninf, &nsrcc, &zs_ptr, &zg_ptr}) {
+    CK(h, sc.get(a, (size_t)ncomp + 1));
+    CK(h, cudaMemsetAsync(*a, 0, ((size_t)ncomp + 1) * sizeof(int), st));
+  }
+  CK(h, sc.get(&zs_pos, n)); CK(h, sc.get(&zg_pos, n)); CK(h, sc.get(&nsel, 1));
+  CK(h, sc.get(&fs, n)); CK(h, sc.get(&fgz, n));
+  const unsigned* labs = key2;                    // each sorted position's label
+  k_adv_counts<<<g, 256, 0, st>>>(n, rows, labs, s, gv, nzs, nzg, ninf, nsrcc, fs, fgz);
+  CK(h, cudaGetLastError());
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nzs, zs_ptr, ncomp + 1, st); }));
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nzg, zg_ptr, ncomp + 1, st); }));
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, val, fs, zs_pos, nsel, n, st); }));
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, val, fgz, zg_pos, nsel, n, st); }));
+  long long *solved, *iscol, *nset, *nsrc, *xsolved, *colx, *setx, *srcx;
+  for (long long** a : {&solved, &iscol, &nset, &nsrc, &xsolved, &colx, &setx, &srcx}) CK(h, sc.get(a, (size_t)ncomp + 1));
+  for (long long* a : {solved, iscol, nset, nsrc}) CK(h, cudaMemsetAsync(a + ncomp, 0, sizeof(long long), st));
+  const int gs = (int)std::max<int64_t>(1, std::min<int64_t>((ncomp + ADV_SUM_THREADS - 1) / ADV_SUM_THREADS,
+                                                             (int64_t)h->num_sms * 32));
+  k_adv_sums<<<gs, ADV_SUM_THREADS, 0, st>>>(ncomp, cptr, rows, s, gv, zs_ptr, zs_pos, zg_ptr, zg_pos, ninf, nsrcc,
+                                             solved, iscol, nset, nsrc);
+  CK(h, cudaGetLastError());
+  long long tot[4];
+  {
+    long long* in[4] = {solved, iscol, nset, nsrc};
+    long long* outx[4] = {xsolved, colx, setx, srcx};
+    for (int i = 0; i < 4; ++i) {
+      CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in[i], outx[i], ncomp + 1, st); }));
+      CK(h, cudaMemcpyAsync(tot + i, outx[i] + ncomp, sizeof(long long), cudaMemcpyDeviceToHost, st));
+    }
+  }
+  CK(h, cudaStreamSynchronize(st));
+  const PlanView sz(nullptr, tot[1], tot[2], tot[3], n);
+  CK(h, cudaMalloc(&h->d_plan, std::max<size_t>(sz.bytes, 1)));
+  const PlanView pv(h->d_plan, tot[1], tot[2], tot[3], n);
+  CK(h, cudaMemsetAsync(pv.set_ptr, 0, sizeof(long long), st));
+  CK(h, cudaMemsetAsync(pv.src_ptr, 0, sizeof(long long), st));
+  CK(h, cudaMemsetAsync(pv.col_of_row, 0xff, (size_t)n * sizeof(int), st));
+  const int gc = (int)std::max<int64_t>(1, std::min<int64_t>((ncomp + 255) / 256, (int64_t)h->num_sms * 32));
+  k_adv_ptrs<<<gc, 256, 0, st>>>(ncomp, iscol, colx, setx, nset, srcx, nsrc, pv.col_comp, pv.set_ptr, pv.src_ptr);
+  CK(h, cudaGetLastError());
+  // fs / fgz are done with: they take the set and source flags; zs_pos / zg_pos the selected rows
+  k_adv_mark<<<g, 256, 0, st>>>(n, rows, labs, s, gv, iscol, colx, pv.col_of_row, fs, fgz);
+  CK(h, cudaGetLastError());
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, rows, fs, zs_pos, nsel, n, st); }));
+  CK(h, cub2([&](void* t, size_t& b) { return cub::DeviceSelect::Flagged(t, b, rows, fgz, zg_pos, nsel, n, st); }));
+  const int gn = (int)std::max<int64_t>(1, std::min<int64_t>((tot[2] + tot[3] + 255) / 256, (int64_t)h->num_sms * 32));
+  k_adv_widen<<<gn, 256, 0, st>>>((int)tot[2], zs_pos, (int)tot[3], zg_pos, s, pv.set_rows, pv.src_rows, pv.src_vals);
+  CK(h, cudaGetLastError());
+  CK(h, cudaStreamSynchronize(st));
+  h->stats.kernel_launches += 5;
+  h->plan_ncol = tot[1];
+  h->plan_nset = tot[2];
+  h->plan_nsrc = tot[3];
+  *ncol = tot[1];
+  *nsolved = tot[0];
+  *nset_rows = tot[2];
+  *nsrc_rows = tot[3];
+  *finite_applied = hf[1];
+  if (!hf[1]) return CS_B200_OK;     // no finite ground: the operator stays as it is
+  cudaEventRecord(h->ev0, st);
+  void* fg = d_f;
+  d_f = nullptr;
+  return apply_grounds(h, fg, nullptr);
+}
+
+int cs_b200_read_advanced_plan(cs_b200_handle* h, int64_t* col_comp, int64_t* set_ptr, int64_t* set_rows,
+                               int64_t* src_ptr, int64_t* src_rows, double* src_vals, int32_t* col_of_row) {
+  if (!h) return CS_B200_ERR_ARG;
+  if (!h->d_plan) return set_err(h, CS_B200_ERR_ARG, "cs_b200_read_advanced_plan: no plan (cs_b200_plan_advanced)");
+  if (!col_comp || !set_ptr || !set_rows || !src_ptr || !src_rows || !src_vals || !col_of_row)
+    return set_err(h, CS_B200_ERR_ARG, "cs_b200_read_advanced_plan: a NULL argument");
+  cudaSetDevice(h->device);
+  const int64_t nc = h->plan_ncol, ns = h->plan_nset, nv = h->plan_nsrc;
+  const PlanView pv(h->d_plan, nc, ns, nv, h->n);
+  const cudaMemcpyKind d2h = cudaMemcpyDeviceToHost;
+  CK(h, cudaMemcpyAsync(col_comp, pv.col_comp, (size_t)nc * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(set_ptr, pv.set_ptr, (size_t)(nc + 1) * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(set_rows, pv.set_rows, (size_t)ns * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(src_ptr, pv.src_ptr, (size_t)(nc + 1) * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(src_rows, pv.src_rows, (size_t)nv * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(src_vals, pv.src_vals, (size_t)nv * 8, d2h, h->stream));
+  CK(h, cudaMemcpyAsync(col_of_row, pv.col_of_row, (size_t)h->n * 4, d2h, h->stream));
+  CK(h, cudaStreamSynchronize(h->stream));
+  cudaFree(h->d_plan);
+  h->d_plan = nullptr;
+  h->plan_ncol = h->plan_nset = h->plan_nsrc = 0;
   return CS_B200_OK;
 }
 

@@ -3129,4 +3129,222 @@ __global__ void k_cc_label(int n, int* __restrict__ lab, const int* __restrict__
   for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) lab[v] = idx[lab[v]];
 }
 
+// ---------------------------------------------------------------------------
+// raster advanced mode's column plan (cs_b200_plan_advanced): node values summed in np.add.at's order, the
+// conflict policy, component sums and the columns, with integer atomics only
+// ---------------------------------------------------------------------------
+// key[i] = the 0-based node of row-major cell i = r * ncols + c (n: no node), val[i] = i; cnt[v] counts node v's
+// cells; *bad |= 1 for a node map entry outside [0, n]
+__global__ void k_adv_cells(int ncell, int nrows, int ncols, int n, const int* __restrict__ nodemap,
+                            unsigned* __restrict__ key, int* __restrict__ val, int* __restrict__ cnt, int* bad) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < ncell; i += gridDim.x * blockDim.x) {
+    const int r = i / ncols, c = i - r * ncols;
+    const int v = nodemap[(int64_t)c * nrows + r];
+    unsigned k = (unsigned)n;
+    if (v < 0 || v > n) atomicOr(bad, 1);
+    else if (v > 0) { k = (unsigned)(v - 1); atomicAdd(cnt + k, 1); }
+    key[i] = k;
+    val[i] = i;
+  }
+}
+
+// key[r] = lab[r], val[r] = r, cnt[lab[r]] counts each component's rows
+__global__ void k_adv_rows(int n, const int* __restrict__ lab, unsigned* __restrict__ key, int* __restrict__ val,
+                           int* __restrict__ cnt) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+    key[r] = (unsigned)lab[r];
+    val[r] = r;
+    atomicAdd(cnt + lab[r], 1);
+  }
+}
+
+// One thread per node: its cells (ptr / cell: row-major indices grouped by node, ascending) summed in that order
+// from +0.0, zeros skipped, as np.add.at adds the selected cells; f = the finite part of the summed grounds
+// (before the policy, as resolve_conflicts takes it); then the policy and the Inf-ground rule.  flags[0] |= 2 for
+// a node without a cell, flags[1] = 1 when some f != 0.
+template <typename M, typename T>
+__global__ void k_adv_node_values(int n, int nrows, int ncols, const int* __restrict__ ptr,
+                                  const int* __restrict__ cell, const M* __restrict__ src,
+                                  const M* __restrict__ gnd, int policy, double* __restrict__ s_out,
+                                  double* __restrict__ g_out, T* __restrict__ f_out, int* flags) {
+  for (int v = blockIdx.x * blockDim.x + threadIdx.x; v < n; v += gridDim.x * blockDim.x) {
+    const int b = ptr[v], e = ptr[v + 1];
+    if (b == e) atomicOr(flags, 2);
+    double s = 0.0, g = 0.0;
+    for (int j = b; j < e; ++j) {
+      const int i = cell[j], r = i / ncols;
+      const int64_t x = (int64_t)(i - r * ncols) * nrows + r;     // column-major cell
+      const double a = (double)src[x], q = (double)gnd[x];
+      if (a != 0.0) s += a;
+      if (q != 0.0) g += q;
+    }
+    const double f = isfinite(g) ? g : 0.0;
+    f_out[v] = (T)f;
+    if (f != 0.0) atomicOr(flags + 1, 1);
+    const bool both = s != 0.0 && g != 0.0;
+    if (both && (policy == 1 || policy == 3)) s = 0.0;          // rmvsrc, rmvall (sources only)
+    else if (both && policy == 2) g = 0.0;                      // rmvgnd
+    if (isinf(g) && s > 0.0) g = 0.0;
+    s_out[v] = s;
+    g_out[v] = g;
+  }
+}
+
+// Per sorted position j (rows: each component's rows ascending, lab: their labels): each component's counts of
+// nonzero source and ground terms, Inf-ground rows and source rows (s != 0, g != Inf), with integer atomics, and
+// the flags that select the nonzero terms of the two sums.
+__global__ void k_adv_counts(int n, const int* __restrict__ rows, const unsigned* __restrict__ lab,
+                             const double* __restrict__ s, const double* __restrict__ g, int* __restrict__ nzs,
+                             int* __restrict__ nzg, int* __restrict__ ninf, int* __restrict__ nsrc,
+                             unsigned char* __restrict__ fs, unsigned char* __restrict__ fg) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const int r = rows[j], c = (int)lab[j];
+    const double sv = s[r], gv = g[r];
+    const bool inf = gv == __longlong_as_double(0x7ff0000000000000LL);
+    fs[j] = sv != 0.0;
+    fg[j] = gv != 0.0;
+    if (sv != 0.0) atomicAdd(nzs + c, 1);
+    if (gv != 0.0) atomicAdd(nzg + c, 1);
+    if (inf) atomicAdd(ninf + c, 1);
+    if (sv != 0.0 && !inf) atomicAdd(nsrc + c, 1);
+  }
+}
+
+constexpr int ADV_SUM_THREADS = 64;
+constexpr int ADV_SUM_DEPTH = 32;   // frames of the pairwise recursion: ranges of <= 2^30 terms need <= 24
+
+// numpy's pairwise_sum (umath/loops_utils.h: fewer than 8 terms added in order from 0; up to 128 terms in 8 strided
+// accumulators r0..r7 combined as ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7)), then the remaining n % 8 in
+// order; longer ranges split at n / 2 rounded down to a multiple of 8, left + right) over the n terms of one
+// component, of which only the nz nonzero ones are given: positions j = pos[0..nz) ascending (base: the
+// component's first position), values x[rows[j]].  A +0.0 term leaves every partial sum as it is, so leaving the
+// zeros out, and skipping subtrees without a nonzero term, gives the same bits.  The recursion's frames are the
+// thread's column of shared memory.
+__device__ double adv_pairwise(int n, int base, const int* __restrict__ pos, int nz, const int* __restrict__ rows,
+                               const double* __restrict__ x, int* f_lo, int* f_len, double* f_left) {
+  const int t = threadIdx.x;
+  int k = 0, sp = 0, lo = 0, len = n;
+  unsigned right = 0;                                      // bit d: frame d's left half is done
+  for (;;) {
+    double v = 0.0;
+    if (k >= nz || pos[k] - base >= lo + len || len <= 128) {
+      if (k < nz && pos[k] - base < lo + len) {            // a leaf with nonzero terms
+        const int m = len < 8 ? 0 : len - (len & 7);
+        double r0 = 0.0, r1 = 0.0, r2 = 0.0, r3 = 0.0, r4 = 0.0, r5 = 0.0, r6 = 0.0, r7 = 0.0;
+        for (; k < nz && pos[k] - base < lo + m; ++k) {
+          const double a = x[rows[pos[k]]];
+          switch ((pos[k] - base - lo) & 7) {
+            case 0: r0 += a; break;
+            case 1: r1 += a; break;
+            case 2: r2 += a; break;
+            case 3: r3 += a; break;
+            case 4: r4 += a; break;
+            case 5: r5 += a; break;
+            case 6: r6 += a; break;
+            default: r7 += a; break;
+          }
+        }
+        v = ((r0 + r1) + (r2 + r3)) + ((r4 + r5) + (r6 + r7));
+        for (; k < nz && pos[k] - base < lo + len; ++k) v += x[rows[pos[k]]];
+      }
+      for (;;) {                                           // hand v up to the frames above
+        if (sp == 0) return v;
+        const int d = sp - 1, idx = d * ADV_SUM_THREADS + t;
+        if (!((right >> d) & 1u)) {
+          f_left[idx] = v;
+          right |= 1u << d;
+          int h = f_len[idx] / 2;
+          h -= h % 8;
+          lo = f_lo[idx] + h;
+          len = f_len[idx] - h;
+          break;
+        }
+        v = f_left[idx] + v;
+        right &= ~(1u << d);
+        --sp;
+      }
+    } else {                                               // split: descend into the left half
+      const int idx = sp * ADV_SUM_THREADS + t;
+      f_lo[idx] = lo;
+      f_len[idx] = len;
+      right &= ~(1u << sp);
+      ++sp;
+      len = len / 2;
+      len -= len % 8;
+    }
+  }
+}
+
+// One thread per component: its source and ground sums by adv_pairwise over the compacted nonzero terms
+// (zs_pos / zg_pos, CSR zs_ptr / zg_ptr), solved = both != 0 (NaN counts); a solved component with a source row off
+// the Inf grounds is a column.  Per component: solved, column, and for a column its Inf-ground and source row
+// counts (0 otherwise).
+__global__ void __launch_bounds__(ADV_SUM_THREADS)
+k_adv_sums(int ncomp, const int* __restrict__ cptr, const int* __restrict__ rows, const double* __restrict__ s,
+           const double* __restrict__ g, const int* __restrict__ zs_ptr, const int* __restrict__ zs_pos,
+           const int* __restrict__ zg_ptr, const int* __restrict__ zg_pos, const int* __restrict__ ninf,
+           const int* __restrict__ nsrc, long long* __restrict__ solved, long long* __restrict__ iscol,
+           long long* __restrict__ nset, long long* __restrict__ nsrc_col) {
+  __shared__ int f_lo[ADV_SUM_DEPTH * ADV_SUM_THREADS], f_len[ADV_SUM_DEPTH * ADV_SUM_THREADS];
+  __shared__ double f_left[ADV_SUM_DEPTH * ADV_SUM_THREADS];
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < ncomp; c += gridDim.x * blockDim.x) {
+    const int base = cptr[c], n = cptr[c + 1] - base;
+    const double ss = adv_pairwise(n, base, zs_pos + zs_ptr[c], zs_ptr[c + 1] - zs_ptr[c], rows, s, f_lo, f_len, f_left);
+    const double gs = adv_pairwise(n, base, zg_pos + zg_ptr[c], zg_ptr[c + 1] - zg_ptr[c], rows, g, f_lo, f_len, f_left);
+    const bool sol = ss != 0.0 && gs != 0.0, col = sol && nsrc[c] > 0;
+    solved[c] = sol;
+    iscol[c] = col;
+    nset[c] = col ? ninf[c] : 0;
+    nsrc_col[c] = col ? nsrc[c] : 0;
+  }
+}
+
+// One thread per column component: its label and the ends of its set and source row ranges (colx / setx / srcx:
+// the exclusive scans of iscol / nset / nsrc; set_ptr[0] and src_ptr[0] are written by the caller).
+__global__ void k_adv_ptrs(int ncomp, const long long* __restrict__ iscol, const long long* __restrict__ colx,
+                           const long long* __restrict__ setx, const long long* __restrict__ nset,
+                           const long long* __restrict__ srcx, const long long* __restrict__ nsrc,
+                           long long* __restrict__ col_comp, long long* __restrict__ set_ptr,
+                           long long* __restrict__ src_ptr) {
+  for (int c = blockIdx.x * blockDim.x + threadIdx.x; c < ncomp; c += gridDim.x * blockDim.x) {
+    if (!iscol[c]) continue;
+    const long long col = colx[c];
+    col_comp[col] = c;
+    set_ptr[col + 1] = setx[c] + nset[c];
+    src_ptr[col + 1] = srcx[c] + nsrc[c];
+  }
+}
+
+// Per sorted position j: col_of_row of the rows of column components, and the flags that select each column's
+// Inf-ground rows and source rows (in position order: columns in label order, rows ascending).
+__global__ void k_adv_mark(int n, const int* __restrict__ rows, const unsigned* __restrict__ lab,
+                           const double* __restrict__ s, const double* __restrict__ g,
+                           const long long* __restrict__ iscol, const long long* __restrict__ colx,
+                           int* __restrict__ col_of_row, unsigned char* __restrict__ fset,
+                           unsigned char* __restrict__ fsrc) {
+  for (int j = blockIdx.x * blockDim.x + threadIdx.x; j < n; j += gridDim.x * blockDim.x) {
+    const int r = rows[j], c = (int)lab[j];
+    const bool col = iscol[c] != 0;
+    const bool inf = g[r] == __longlong_as_double(0x7ff0000000000000LL);
+    if (col) col_of_row[r] = (int)colx[c];
+    fset[j] = col && inf;
+    fsrc[j] = col && s[r] != 0.0 && !inf;
+  }
+}
+
+// The selected set rows and source rows (int32, in order) into the plan: int64 rows and the sources' node values.
+__global__ void k_adv_widen(int nset, const int* __restrict__ sel_set, int nsrc, const int* __restrict__ sel_src,
+                            const double* __restrict__ s, long long* __restrict__ set_rows,
+                            long long* __restrict__ src_rows, double* __restrict__ src_vals) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < nset + nsrc; i += gridDim.x * blockDim.x) {
+    if (i < nset) {
+      set_rows[i] = sel_set[i];
+    } else {
+      const int r = sel_src[i - nset];
+      src_rows[i - nset] = r;
+      src_vals[i - nset] = s[r];
+    }
+  }
+}
+
 }  // namespace csb

@@ -56,6 +56,9 @@ class CUDASolver:
     pairwise_raster: bool = False    # raster pairwise with distinct point ids: every component's pairs as columns
                                      # on one whole-raster handle, components labelled on the device
                                      # (core._raster_pairs_device) instead of a host graph and a handle per component
+    front_end_on_device: bool = False    # raster advanced, one-to-all (onetoall_raster) and focal regions: node
+                                         # map, component labels and advanced mode's columns from the whole-raster
+                                         # handle (components, plan_advanced) instead of a host graph
 
     @property
     def dtype(self):
@@ -434,6 +437,36 @@ class B200Factor:
         comp_of = np.empty(self.n, dtype=np.int32)
         _lib.check(self._lib, self._h, self._lib.cs_b200_components(self._h, C.byref(nc), _lib._ptr(comp_of)))
         return nc.value, comp_of
+
+    POLICIES = ("keepall", "rmvsrc", "rmvgnd", "rmvall")
+
+    def plan_advanced(self, nodemap, source_map, ground_map, policy):
+        """Raster advanced mode's columns planned on the device (cs_b200_plan_advanced + _read_advanced_plan):
+        `nodemap` this handle's node map, the advanced-mode maps (float32 when both are, else float64), `policy`
+        a name of POLICIES; any other value is keepall, as resolve_conflicts treats it.  Applies the finite grounds to the handle when any is nonzero.  Returns dict with
+        nsolved, finite_applied, col_comp (ncol,), set_ptr / src_ptr (ncol + 1,), set_rows, src_rows (int64),
+        src_vals (float64) and col_of_row (n,) int32."""
+        sm, gm = np.asarray(source_map), np.asarray(ground_map)
+        dt = np.float32 if sm.dtype == np.float32 and gm.dtype == np.float32 else np.float64
+        nm = np.asfortranarray(nodemap, dtype=np.int32)
+        sm, gm = np.asfortranarray(sm, dtype=dt), np.asfortranarray(gm, dtype=dt)
+        if sm.shape != nm.shape or gm.shape != nm.shape:
+            raise ValueError("the source and ground maps must have the node map's shape")
+        ncol, nsolved, nset, nsrc = (C.c_int64() for _ in range(4))
+        fin = C.c_int()
+        _lib.check(self._lib, self._h, self._lib.cs_b200_plan_advanced(
+            self._h, nm.shape[0], nm.shape[1], _lib._ptr(nm), _lib._ptr(sm), _lib._ptr(gm), _lib.dtype_code(dt),
+            self.POLICIES.index(policy) if policy in self.POLICIES else 0, C.byref(ncol), C.byref(nsolved), C.byref(nset), C.byref(nsrc),
+            C.byref(fin)))
+        k = ncol.value
+        out = dict(nsolved=nsolved.value, finite_applied=bool(fin.value), col_comp=np.empty(k, dtype=np.int64),
+                   set_ptr=np.empty(k + 1, dtype=np.int64), set_rows=np.empty(nset.value, dtype=np.int64),
+                   src_ptr=np.empty(k + 1, dtype=np.int64), src_rows=np.empty(nsrc.value, dtype=np.int64),
+                   src_vals=np.empty(nsrc.value, dtype=np.float64), col_of_row=np.empty(self.n, dtype=np.int32))
+        _lib.check(self._lib, self._h, self._lib.cs_b200_read_advanced_plan(
+            self._h, *(_lib._ptr(out[a]) for a in ("col_comp", "set_ptr", "set_rows", "src_ptr", "src_rows",
+                                                    "src_vals", "col_of_row"))))
+        return out
 
     def read_branch_currents(self):
         """The cumulative branch vector (nb,) that solve_pairs(want_branch=True, accumulate=True) adds into."""

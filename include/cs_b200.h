@@ -238,6 +238,37 @@ int cs_b200_branch_index(cs_b200_handle* h, int64_t* nb, int64_t* lo, int64_t* h
  * races.  Scratch comes from the stream-ordered pool and is released before return.                      */
 int cs_b200_components(cs_b200_handle* h, int64_t* ncomp, int32_t* comp_of);
 
+/* Raster advanced mode's columns on a whole-raster handle (src/raster/advanced.jl:81-196), planned on the device.
+ * nodemap: the nrows x ncols column-major 1-based node map cs_b200_create_from_raster[_poly] returned for this
+ * handle; src / gnd: the advanced-mode maps, column-major, of dtype (CS_B200_F32 / F64): source currents per cell,
+ * ground conductances with Inf for a direct ground; policy 0 keepall, 1 rmvsrc, 2 rmvgnd, 3 rmvall.
+ *   - node values: each node's nonzero cell values summed in fp64 from +0.0 in row-major cell order (np.add.at's
+ *     order), for sources and grounds alike;
+ *   - f = isfinite(g) ? g : 0 of those grounds; then the policy (rmvsrc / rmvall zero the sources, rmvgnd the
+ *     grounds, where both are nonzero) and every Inf ground under a source > 0 zeroed;
+ *   - if some f != 0 the handle takes cs_b200_set_grounds(f, NULL) through the same code (*finite_applied = 1);
+ *     otherwise it is untouched (0);
+ *   - components: the labels of cs_b200_components; a component is solved iff its source sum and its ground sum
+ *     over its rows in ascending order are both != 0 (NaN counts), each sum numpy's pairwise summation of those
+ *     n terms (blocks of <= 128 in 8 strided accumulators, halves split at a multiple of 8), the `s[rows].sum()`
+ *     of core.raster_advanced bit for bit; *nsolved counts them;
+ *   - a solved component with a row where s != 0 and g != Inf is a column, in label order.
+ * Returns the column count and the total set / source rows; the plan stays on the device until
+ * cs_b200_read_advanced_plan, the next plan or cs_b200_destroy.  CS_B200_ERR_ARG before the handle changes for a
+ * NULL pointer, a bad dtype or policy, more than 2^30 cells, a node map entry outside [0, n] or a node without a
+ * cell; CS_B200_ERR_UNSUPPORTED, also before any change and with no plan kept, when finite grounds would apply
+ * to a handle cs_b200_set_grounds refuses.  Integer atomics only: the outputs repeat bit for bit.              */
+int cs_b200_plan_advanced(cs_b200_handle* h, int64_t nrows, int64_t ncols, const int32_t* nodemap,
+                          const void* src, const void* gnd, int dtype, int policy,
+                          int64_t* ncol, int64_t* nsolved, int64_t* nset_rows, int64_t* nsrc_rows,
+                          int* finite_applied);
+/* Copies the plan of cs_b200_plan_advanced to host buffers and frees it: col_comp (ncol) each column's component
+ * label; set_ptr (ncol + 1) / set_rows (nset_rows) each column's Inf-ground rows, ascending; src_ptr (ncol + 1) /
+ * src_rows / src_vals (nsrc_rows) its rows with s != 0 and g != Inf, ascending, with their node source values;
+ * col_of_row (n int32) the column of every row, or -1.  CS_B200_ERR_ARG without a plan.                       */
+int cs_b200_read_advanced_plan(cs_b200_handle* h, int64_t* col_comp, int64_t* set_ptr, int64_t* set_rows,
+                               int64_t* src_ptr, int64_t* src_rows, double* src_vals, int32_t* col_of_row);
+
 /* cs_b200_solve_pairs with branch currents (network pairwise, src/out.jl:150-158, 250-290): arguments and
  * outputs as cs_b200_solve_pairs, plus branch: NULL or host column-major nb x k of the per-pair branch
  * currents |b|, b = |a_{hi,lo}| (v_lo - v_hi) zeroed where |b / max_e b| < 1e-8 (the maximum over the
