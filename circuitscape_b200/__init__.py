@@ -12,6 +12,7 @@ from .core import (GraphProblem, AdvancedProblem, Flags, OutputFlags, get_solver
                    single_ground_all_pairs, solve, advanced_kernel, multiple_solver, compute_3col,
                    RasterData, onetoall_kernel, resolve_conflicts, compute_omniscape_current,
                    compute_omniscape_currents, OmniscapeBatch, moving_window_current_map, MovingWindowMap,
+                   omniscape_current_maps, OmniscapeMaps,
                    all_to_one_batched, raster_pairwise,
                    raster_advanced, AdvancedOutput, network_advanced)
 from ._lib import B200Unavailable, B200Error, LIB_PATH, EXPORTED_SYMBOLS  # noqa: F401

@@ -103,6 +103,11 @@ _PROTOS = {
                                                C.c_void_p, C.c_void_p, C.c_int64, C.c_int, C.c_void_p, C.c_void_p,
                                                C.c_int, C.c_int, C.c_double, C.c_int64, C.c_int64, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
+    "cs_b200_solve_omniscape": (C.c_int, [C.c_int64, C.c_int64, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                          C.c_int64, C.c_double, C.c_int, C.c_int, C.c_int, C.c_double, C.c_int64,
+                                          C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64,
+                                          C.POINTER(C.c_int64), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]),
     "cs_b200_solve_advanced_network": (C.c_int, [_H, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_double,
                                                  C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,

@@ -881,6 +881,66 @@ def moving_window_current_map(conductance, source, targets, radius, cs_cfg, *, s
     return MovingWindowMap(res["cum"], res["iters"], res["relres"])
 
 
+@dataclass
+class OmniscapeMaps:
+    """Result of omniscape_current_maps (maps (nrows, ncols) float64, -9999 where the conductance is
+    NaN or -9999; per-target arrays in target order)."""
+    cum_currmap: np.ndarray
+    flow_potential: np.ndarray | None              # None unless flow_potential was requested
+    normalized_cum_currmap: np.ndarray | None      # cum_currmap / flow_potential where that is > 0, else 0
+    targets: np.ndarray                            # (n, 2) int64 (row, col) block centres with amps > 0
+    amps: np.ndarray                               # the source strength of each target's block
+    scale: np.ndarray                              # each window's source multiplier (0: nothing to inject)
+    iterations: np.ndarray                         # per conductance window, as OmniscapeBatch.iterations
+    relres: np.ndarray
+    fp_iterations: np.ndarray | None               # per flow-potential window
+    fp_relres: np.ndarray | None
+
+
+def omniscape_current_maps(conductance, source_strength, radius, cs_cfg, *, block_size=1, source_threshold=0.0,
+                           flow_potential=False, solver=None, max_batch_bytes=1 << 30) -> OmniscapeMaps:
+    """A whole Omniscape job on the device (cs_b200_solve_omniscape).
+
+    conductance / source_strength: 2-D landscape rasters of one shape, row-major (NODATA, 0 and NaN
+    conductance = no node).  A source counts where it is finite, above `source_threshold` and on a node.
+    One target sits at the centre of every `block_size` x `block_size` block (block_size odd) whose sources
+    sum to amps > 0.  Its window is the disc of `radius` around it, its sources those in the disc outside
+    its block, scaled to sum to amps, its ground a direct ground at the target; the windows' currents are
+    summed into cum_currmap in target order.  With `flow_potential` every window is solved once more with
+    conductance 1 on every landscape cell in the disc, giving flow_potential and normalized_cum_currmap.
+    Settings (`connect_four_neighbors_only`, rtol, itmax, device) are those of compute_omniscape_currents;
+    float32 rasters stay float32 on the way in when both are float32.  Targets go to the device in batches
+    of at most `max_batch_bytes` (S.advanced_batch_bytes per window); the maps do not depend on the split.
+    A window whose component fails the 1e-4 gate raises SolverResidualError naming its target (`.window`)
+    and its kind."""
+    g, s = np.asarray(conductance), np.asarray(source_strength)
+    for a, name in ((g, "conductance"), (s, "source_strength")):
+        if a.ndim != 2 or a.size == 0 or not (np.issubdtype(a.dtype, np.number) or a.dtype == bool):
+            raise ValueError(f"{name}: expected a non-empty numeric 2-D raster, got shape {a.shape} dtype {a.dtype}")
+    if g.shape != s.shape:
+        raise ValueError(f"conductance {g.shape} and source_strength {s.shape} differ")
+    if isinstance(radius, bool) or not isinstance(radius, (int, np.integer)) or radius < 0:
+        raise ValueError(f"radius must be an integer >= 0, got {radius!r}")
+    if (isinstance(block_size, bool) or not isinstance(block_size, (int, np.integer)) or block_size < 1
+            or block_size % 2 == 0):
+        raise ValueError(f"block_size must be an odd integer >= 1, got {block_size!r}")
+    if not float(source_threshold) >= 0.0:
+        raise ValueError(f"source_threshold must be >= 0, got {source_threshold!r}")
+    if max_batch_bytes <= 0:
+        raise ValueError("max_batch_bytes must be positive")
+    solver = solver if solver is not None else get_solver(cs_cfg)
+    dtype = np.float32 if g.dtype == np.float32 and s.dtype == np.float32 else np.float64
+    res = S.solve_omniscape(g.astype(dtype, copy=False), s.astype(dtype, copy=False), int(radius), int(block_size),
+                            float(source_threshold), bool(flow_potential), _flag(cs_cfg, "connect_four_neighbors_only"),
+                            solver.device, solver.rtol, solver.itmax, max_batch_bytes)
+    if res["rc"] == _lib.ERR_RESIDUAL:
+        err = S.SolverResidualError(res["msg"])
+        err.window = res["first_failed"]
+        raise err
+    return OmniscapeMaps(res["cum"], res["fp"], res["normalized"], res["targets"], res["amps"], res["scale"],
+                         res["iters"], res["relres"], res["fp_iters"], res["fp_relres"])
+
+
 def resolve_conflicts(sources, grounds, policy):
     """src/raster/advanced.jl:119-149 (`rmvall` only zeroes the sources -- pinned upstream by
     test/internal.jl:130-135)."""

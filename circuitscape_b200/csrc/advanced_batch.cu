@@ -25,6 +25,7 @@
 
 #include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
+#include <cub/device/device_select.cuh>
 
 #include <algorithm>
 #include <climits>
@@ -384,7 +385,10 @@ size_t align256(size_t b) { return (b + 255) / 256 * 256; }
 // for the tiles its square overlaps (k_window_tiles), a stable radix sort by tile keeps window order
 // inside a tile, and k_tile_bounds marks where each tile's run starts and ends.  The map stays on the
 // device across batches and each cell is one fixed chain of fp64 adds from +0.0, so the result does
-// not depend on the batch split.
+// not depend on the batch split.  cs_b200_solve_omniscape runs the same loop: k_block_targets and a cub
+// select find the targets first, k_window_cut's Omniscape modes normalise each window's sources (and cut
+// a flow-potential window beside each conductance window), the tile lists serve both maps, and
+// k_omniscape_finish writes the normalised map and the NODATA mask.
 // ---------------------------------------------------------------------------------------------------
 constexpr int TILE = 32;
 constexpr int TILE_COLS = BT / TILE;            // tile columns one CTA pass covers
@@ -398,16 +402,58 @@ struct Land {
   int span;            // most tiles a window overlaps along one axis
 };
 
-// window w's g / src / gnd in k_advanced_batch's layout (window-major, column-major inside)
+// What k_window_cut writes.  CUT_WINDOW: the window of cs_b200_solve_moving_windows (per-window scale and
+// ground).  CUT_OMNI: Omniscape's conductance window -- sources s' outside the target's block, scaled to
+// sum to the target's amps (the scale is reduced here and stored per target), a direct ground at the
+// centre.  CUT_FLOW: the flow-potential window of the same target -- g = 1 on every landscape cell in the
+// square (and disc), the CUT_OMNI sources (its stored scale), a direct ground at the centre.
+enum CutMode { CUT_WINDOW = 0, CUT_OMNI = 1, CUT_FLOW = 2 };
+
+struct BlockRule {          // Omniscape's source rule (CUT_OMNI, CUT_FLOW)
+  double theta;             // source threshold
+  int half;                 // (block size - 1) / 2
+  const double* amps;       // per target
+  double* scale;            // per target: written by CUT_OMNI, read by CUT_FLOW
+};
+
+// effective source strength s' of a landscape cell: s where s > theta, s is finite and g > 0, else 0
 template <typename T>
+__device__ __forceinline__ double eff_strength(T s, T g, double theta) {
+  const double sd = (double)s;
+  return (sd > theta && isfinite(sd) && (double)g > 0.0) ? sd : 0.0;
+}
+
+// window w's g / src / gnd in k_advanced_batch's layout (window-major, column-major inside)
+template <int MODE, typename T>
 __global__ void __launch_bounds__(BT)
 k_window_cut(Land L, int w0, const T* __restrict__ G, const T* __restrict__ S, const int* __restrict__ trow,
              const int* __restrict__ tcol, const double* __restrict__ scale, const double* __restrict__ gnd,
-             T* __restrict__ g_all, T* __restrict__ src_all, T* __restrict__ gnd_all) {
+             BlockRule br, T* __restrict__ g_all, T* __restrict__ src_all, T* __restrict__ gnd_all) {
   const int w = w0 + blockIdx.x, R = L.radius, W = L.side, n = W * W;
   const int r0 = trow[w] - R, c0 = tcol[w] - R;
-  const double sc = scale ? scale[w] : 1.0;
-  const T gc = gnd ? (T)gnd[w] : (T)INFINITY;
+  double sc;
+  if constexpr (MODE == CUT_WINDOW) {
+    sc = scale ? scale[w] : 1.0;
+  } else if constexpr (MODE == CUT_FLOW) {
+    sc = br.scale[w];
+  } else {
+    // the window's source sum: s' over the landscape cells in the disc outside the target's block, a
+    // strided fp64 partial per thread, then the fixed-order CTA tree
+    __shared__ double red[NWARP + 1];
+    double part = 0.0;
+    for (int i = threadIdx.x; i < n; i += BT) {
+      const int dr = i % W - R, dc = i / W - R, r = r0 + R + dr, c = c0 + R + dc;
+      if (r >= 0 && r < L.nrows && c >= 0 && c < L.ncols && (!L.circular || dr * dr + dc * dc <= R * R) &&
+          (abs(dr) > br.half || abs(dc) > br.half)) {
+        const int64_t j = (int64_t)c * L.nrows + r;
+        part += eff_strength(S[j], G[j], br.theta);
+      }
+    }
+    const double sum = block_sum(part, red);
+    sc = sum > 0.0 ? br.amps[w] / sum : 0.0;
+    if (threadIdx.x == 0) br.scale[w] = sc;
+  }
+  const T gc = MODE == CUT_WINDOW && gnd ? (T)gnd[w] : (T)INFINITY;
   const int64_t base = (int64_t)blockIdx.x * n;
   for (int i = threadIdx.x; i < n; i += BT) {
     const int dr = i % W - R, dc = i / W - R, r = r0 + R + dr, c = c0 + R + dc;
@@ -415,9 +461,15 @@ k_window_cut(Land L, int w0, const T* __restrict__ G, const T* __restrict__ S, c
     if (r >= 0 && r < L.nrows && c >= 0 && c < L.ncols && (!L.circular || dr * dr + dc * dc <= R * R)) {
       const int64_t j = (int64_t)c * L.nrows + r;
       const T gl = G[j];
-      if ((double)gl > 0.0) {
-        gv = gl;
-        sv = (T)(sc * (double)S[j]);
+      if constexpr (MODE == CUT_WINDOW) {
+        if ((double)gl > 0.0) {
+          gv = gl;
+          sv = (T)(sc * (double)S[j]);
+          if (dr == 0 && dc == 0) nv = gc;
+        }
+      } else if (MODE == CUT_FLOW || (double)gl > 0.0) {
+        gv = MODE == CUT_FLOW ? (T)1 : gl;
+        if (abs(dr) > br.half || abs(dc) > br.half) sv = (T)(sc * eff_strength(S[j], gl, br.theta));
         if (dr == 0 && dc == 0) nv = gc;
       }
     }
@@ -425,6 +477,45 @@ k_window_cut(Land L, int w0, const T* __restrict__ G, const T* __restrict__ S, c
     src_all[base + i] = sv;
     gnd_all[base + i] = nv;
   }
+}
+
+// Omniscape's targets: one thread per block centre (candidate k = i + j * ni, block-column-major), the
+// amps summed sequentially in fp64 over the block clipped to the landscape, column outer, row inner
+template <typename T>
+__global__ void k_block_targets(int nrows, int ncols, int bsz, int ni, int ncand, double theta,
+                                const T* __restrict__ G, const T* __restrict__ S, int* __restrict__ crow,
+                                int* __restrict__ ccol, double* __restrict__ camps, char* __restrict__ flag) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= ncand) return;
+  const int half = (bsz - 1) / 2, tr = half + (k % ni) * bsz, tc = half + (k / ni) * bsz;
+  const int r1 = min(tr + half, nrows - 1), c1 = min(tc + half, ncols - 1);
+  double a = 0.0;
+  for (int c = tc - half; c <= c1; ++c)
+    for (int r = tr - half; r <= r1; ++r) {
+      const int64_t j = (int64_t)c * nrows + r;
+      a += eff_strength(S[j], G[j], theta);
+    }
+  crow[k] = tr;
+  ccol[k] = tc;
+  camps[k] = a;
+  flag[k] = a > 0.0 ? 1 : 0;
+}
+
+// the returned maps: normalized = fp > 0 ? cum / fp : 0, then NODATA (-9999) in every map where g is NaN
+// or -9999; fp and norm are null without flow potential
+template <typename T>
+__global__ void k_omniscape_finish(int64_t cells, const T* __restrict__ G, double* __restrict__ cum,
+                                   double* __restrict__ fp, double* __restrict__ norm) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= cells) return;
+  const double g = (double)G[i];
+  const bool mask = isnan(g) || g == kNodata;
+  if (fp) {
+    const double f = fp[i];
+    norm[i] = mask ? kNodata : (f > 0.0 ? cum[i] / f : 0.0);
+    if (mask) fp[i] = kNodata;
+  }
+  if (mask) cum[i] = kNodata;
 }
 
 // (tile, window-in-batch) for every tile window w0 + wl overlaps; span^2 slots per window, the unused
@@ -520,20 +611,34 @@ struct Stream {
                      __FILE__, __LINE__, #call);                                                 \
   } while (0)
 
-// the batches of cs_b200_solve_moving_windows; wo receives every window's WinOut
+// Omniscape's block rule and flow potential on top of the moving-window loop (cs_b200_solve_omniscape)
+struct OmniJob {
+  int bsz;                      // block size (odd)
+  double theta;                 // source threshold
+  bool flow;                    // also cut, solve and accumulate the flow-potential window of every target
+  double *fp, *norm;            // host maps (flow only)
+  std::vector<double> amps, scale;   // per target, filled by the call
+  std::vector<WinOut> wo_fp;         // per target's flow-potential window, filled by the call
+};
+
+// the batches of cs_b200_solve_moving_windows (om null: trow / tcol are the targets) and of
+// cs_b200_solve_omniscape (om set: trow / tcol receive the targets found on the device).  Batches are as
+// many targets as fit `budget` at `per` bytes per window, every window of a target counted; wo receives
+// every (conductance) window's WinOut.
 template <typename T>
-int moving_windows(const Land& L, int nwin, int bw, const void* g, const void* src, const std::vector<int>& trow,
-                   const std::vector<int>& tcol, const double* scale, const double* gnd, int four, double rtol,
-                   long long itmax, double* cum, std::vector<WinOut>& wo) {
+int moving_windows(const Land& L, size_t budget, size_t per_win, const void* g, const void* src,
+                   std::vector<int>& trow, std::vector<int>& tcol, const double* scale, const double* gnd, int four,
+                   double rtol, long long itmax, double* cum, std::vector<WinOut>& wo, OmniJob* om) {
   const size_t cells = (size_t)L.nrows * L.ncols, ncell = (size_t)L.side * L.side, per = (size_t)L.span * L.span;
   const Shape s{L.side, L.side, (int)ncell, four};
   const double atol = std::sqrt(2.220446049250313e-16);   // sqrt(eps(Float64)), as cs_b200_solve_advanced_batch
+  const int kinds = om && om->flow ? 2 : 1;               // windows per target
   int nbits = 1;
   while (nbits < 32 && (1ull << nbits) <= (unsigned long long)L.ntiles) ++nbits;   // keys 0 .. ntiles
   Stream st;
   DevBufs d;
   T *dG, *dS, *wg, *ws, *wn;
-  double *dcum, *dscale = nullptr, *dgnd = nullptr, *wcur, *wvec;
+  double *dcum, *dfp = nullptr, *dnorm = nullptr, *dscale = nullptr, *dgnd = nullptr, *damps = nullptr, *wcur, *wvec;
   int *dtr, *dtc, *wlab, *wflag, *wlist, *val_in, *val_out, *beg, *end;
   unsigned *key_in, *key_out;
   WinOut* dout;
@@ -543,19 +648,82 @@ int moving_windows(const Land& L, int nwin, int bw, const void* g, const void* s
   CKM(d.get(&dG, cells));
   CKM(d.get(&dS, cells));
   CKM(d.get(&dcum, cells));
-  CKM(d.get(&dtr, (size_t)nwin));
-  CKM(d.get(&dtc, (size_t)nwin));
-  if (scale) CKM(d.get(&dscale, (size_t)nwin));
-  if (gnd) CKM(d.get(&dgnd, (size_t)nwin));
-  CKM(d.get(&wg, bw * ncell));
-  CKM(d.get(&ws, bw * ncell));
-  CKM(d.get(&wn, bw * ncell));
-  CKM(d.get(&wcur, bw * ncell));
-  CKM(d.get(&wvec, bw * ncell * NVEC));
-  CKM(d.get(&wlab, bw * ncell));
-  CKM(d.get(&wflag, bw * ncell));
-  CKM(d.get(&wlist, bw * ncell));
-  CKM(d.get(&dout, (size_t)bw));
+  if (kinds == 2) {
+    CKM(d.get(&dfp, cells));
+    CKM(d.get(&dnorm, cells));
+  }
+  CKM(cudaMemcpyAsync(dG, g, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
+  CKM(cudaMemcpyAsync(dS, src, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
+  CKM(cudaMemsetAsync(dcum, 0, cells * sizeof(double), st.s));
+  if (dfp) CKM(cudaMemsetAsync(dfp, 0, cells * sizeof(double), st.s));
+
+  int nwin = (int)trow.size();
+  if (!om) {
+    CKM(d.get(&dtr, (size_t)nwin));
+    CKM(d.get(&dtc, (size_t)nwin));
+    if (scale) CKM(d.get(&dscale, (size_t)nwin));
+    if (gnd) CKM(d.get(&dgnd, (size_t)nwin));
+    CKM(cudaMemcpyAsync(dtr, trow.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
+    CKM(cudaMemcpyAsync(dtc, tcol.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
+    if (scale) CKM(cudaMemcpyAsync(dscale, scale, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
+    if (gnd) CKM(cudaMemcpyAsync(dgnd, gnd, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  } else {
+    // the block centres, then the ones with amps > 0 compacted in candidate order
+    const int half = (om->bsz - 1) / 2;
+    const int ni = L.nrows > half ? (L.nrows - 1 - half) / om->bsz + 1 : 0;
+    const int nj = L.ncols > half ? (L.ncols - 1 - half) / om->bsz + 1 : 0;
+    const int ncand = ni * nj;
+    int *crow, *ccol, *dnum;
+    double* camps;
+    char* cflag;
+    CKM(d.get(&crow, (size_t)ncand));
+    CKM(d.get(&ccol, (size_t)ncand));
+    CKM(d.get(&camps, (size_t)ncand));
+    CKM(d.get(&cflag, (size_t)ncand));
+    CKM(d.get(&dtr, (size_t)ncand));
+    CKM(d.get(&dtc, (size_t)ncand));
+    CKM(d.get(&damps, (size_t)ncand));
+    CKM(d.get(&dscale, (size_t)ncand));
+    CKM(d.get(&dnum, 1));
+    size_t sel_i = 0, sel_d = 0;
+    CKM(cub::DeviceSelect::Flagged(nullptr, sel_i, crow, cflag, dtr, dnum, ncand, st.s));
+    CKM(cub::DeviceSelect::Flagged(nullptr, sel_d, camps, cflag, damps, dnum, ncand, st.s));
+    unsigned char* sel_tmp;
+    CKM(d.get(&sel_tmp, std::max(sel_i, sel_d)));
+    int nt = 0;
+    if (ncand > 0) {
+      k_block_targets<T><<<(ncand + BT - 1) / BT, BT, 0, st.s>>>(L.nrows, L.ncols, om->bsz, ni, ncand, om->theta, dG,
+                                                                 dS, crow, ccol, camps, cflag);
+      CKM(cudaGetLastError());
+      CKM(cub::DeviceSelect::Flagged(sel_tmp, sel_i, crow, cflag, dtr, dnum, ncand, st.s));
+      CKM(cub::DeviceSelect::Flagged(sel_tmp, sel_i, ccol, cflag, dtc, dnum, ncand, st.s));
+      CKM(cub::DeviceSelect::Flagged(sel_tmp, sel_d, camps, cflag, damps, dnum, ncand, st.s));
+      CKM(cudaMemcpyAsync(&nt, dnum, sizeof(int), cudaMemcpyDeviceToHost, st.s));
+      CKM(cudaStreamSynchronize(st.s));
+    }
+    nwin = nt;
+    trow.resize((size_t)nt);
+    tcol.resize((size_t)nt);
+    om->amps.resize((size_t)nt);
+    om->scale.resize((size_t)nt);
+    wo.resize((size_t)nt);
+    om->wo_fp.resize((size_t)nt);
+    CKM(cudaMemcpyAsync(trow.data(), dtr, (size_t)nt * sizeof(int), cudaMemcpyDeviceToHost, st.s));
+    CKM(cudaMemcpyAsync(tcol.data(), dtc, (size_t)nt * sizeof(int), cudaMemcpyDeviceToHost, st.s));
+    CKM(cudaMemcpyAsync(om->amps.data(), damps, (size_t)nt * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+  }
+
+  // targets per batch
+  const int bw = (int)std::max<size_t>(1, std::min({budget / (per_win * kinds), (size_t)nwin, INT_MAX / per}));
+  CKM(d.get(&wg, kinds * bw * ncell));
+  CKM(d.get(&ws, kinds * bw * ncell));
+  CKM(d.get(&wn, kinds * bw * ncell));
+  CKM(d.get(&wcur, kinds * bw * ncell));
+  CKM(d.get(&wvec, kinds * bw * ncell * NVEC));
+  CKM(d.get(&wlab, kinds * bw * ncell));
+  CKM(d.get(&wflag, kinds * bw * ncell));
+  CKM(d.get(&wlist, kinds * bw * ncell));
+  CKM(d.get(&dout, (size_t)(kinds * bw)));
   CKM(d.get(&key_in, bw * per));
   CKM(d.get(&key_out, bw * per));
   CKM(d.get(&val_in, bw * per));
@@ -566,18 +734,23 @@ int moving_windows(const Land& L, int nwin, int bw, const void* g, const void* s
                                       nbits, st.s));
   CKM(d.get(&tmp, tmp_bytes));
 
-  CKM(cudaMemcpyAsync(dG, g, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
-  CKM(cudaMemcpyAsync(dS, src, cells * sizeof(T), cudaMemcpyHostToDevice, st.s));
-  CKM(cudaMemsetAsync(dcum, 0, cells * sizeof(double), st.s));
-  CKM(cudaMemcpyAsync(dtr, trow.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
-  CKM(cudaMemcpyAsync(dtc, tcol.data(), (size_t)nwin * sizeof(int), cudaMemcpyHostToDevice, st.s));
-  if (scale) CKM(cudaMemcpyAsync(dscale, scale, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
-  if (gnd) CKM(cudaMemcpyAsync(dgnd, gnd, (size_t)nwin * sizeof(double), cudaMemcpyHostToDevice, st.s));
+  const BlockRule br{om ? om->theta : 0.0, om ? (om->bsz - 1) / 2 : 0, damps, dscale};
   for (int w0 = 0; w0 < nwin; w0 += bw) {
     const int nb = std::min(bw, nwin - w0), np = (int)(nb * per);
-    k_window_cut<T><<<nb, BT, 0, st.s>>>(L, w0, dG, dS, dtr, dtc, dscale, dgnd, wg, ws, wn);
+    const size_t second = (size_t)nb * ncell;   // the flow-potential windows follow the batch's conductance windows
+    if (!om) {
+      k_window_cut<CUT_WINDOW, T><<<nb, BT, 0, st.s>>>(L, w0, dG, dS, dtr, dtc, dscale, dgnd, br, wg, ws, wn);
+    } else {
+      k_window_cut<CUT_OMNI, T><<<nb, BT, 0, st.s>>>(L, w0, dG, dS, dtr, dtc, nullptr, nullptr, br, wg, ws, wn);
+      if (kinds == 2) {
+        CKM(cudaGetLastError());
+        k_window_cut<CUT_FLOW, T><<<nb, BT, 0, st.s>>>(L, w0, dG, dS, dtr, dtc, nullptr, nullptr, br, wg + second,
+                                                       ws + second, wn + second);
+      }
+    }
     CKM(cudaGetLastError());
-    CKM((launch<T>(nb, s, wg, ws, wn, rtol, atol, itmax, wcur, nullptr, wvec, wlab, wflag, wlist, dout, st.s)));
+    CKM((launch<T>(kinds * nb, s, wg, ws, wn, rtol, atol, itmax, wcur, nullptr, wvec, wlab, wflag, wlist, dout,
+                   st.s)));
     k_window_tiles<<<(np + BT - 1) / BT, BT, 0, st.s>>>(L, w0, nb, dtr, dtc, key_in, val_in);
     CKM(cudaGetLastError());
     size_t tb = tmp_bytes;
@@ -589,10 +762,46 @@ int moving_windows(const Land& L, int nwin, int bw, const void* g, const void* s
     k_window_accumulate<<<L.ntiles, BT, 0, st.s>>>(L, w0, dtr, dtc, beg, end, val_out, wcur, dcum);
     CKM(cudaGetLastError());
     CKM(cudaMemcpyAsync(wo.data() + w0, dout, (size_t)nb * sizeof(WinOut), cudaMemcpyDeviceToHost, st.s));
+    if (kinds == 2) {   // the same tile lists place the flow-potential windows
+      k_window_accumulate<<<L.ntiles, BT, 0, st.s>>>(L, w0, dtr, dtc, beg, end, val_out, wcur + second, dfp);
+      CKM(cudaGetLastError());
+      CKM(cudaMemcpyAsync(om->wo_fp.data() + w0, dout + nb, (size_t)nb * sizeof(WinOut), cudaMemcpyDeviceToHost,
+                          st.s));
+    }
+  }
+  if (om) {
+    k_omniscape_finish<T><<<(unsigned)((cells + BT - 1) / BT), BT, 0, st.s>>>((int64_t)cells, dG, dcum, dfp, dnorm);
+    CKM(cudaGetLastError());
+    CKM(cudaMemcpyAsync(om->scale.data(), dscale, (size_t)nwin * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+    if (dfp) {
+      CKM(cudaMemcpyAsync(om->fp, dfp, cells * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+      CKM(cudaMemcpyAsync(om->norm, dnorm, cells * sizeof(double), cudaMemcpyDeviceToHost, st.s));
+    }
   }
   CKM(cudaMemcpyAsync(cum, dcum, cells * sizeof(double), cudaMemcpyDeviceToHost, st.s));
   CKM(cudaStreamSynchronize(st.s));
   return CS_B200_OK;
+}
+
+// the Land of a landscape and radius (tile grid and the most tiles a window overlaps along one axis)
+Land make_land(int64_t nrows, int64_t ncols, int64_t radius, int circular) {
+  Land L;
+  L.nrows = (int)nrows;
+  L.ncols = (int)ncols;
+  L.radius = (int)radius;
+  L.side = 2 * L.radius + 1;
+  L.circular = circular ? 1 : 0;
+  L.tiles_r = (L.nrows + TILE - 1) / TILE;
+  L.ntiles = L.tiles_r * ((L.ncols + TILE - 1) / TILE);
+  L.span = std::min((L.side + TILE - 1) / TILE + 1, std::max(L.tiles_r, L.ntiles / L.tiles_r));
+  return L;
+}
+
+// device bytes of one window's stack, solver.advanced_batch_bytes(ncell, itemsize, False): the inputs,
+// the current raster, NVEC fp64 CG vectors, three int32 label arrays and its WinOut
+size_t window_bytes(const Land& L, int dtype) {
+  const size_t isz = dtype == CS_B200_F64 ? 8 : 4, ncell = (size_t)L.side * L.side;
+  return ncell * (3 * isz + 8 + NVEC * 8 + 3 * 4) + sizeof(WinOut);
 }
 
 }  // namespace
@@ -739,29 +948,17 @@ extern "C" int cs_b200_solve_moving_windows(int64_t nrows, int64_t ncols, const 
     return set_err(CS_B200_ERR_ARG, "device %d out of range (0..%d)", device, ndev - 1);
   if (nwin == 0) return CS_B200_OK;
 
-  Land L;
-  L.nrows = (int)nrows;
-  L.ncols = (int)ncols;
-  L.radius = (int)radius;
-  L.side = 2 * L.radius + 1;
-  L.circular = circular ? 1 : 0;
-  L.tiles_r = (L.nrows + TILE - 1) / TILE;
-  L.ntiles = L.tiles_r * ((L.ncols + TILE - 1) / TILE);
-  L.span = std::min((L.side + TILE - 1) / TILE + 1, std::max(L.tiles_r, L.ntiles / L.tiles_r));
-  // windows per batch: the device bytes of one window's stack, solver.advanced_batch_bytes(ncell, itemsize,
-  // False) -- the inputs, the current raster, NVEC fp64 CG vectors, three int32 label arrays and its WinOut
-  const size_t isz = dtype == CS_B200_F64 ? 8 : 4, ncell = (size_t)L.side * L.side;
-  const size_t per = ncell * (3 * isz + 8 + NVEC * 8 + 3 * 4) + sizeof(WinOut);
-  const size_t pairs = (size_t)L.span * L.span;
-  const size_t bw = std::max<size_t>(1, std::min({(size_t)max_batch_bytes / per, (size_t)nwin, INT_MAX / pairs}));
+  const Land L = make_land(nrows, ncols, radius, circular);
   std::vector<WinOut> wo((size_t)nwin);
   e = cudaSetDevice(device);
   if (e != cudaSuccess) return set_err(CS_B200_ERR_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
   const int rc = dtype == CS_B200_F64
-                     ? moving_windows<double>(L, (int)nwin, (int)bw, g, src, trow, tcol, source_scale, ground,
-                                              four_neighbors ? 1 : 0, rtol, (long long)itmax, cum, wo)
-                     : moving_windows<float>(L, (int)nwin, (int)bw, g, src, trow, tcol, source_scale, ground,
-                                             four_neighbors ? 1 : 0, rtol, (long long)itmax, cum, wo);
+                     ? moving_windows<double>(L, (size_t)max_batch_bytes, window_bytes(L, dtype), g, src, trow, tcol,
+                                              source_scale, ground, four_neighbors ? 1 : 0, rtol, (long long)itmax,
+                                              cum, wo, nullptr)
+                     : moving_windows<float>(L, (size_t)max_batch_bytes, window_bytes(L, dtype), g, src, trow, tcol,
+                                             source_scale, ground, four_neighbors ? 1 : 0, rtol, (long long)itmax,
+                                             cum, wo, nullptr);
   if (rc != CS_B200_OK) return rc;
 
   int64_t bad = -1;
@@ -780,5 +977,98 @@ extern "C" int cs_b200_solve_moving_windows(int64_t nrows, int64_t ncols, const 
     return set_err(CS_B200_ERR_MAXITER,
                    "CUDA PCG solver reached itmax = %lld before rtol for window %lld (residual %g)",
                    (long long)itmax, (long long)bad, wo[bad].fail_relres);
+  return CS_B200_OK;
+}
+
+extern "C" int cs_b200_solve_omniscape(int64_t nrows, int64_t ncols, const void* g, const void* src, int dtype,
+                                       int64_t radius, int64_t block_size, double source_threshold,
+                                       int flow_potential, int four_neighbors, int device, double rtol, int64_t itmax,
+                                       int64_t max_batch_bytes, double* cum, double* fp, double* normalized,
+                                       int64_t max_targets, int64_t* ntargets, int64_t* target_rows,
+                                       int64_t* target_cols, double* amps, double* scale, int64_t* iters,
+                                       double* relres, int64_t* fp_iters, double* fp_relres, int64_t* first_failed) {
+  if (first_failed) *first_failed = -1;
+  if (ntargets) *ntargets = 0;
+  if (nrows < 1 || ncols < 1 || nrows > INT_MAX / ncols)
+    return set_err(CS_B200_ERR_ARG, "bad landscape shape %lld x %lld (at most INT_MAX cells)", (long long)nrows,
+                   (long long)ncols);
+  if (radius < 0 || 2 * radius + 1 > 46340)   // (2R+1)^2 cells per window must fit an int
+    return set_err(CS_B200_ERR_ARG, "bad radius %lld (0 <= radius, (2 radius + 1)^2 <= INT_MAX)", (long long)radius);
+  if (block_size < 1 || block_size % 2 == 0 || block_size > INT_MAX)
+    return set_err(CS_B200_ERR_ARG, "bad block_size %lld (an odd number >= 1)", (long long)block_size);
+  if (!(source_threshold >= 0.0))
+    return set_err(CS_B200_ERR_ARG, "bad source_threshold %g (>= 0)", source_threshold);
+  if (dtype != CS_B200_F32 && dtype != CS_B200_F64) return set_err(CS_B200_ERR_ARG, "bad dtype %d", dtype);
+  if (!(rtol >= 0.0) || itmax < 0)
+    return set_err(CS_B200_ERR_ARG, "bad rtol %g / itmax %lld", rtol, (long long)itmax);
+  if (max_batch_bytes <= 0) return set_err(CS_B200_ERR_ARG, "bad max_batch_bytes %lld", (long long)max_batch_bytes);
+  if (!g || !src || !cum || !ntargets || !target_rows || !target_cols || !amps || !scale)
+    return set_err(CS_B200_ERR_ARG, "g, src, cum, ntargets, target_rows, target_cols, amps and scale must not be NULL");
+  if (flow_potential && (!fp || !normalized))
+    return set_err(CS_B200_ERR_ARG, "fp and normalized must not be NULL with flow_potential");
+  const int64_t half = (block_size - 1) / 2;
+  const int64_t ncand = (nrows > half ? (nrows - 1 - half) / block_size + 1 : 0) *
+                        (ncols > half ? (ncols - 1 - half) / block_size + 1 : 0);
+  if (max_targets < ncand)
+    return set_err(CS_B200_ERR_ARG, "max_targets %lld is below the %lld block centres", (long long)max_targets,
+                   (long long)ncand);
+  const size_t cells = (size_t)nrows * ncols;
+  std::fill(cum, cum + cells, 0.0);
+  if (flow_potential) {
+    std::fill(fp, fp + cells, 0.0);
+    std::fill(normalized, normalized + cells, 0.0);
+  }
+  int ndev = 0;
+  cudaError_t e = cudaGetDeviceCount(&ndev);
+  if (e != cudaSuccess || ndev == 0)
+    return set_err(CS_B200_ERR_CUDA, "no CUDA device available (%s): libcsb200 has no CPU fallback",
+                   cudaGetErrorString(e));
+  if (device < 0 || device >= ndev)
+    return set_err(CS_B200_ERR_ARG, "device %d out of range (0..%d)", device, ndev - 1);
+
+  const Land L = make_land(nrows, ncols, radius, 1);
+  OmniJob om{(int)block_size, source_threshold, flow_potential != 0, fp, normalized, {}, {}, {}};
+  std::vector<int> trow, tcol;
+  std::vector<WinOut> wo;
+  e = cudaSetDevice(device);
+  if (e != cudaSuccess) return set_err(CS_B200_ERR_CUDA, "cudaSetDevice(%d): %s", device, cudaGetErrorString(e));
+  const int rc = dtype == CS_B200_F64
+                     ? moving_windows<double>(L, (size_t)max_batch_bytes, window_bytes(L, dtype), g, src, trow, tcol,
+                                              nullptr, nullptr, four_neighbors ? 1 : 0, rtol, (long long)itmax, cum,
+                                              wo, &om)
+                     : moving_windows<float>(L, (size_t)max_batch_bytes, window_bytes(L, dtype), g, src, trow, tcol,
+                                             nullptr, nullptr, four_neighbors ? 1 : 0, rtol, (long long)itmax, cum,
+                                             wo, &om);
+  if (rc != CS_B200_OK) return rc;
+
+  const int64_t nt = (int64_t)trow.size();
+  *ntargets = nt;
+  int64_t bad = -1;
+  int worst = WIN_OK;
+  bool bad_fp = false;
+  for (int64_t t = 0; t < nt; ++t) {
+    target_rows[t] = trow[t];
+    target_cols[t] = tcol[t];
+    amps[t] = om.amps[t];
+    scale[t] = om.scale[t];
+    if (iters) iters[t] = wo[t].iters;
+    if (relres) relres[t] = wo[t].relres;
+    if (wo[t].status > worst) { worst = wo[t].status; bad = t; bad_fp = false; }
+    if (!om.flow) continue;
+    if (fp_iters) fp_iters[t] = om.wo_fp[t].iters;
+    if (fp_relres) fp_relres[t] = om.wo_fp[t].relres;
+    if (om.wo_fp[t].status > worst) { worst = om.wo_fp[t].status; bad = t; bad_fp = true; }
+  }
+  if (first_failed) *first_failed = bad;
+  const WinOut* f = bad < 0 ? nullptr : bad_fp ? &om.wo_fp[bad] : &wo[bad];
+  const char* kind = bad_fp ? "flow-potential" : "conductance";
+  if (worst == WIN_RESIDUAL)
+    return set_err(CS_B200_ERR_RESIDUAL,
+                   "CUDA PCG solver residual %g exceeds tolerance %g for target %lld, %s window (%d iterations)",
+                   f->fail_relres, kGate, (long long)bad, kind, f->fail_iters);
+  if (worst == WIN_MAXITER)
+    return set_err(CS_B200_ERR_MAXITER,
+                   "CUDA PCG solver reached itmax = %lld before rtol for target %lld, %s window (residual %g)",
+                   (long long)itmax, (long long)bad, kind, f->fail_relres);
   return CS_B200_OK;
 }

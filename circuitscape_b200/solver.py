@@ -690,6 +690,48 @@ def solve_moving_windows(g, src, target_rows, target_cols, radius, circular, sou
                 msg=msg)
 
 
+def omniscape_candidates(nrows, ncols, block_size):
+    """Number of Omniscape block centres (block_size // 2 + i * block_size, ...) inside the landscape."""
+    h = (block_size - 1) // 2
+    return ((nrows - 1 - h) // block_size + 1 if nrows > h else 0) * ((ncols - 1 - h) // block_size + 1
+                                                                      if ncols > h else 0)
+
+
+def solve_omniscape(g, src, radius, block_size, source_threshold, flow_potential, four_neighbors, device, rtol,
+                    itmax, max_batch_bytes):
+    """One cs_b200_solve_omniscape call: landscape rasters g / src (nrows, ncols) of one float dtype.
+    Returns dict with cum, fp, normalized (nrows, ncols) float64 (fp / normalized None without
+    flow_potential), targets (nt, 2) int64, amps, scale, iters, relres, fp_iters, fp_relres (nt,), rc (OK,
+    ERR_RESIDUAL or ERR_MAXITER), first_failed (target index or -1) and msg; other failures raise."""
+    lib = _lib.load()
+    nr, nc = g.shape
+    dt = _lib.dtype_code(g.dtype)
+    g_, s_ = (np.ascontiguousarray(np.asarray(a, dtype=g.dtype).T) for a in (g, src))
+    cap = omniscape_candidates(nr, nc, int(block_size))
+    cum = np.empty((nc, nr), dtype=np.float64)
+    fp, norm = (np.empty((nc, nr), dtype=np.float64) if flow_potential else None for _ in range(2))
+    rows, cols, iters, fp_iters = (np.zeros(cap, dtype=np.int64) for _ in range(4))
+    amps, scale, relres, fp_relres = (np.zeros(cap, dtype=np.float64) for _ in range(4))
+    nt, bad = C.c_int64(0), C.c_int64(-1)
+    rc = lib.cs_b200_solve_omniscape(nr, nc, _lib._ptr(g_), _lib._ptr(s_), dt, int(radius), int(block_size),
+                                     float(source_threshold), 1 if flow_potential else 0, 1 if four_neighbors else 0,
+                                     device, float(rtol), int(itmax), int(max_batch_bytes), _lib._ptr(cum),
+                                     _lib._ptr(fp), _lib._ptr(norm), cap, C.byref(nt), _lib._ptr(rows),
+                                     _lib._ptr(cols), _lib._ptr(amps), _lib._ptr(scale), _lib._ptr(iters),
+                                     _lib._ptr(relres), _lib._ptr(fp_iters), _lib._ptr(fp_relres), C.byref(bad))
+    msg = ""
+    if rc not in (_lib.OK, _lib.ERR_RESIDUAL, _lib.ERR_MAXITER):
+        _lib.check(lib, None, rc)
+    if rc != _lib.OK:
+        msg = lib.cs_b200_last_error(None).decode()
+    n = nt.value
+    t = lambda a: None if a is None else np.ascontiguousarray(a.T)
+    return dict(cum=t(cum), fp=t(fp), normalized=t(norm), targets=np.stack([rows[:n], cols[:n]], 1),
+                amps=amps[:n], scale=scale[:n], iters=iters[:n], relres=relres[:n],
+                fp_iters=fp_iters[:n] if flow_potential else None, fp_relres=fp_relres[:n] if flow_potential else None,
+                rc=rc, first_failed=int(bad.value), msg=msg)
+
+
 # ---------------------------------------------------------------------------
 # the three plug-in hooks
 # ---------------------------------------------------------------------------

@@ -423,6 +423,49 @@ int cs_b200_solve_moving_windows(int64_t nrows, int64_t ncols, const void* g, co
                                  int64_t max_batch_bytes, double* cum, int64_t* iters, double* relres,
                                  int64_t* first_failed);
 
+/* A whole Omniscape job over one landscape: block targets, per-window source normalisation, the
+ * moving-window solves of cs_b200_solve_moving_windows (disc on, direct ground at the target), and
+ * optionally the flow potential and the normalised current map, all on the device.
+ *   g, src: host, nrows x ncols, column-major, element type `dtype`: conductance (a cell is a node when
+ *           g > 0) and source strength; uploaded once.  half = (block_size - 1) / 2.
+ *   1. s'[c] = src[c] where src[c] > source_threshold, src[c] is finite and g[c] > 0; else 0.
+ *   2. Candidates: the block centres (half + i block_size, half + j block_size) inside the landscape, j
+ *      outer, i inner.  amps = sum of s' over the block clipped to the landscape, fp64 from +0.0, column
+ *      outer, row inner.  Targets: the candidates with amps > 0, in candidate order.
+ *   3. Window sum S_w = sum of s' over the landscape cells in the disc of `radius` around the target and
+ *      outside its block (|dr| > half or |dc| > half), fp64 in a fixed CTA order; scale = S_w > 0 ?
+ *      amps / S_w : 0.
+ *   4. Conductance window: cs_b200_solve_moving_windows's circular window, sources (T)(scale * s') on
+ *      nodes outside the block, 0 inside it, a direct (Inf) ground at the centre.
+ *   5. Flow-potential window (flow_potential != 0): the same square and disc with g = 1 on every
+ *      landscape cell in the disc (NODATA, 0 and NaN cells included), the same sources, a direct ground
+ *      at the centre.
+ *   6. cum / fp: every target's window currents summed in target order from +0.0 in fp64 (bit-identical
+ *      whatever the batch split); normalized = fp > 0 ? cum / fp : 0; then every cell where g is NaN or
+ *      -9999 is -9999 in every returned map.
+ *   cum (and fp, normalized when flow_potential): host, nrows x ncols fp64, column-major.
+ *   max_targets: capacity of target_rows, target_cols, amps, scale, iters, relres, fp_iters and
+ *   fp_relres; at least the number of block centres.  *ntargets receives the number of targets; the
+ *   target arrays (0-based rows and columns), amps and scale receive one value per target.
+ *   iters, relres (conductance windows), fp_iters, fp_relres (flow-potential windows): may be NULL.
+ * Each window is solved exactly as one window of cs_b200_solve_advanced_batch.  Batches hold as many
+ * targets as fit max_batch_bytes at the per-window bytes of cs_b200_solve_advanced_batch, both windows of
+ * a target counted (at least one target).
+ * CS_B200_ERR_RESIDUAL / CS_B200_ERR_MAXITER: *first_failed is the target of the first failing window
+ * (targets in order, a target's conductance window before its flow-potential window) and
+ * cs_b200_last_error(NULL) names it and its window kind; every output is still written.
+ * CS_B200_ERR_ARG before any device work: a bad shape, more than INT_MAX landscape or window cells, a
+ * negative radius, an even or < 1 block_size, source_threshold < 0 or NaN, max_targets below the number
+ * of block centres, a NULL g, src, cum, ntargets, target_rows, target_cols, amps or scale, a NULL fp or
+ * normalized with flow_potential, max_batch_bytes <= 0, a bad dtype, rtol or itmax.                   */
+int cs_b200_solve_omniscape(int64_t nrows, int64_t ncols, const void* g, const void* src, int dtype,
+                            int64_t radius, int64_t block_size, double source_threshold, int flow_potential,
+                            int four_neighbors, int device, double rtol, int64_t itmax, int64_t max_batch_bytes,
+                            double* cum, double* fp, double* normalized, int64_t max_targets, int64_t* ntargets,
+                            int64_t* target_rows, int64_t* target_cols, double* amps, double* scale,
+                            int64_t* iters, double* relres, int64_t* fp_iters, double* fp_relres,
+                            int64_t* first_failed);
+
 /* Cumulative / max node-current vectors (n values of dtype each; either may be
  * NULL).  max is initialised to -9999 like src/utils.jl:124.                        */
 int cs_b200_read_currents(cs_b200_handle* h, void* cum, void* max);
